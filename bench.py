@@ -1,6 +1,7 @@
-"""bench.py -- real-time factor of the stem-separation hot path (BASELINE.json metric) on N B200s, or the CPU reference arm.
+"""bench.py -- real-time factor of the stem-separation hot path (BASELINE.json metric) on N H100s, or the CPU reference arm.
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--workload mdx|htdemucs_ft|mdx23c|vr] [--also htdemucs_ft|none]
+                  [--dump-outputs DIR]
 
 Workloads (BASELINE.json configs; there are no model files offline, so every network runs seeded synthetic weights of the released
 geometry -- data: "synthetic"):
@@ -15,6 +16,8 @@ One step = separate the whole workload.
   e2e   : the same through the plugin-level entry point with HOST buffers: pinned input uploaded and stems downloaded inside the timed region
   parity: N > 1 -- the sharded result against a single-GPU run of the same engine on rank 0 (bit-identical expected);
           N = 1 -- the tensor-core path against the fp32 SIMT path of the same library on a 10-s excerpt (gate 1e-4).
+--dump-outputs DIR: after the timed steps, the arrays the timed path returned in its last step as DIR/<workload>_<i>.npy (float32), 64 MB in all;
+         a larger output is sampled at fixed seeded positions.  Inputs are seeded, so two builds can be compared output for output.
 N > 1  : one process per GPU (torchrun); chunks / segments of the ONE track are time-sharded with an overlap-region halo exchange over NCCL
          (strong scaling), audio_separator/separator/b200/sharded.py; the VR batch distributes whole tracks (no collective).
 --impl reference: the reference's algorithm on the host CPU (torch-CPU restatement in oracle/; the reference package itself cannot be installed
@@ -44,23 +47,11 @@ def load_peaks():
         with open(p) as f:
             d = json.load(f)
         return {"hbm_gbs": d.get("hbm_gbs", 6650.0), "bf16_tflops": d.get("bf16_tflops_sustained", d.get("bf16_tflops", 1590.0)), "source": "measured (MEASURED_PEAKS.json, sustained bf16 / copy)"}
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1400.0, "source": "fallback (B200_PROFILING.md)"}
-
-
-def ncu_traffic(kernel_key):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of the dominant kernel, parsed from the committed `ncu --set full` capture of the
-    same launch shape (profiles/ncu_dram_bytes.json: {key: {"bytes": ..., "source": file}}); None when no capture of this build is committed."""
-    p = os.path.join(ROOT, "profiles", "ncu_dram_bytes.json")
-    try:
-        with open(p) as f:
-            e = json.load(f).get(kernel_key)
-        return (float(e["bytes"]), e.get("source")) if e else (None, None)
-    except Exception:
-        return None, None
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "source": "NVIDIA H100 SXM data sheet (HBM3, dense bf16 at 700 W; not a measured rate)"}
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     Q = "clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
 
@@ -158,7 +149,8 @@ class Ctx:
         return t
 
     def timed(self, fn, steps, warmup):
-        """`warmup` untimed + exactly `steps` timed calls, barrier + synchronize on both sides, CUDA events, max over ranks -> ms per step."""
+        """`warmup` untimed + exactly `steps` timed calls, barrier + synchronize on both sides, CUDA events, max over ranks -> ms per step.
+        What the last timed call returned is kept in self.last_out."""
         torch = self.torch
         for _ in range(warmup):
             fn()
@@ -167,7 +159,7 @@ class Ctx:
         self.barrier()
         e0.record()
         for _ in range(steps):
-            fn()
+            self.last_out = fn()
         e1.record()
         self.barrier()
         return self.max_over_ranks(e0.elapsed_time(e1))[0] / steps
@@ -262,11 +254,10 @@ class MdxWorkload:
         tname, tv = ("conv3x3_scale0", prof["conv3x3_scale0"]) if prof.get("conv3x3_scale0", {}).get("ms", 0) > 0 else max(prof.items(), key=lambda kv: kv[1]["ms"])
         tf = tv["flops"] / (tv["ms"] * 1e-3) / 1e12 if tv["ms"] > 0 else 0.0
         kname = f"umma_conv3_kernel<48>[{tname}]" if a.precision else f"conv2d_simt_kernel[{tname}]"
-        traffic, tsrc = ncu_traffic(f"{tname}_b{a.batch}_p{a.precision}")
         return {
-            "kernel": kname, "bound": "tensor", "achieved": tf, "peak": peaks["bf16_tflops"], "unit": "TFLOP/s", "frac": tf / peaks["bf16_tflops"], "traffic": traffic,
-            "traffic_source": tsrc, "peak_source": peaks["source"],
-            "arithmetic": "bf16x3 split (3 tcgen05 MMAs per algorithmic MAC): attainable = peak/3" if a.precision else "fp32 FMA (no tensor cores)",
+            "kernel": kname, "bound": "tensor", "achieved": tf, "peak": peaks["bf16_tflops"], "unit": "TFLOP/s", "frac": tf / peaks["bf16_tflops"], "traffic": None,
+            "peak_source": peaks["source"],
+            "arithmetic": "bf16x3 split (3 wgmma products per algorithmic MAC): attainable = peak/3" if a.precision else "fp32 FMA (no tensor cores)",
             "frac_of_attainable": (3.0 if a.precision else 1.0) * tf / peaks["bf16_tflops"],
             "launches": tv["launches"], "avg_launch_ms": tv["ms"] / max(1, tv["launches"]),
             "algorithmic_flops_per_launch": tv["flops"] / max(1, tv["launches"]), "algorithmic_bytes_per_launch": tv["bytes"] / max(1, tv["launches"]),
@@ -304,7 +295,7 @@ class MdxWorkload:
         p, s = self.plugin.separate_host(self.mix_host)
         full = self.step_device()
         same = bool(torch.equal(torch.from_numpy(p).cuda(), full[0]) and torch.equal(torch.from_numpy(s).cuda(), full[1]))
-        return {"kind": "tcgen05 bf16x3 path vs the fp32 SIMT path of the same library, 10-s excerpt (3 chunks, full-size net), both stems; the oracle comparison is tests/test_mdx_gpu.py",
+        return {"kind": "wgmma bf16x3 path vs the fp32 SIMT path of the same library, 10-s excerpt (3 chunks, full-size net), both stems; the oracle comparison is tests/test_mdx_gpu.py",
                 "max_abs_diff": diff, "gate": 1e-4, "e2e_equals_device_resident": same}
 
     # ---- CPU arm: chunks [3i, 3i+3) of the SAME 68-chunk grid per step (run_model + window + accumulate, as the reference's demix loop does)
@@ -392,7 +383,7 @@ class DemucsWorkload:
                 "achieved": tf, "peak": peaks["bf16_tflops"], "unit": "TFLOP/s", "frac": tf / peaks["bf16_tflops"], "traffic": None, "peak_source": peaks["source"],
                 "arithmetic": "bf16x3 split inside the GEMM / conv kernels: attainable = peak/3", "frac_of_attainable": 3.0 * tf / peaks["bf16_tflops"],
                 "forwards_per_step": self.n_forwards, "algorithmic_flops_per_forward": self.FLOPS_PER_FORWARD, "per_gpu": True,
-                "note": "whole-forward figure (algorithmic flops of all forwards / step time / GPUs); per-kernel launch list: profiles/r02_htdemucs_launches_b4.txt"}
+                "note": "whole-forward figure (algorithmic flops of all forwards / step time / GPUs)"}
 
     def parity(self):
         ctx, torch = self.ctx, self.ctx.torch
@@ -553,10 +544,12 @@ class VrWorkload:
         self.patches = None
 
     def step_device(self):
+        out = []
         for d in self.dev:
             spec = self.eng.loading_mix(d)
             y, v = self.eng.inference(spec)
-            self.eng.spec_to_wav(y), self.eng.spec_to_wav(v)
+            out.append((self.eng.spec_to_wav(y), self.eng.spec_to_wav(v)))
+        return out
 
     def step_e2e(self):
         h2d = d2h = 0
@@ -652,7 +645,37 @@ def run_reference(args):
     print(json.dumps(line), flush=True)
 
 
-def measure(wl, ctx, args, steps, warmup, with_cpu):
+def _arrays(out):
+    """The arrays in a step's return value (tensors / numpy arrays, nested in tuples and lists), in order."""
+    import numpy as np
+
+    if isinstance(out, (list, tuple)):
+        return [a for o in out for a in _arrays(o)]
+    if out is None:
+        return []
+    return [out if isinstance(out, np.ndarray) else out.detach()]
+
+
+def dump_outputs(out, directory, prefix, budget_bytes):
+    """Writes the arrays of `out` as <directory>/<prefix>_<i>.npy in float32.  An array larger than its share of `budget_bytes` is reduced to that many
+    elements taken at sorted positions drawn with a fixed seed, so the same arguments always select the same elements."""
+    import numpy as np
+    import torch
+
+    arrays = _arrays(out)
+    if not arrays:
+        return
+    os.makedirs(directory, exist_ok=True)
+    cap = max(1, budget_bytes // 4 // len(arrays))
+    for i, a in enumerate(arrays):
+        flat = torch.as_tensor(a).reshape(-1)
+        if flat.numel() > cap:
+            idx = np.sort(np.random.default_rng(1000 + i).choice(flat.numel(), cap, replace=False))
+            flat = flat[torch.from_numpy(idx).to(flat.device)]
+        np.save(os.path.join(directory, f"{prefix}_{i}.npy"), flat.float().cpu().numpy())
+
+
+def measure(wl, ctx, args, steps, warmup, with_cpu, dump_budget=0):
     """One workload on this rank set -> the JSON line (rank 0) or None."""
     from audio_separator.separator.b200 import _lib
 
@@ -668,6 +691,9 @@ def measure(wl, ctx, args, steps, warmup, with_cpu):
     ms_step = ctx.timed(wl.step_device, steps, 0)
     launches = ctx.sum_over_ranks(_lib.launch_count() - launches0)[0]
     clocks = sampler.summary() if ctx.rank == 0 else None
+    if args.dump_outputs and ctx.rank == 0:
+        dump_outputs(ctx.last_out, args.dump_outputs, wl.name, dump_budget)
+    ctx.last_out = None
     ms_e2e = ctx.timed(wl.step_e2e, steps, 1)
     h2d, d2h = ctx.sum_over_ranks(wl.h2d, wl.d2h)
     peaks = load_peaks()
@@ -703,6 +729,7 @@ def main():
     ap.add_argument("--precision", type=int, default=1)
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-parity", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None, help="write what the timed path computed in its last step to DIR/<workload>_<i>.npy (64 MB in all)")
     args = ap.parse_args()
     if args.batch is None:
         args.batch = 8 if args.gpus == 1 else min(12, -(-68 // args.gpus))  # 8 chunks per forward measured 2 % faster than 4 on one box (1242 vs 1215)
@@ -711,8 +738,10 @@ def main():
         return run_reference(args)
     ctx = Ctx(args)
     warmup = max(args.warmup, 3)
-    line = measure(WORKLOADS[args.workload](args), ctx, args, args.steps, warmup, with_cpu=not args.no_cpu_baseline)
-    if args.workload == "mdx" and args.also in WORKLOADS and args.also != "mdx":
+    also = args.workload == "mdx" and args.also in WORKLOADS and args.also != "mdx"
+    dump_budget = (60 << 20) // (2 if also else 1)  # array data; the .npy headers stay inside 64 MB
+    line = measure(WORKLOADS[args.workload](args), ctx, args, args.steps, warmup, with_cpu=not args.no_cpu_baseline, dump_budget=dump_budget)
+    if also:
         import gc
         import signal
 
@@ -729,7 +758,7 @@ def main():
         gc.collect()
         ctx.torch.cuda.empty_cache()
         try:
-            extra = measure(WORKLOADS[args.also](args), ctx, args, min(args.steps, 2), 3, with_cpu=not args.no_cpu_baseline)
+            extra = measure(WORKLOADS[args.also](args), ctx, args, args.steps, 3, with_cpu=not args.no_cpu_baseline, dump_budget=dump_budget)
         except Exception as e:  # noqa: BLE001
             import traceback
 

@@ -1,5 +1,5 @@
 /*
- * b200sep.h -- C ABI of the B200-native stem-separation hot path (libb200sep.so, sm_100a only).
+ * b200sep.h -- C ABI of the H100-native stem-separation hot path (libb200sep.so, sm_90a only).
  *
  * The reference (nomadkaraoke/python-audio-separator v0.44.1) is pure Python; its hot path calls into
  * third-party wheels (ATen FFT/conv, onnxruntime).  This header is the FFI a maintainer would bind in place
@@ -138,7 +138,7 @@ typedef struct {
   int32_t k;          /* 3 */
   int32_t bn;         /* 8 TDF bottleneck factor */
   int32_t max_batch;  /* chunks per forward the workspace is sized for */
-  int32_t precision;  /* 0 = fp32 SIMT everywhere; 1 = bf16x3 split tcgen05 where profitable */
+  int32_t precision;  /* 0 = fp32 SIMT everywhere; 1 = bf16x3 split wgmma where profitable */
 } b200sep_mdxnet_config;
 
 /* number of float parameters expected in `params_host` for this config */
@@ -259,13 +259,13 @@ int b200sep_gemm_f32(const float* A, const float* Bw, float* C, int M, int N, in
                      int64_t strideB, int64_t strideC, float alpha, const float* bias_n, const float* bias_m, int act, const float* res,
                      const float* res_scale, const void* w_packed, void* stream);
 /* Large conv2d_f32 / gemm_f32 calls run on the tensor cores (csrc/tc_f32.cu: fp32 operands split in-kernel into bf16 hi + lo, three
- * tcgen05 products, fp32 accumulation).  For STATIC B operands (weights) the split can be done once: w_packed (nullable) is the image
+ * wgmma products, fp32 accumulation).  For STATIC B operands (weights) the split can be done once: w_packed (nullable) is the image
  * tc_pack_*_weights writes into a buffer of b200sep_tc_packed_floats(N, K) floats, K = the GEMM K (linear) or ceil8(Cin)*KH*KW (conv). */
 int64_t b200sep_tc_packed_floats(int N, int K);
 int b200sep_tc_pack_linear_weights(const float* W, int N, int K, int ldw, float* packed, void* stream);
 int b200sep_tc_pack_conv_weights(const float* w_blocked, int Cin, int taps, int Cout, float* packed, void* stream);
 /* Fused attention, head dimension 64: out[b, m, h*64 + d] = sum_n softmax_n(alpha <q[b, m, h], k[b, n, h]>) v[b, n, h*64 + d] with the scores kept on chip
- * (one tcgen05 kernel: Q K^T into TMEM, running softmax in registers, P V from shared memory).  q (B, Lq, .) / k (B, Lk, .) / out (B, Lq, .): batch and row
+ * (one wgmma kernel: Q K^T into registers, running softmax on the fragments, P V with P as the register operand).  q (B, Lq, .) / k (B, Lk, .) / out (B, Lq, .): batch and row
  * strides in floats, head h at columns [h*64, h*64 + 64);  v_is_kn = 0: vt = V TRANSPOSED, vt[b * vt_batch_stride + (h*64 + d) * vt_row_stride + n] (keys
  * contiguous);  v_is_kn = 1: plain V, vt[b * vt_batch_stride + n * vt_row_stride + h*64 + d].
  * Replaces gemm_f32 (scores) + softmax_rows_f32 + gemm_f32 (P V) of nn.MultiheadAttention (transformer.py:196-409). */
@@ -412,7 +412,7 @@ int b200sep_ensemble_spec_abs(const float* planes, int n_models, int64_t plane_e
 
 /* ---------------------------------------------------------------------------------------------------
  * Self-tests of the tensor-core ("bf16x3 pair") operators in isolation: fp32 device tensors in, the operator runs
- * exactly as inside the network (split into bf16 hi/lo planes -> tcgen05 kernel -> join), fp32 out.  Synchronous.
+ * exactly as inside the network (split into bf16 hi/lo planes -> wgmma kernel -> join), fp32 out.  Synchronous.
  *   gemm   : out[M][N] = act((a[M][K] @ w[N][K]^T) * scale[c] + shift[c]) (+ res),  c = (row / rows_per_channel) % channels
  *   conv3x3: out(B,Cout,T,F) = act(conv2d(x(B,Cin,T,F), w(Cout,Cin,3,3), padding=1) * scale[co] + shift[co]);  w is a HOST pointer
  */

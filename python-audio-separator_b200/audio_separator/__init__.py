@@ -1,1 +1,1 @@
-"""Drop-in `audio_separator` package whose separation hot path runs on the B200-native engine (libb200sep.so)."""
+"""Drop-in `audio_separator` package whose separation hot path runs on the H100-native engine (libb200sep.so)."""

@@ -1,4 +1,4 @@
-"""B200 Demucs architecture plugin (HTDemucs v4 models and bags: htdemucs, htdemucs_ft, ...; Hybrid Demucs v3: hdemucs_mmi, mdx_extra, ...).
+"""H100 Demucs architecture plugin (HTDemucs v4 models and bags: htdemucs, htdemucs_ft, ...; Hybrid Demucs v3: hdemucs_mmi, mdx_extra, ...).
 
 Plugin contract of the reference's DemucsSeparator (audio_separator/separator/architectures/demucs_separator.py:26-195):
 ctor `(common_config, arch_config)` with arch keys segment_size / shifts / overlap / segments_enabled,
@@ -30,9 +30,9 @@ class DemucsSeparator(CommonSeparator):
         self.shifts = arch_config.get("shifts", 2)
         self.overlap = arch_config.get("overlap", 0.25)
         self.segments_enabled = arch_config.get("segments_enabled", True)
-        self.batch_size = int(arch_config.get("batch_size", 4))  # segments per forward (B200 addition; results do not depend on it)
+        self.batch_size = int(arch_config.get("batch_size", 4))  # segments per forward (H100 addition; results do not depend on it)
         if not torch.cuda.is_available():
-            raise RuntimeError("DemucsSeparator (B200 build) needs a CUDA device: there is no CPU path in this package")
+            raise RuntimeError("DemucsSeparator (H100 build) needs a CUDA device: there is no CPU path in this package")
         self.torch_device = torch.device("cuda", torch.cuda.current_device())
         self.demucs_source_map = DEMUCS_4_SOURCE_MAPPER
         self.load_model()

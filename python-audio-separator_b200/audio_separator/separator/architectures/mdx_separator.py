@@ -1,4 +1,4 @@
-"""B200 MDX architecture plugin.
+"""H100 MDX architecture plugin.
 
 Same plugin contract as the reference's MDXSeparator (audio_separator/separator/architectures/mdx_separator.py):
 ctor `(common_config, arch_config)`, `separate(path, custom_output_names) -> [filenames]`, `demix`, `run_model`,
@@ -36,7 +36,7 @@ class MDXSeparator(CommonSeparator):
         self.config_yaml = self.model_data.get("config_yaml", None)
 
         if not torch.cuda.is_available():
-            raise RuntimeError("MDXSeparator (B200 build) needs a CUDA device: there is no onnxruntime / CPU path in this package")
+            raise RuntimeError("MDXSeparator (H100 build) needs a CUDA device: there is no onnxruntime / CPU path in this package")
         self.torch_device = torch.device("cuda", torch.cuda.current_device())
         self.n_bins = self.trim = self.chunk_size = self.gen_size = 0
         self._host_bufs = {}

@@ -1,4 +1,4 @@
-"""B200 MDXC architecture plugin (non-Roformer TFC_TDF_net models, e.g. MDX23C-8KFFT-InstVoc_HQ).
+"""H100 MDXC architecture plugin (non-Roformer TFC_TDF_net models, e.g. MDX23C-8KFFT-InstVoc_HQ).
 
 Plugin contract of the reference's MDXCSeparator (audio_separator/separator/architectures/mdxc_separator.py:19-228):
 ctor `(common_config, arch_config)` with arch keys segment_size / override_model_segment_size / batch_size / overlap /
@@ -30,7 +30,7 @@ class MDXCSeparator(CommonSeparator):
         if self.pitch_shift:
             raise NotImplementedError("pitch_shift is not part of the accelerated path")
         if not torch.cuda.is_available():
-            raise RuntimeError("MDXCSeparator (B200 build) needs a CUDA device: there is no CPU path in this package")
+            raise RuntimeError("MDXCSeparator (H100 build) needs a CUDA device: there is no CPU path in this package")
         self.torch_device = torch.device("cuda", torch.cuda.current_device())
         self.is_primary_stem_main_target = bool(self.model_data_cfgdict["training"].get("target_instrument"))  # :69, both model families
         self._engines = {}  # dim_t -> engine: the chunk length is fixed per engine, and separate() switches it for clips shorter than 10 s (:137-143)
@@ -43,7 +43,7 @@ class MDXCSeparator(CommonSeparator):
         if self.is_roformer:
             return self._load_roformer(cfg)
         if model.get("norm") != "InstanceNorm" or model.get("act", "gelu") != "gelu" or list(model.get("scale", [2, 2])) != [2, 2]:
-            raise ValueError("the B200 TFC_TDF_net supports norm=InstanceNorm, act=gelu, scale=[2,2] (the MDX23C configuration)")
+            raise ValueError("the H100 TFC_TDF_net supports norm=InstanceNorm, act=gelu, scale=[2,2] (the MDX23C configuration)")
         path = self.model_path
         if path.lower().endswith(".npz"):
             with np.load(path) as z:

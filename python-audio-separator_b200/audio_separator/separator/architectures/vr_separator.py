@@ -1,4 +1,4 @@
-"""B200 VR architecture plugin (CascadedASPPNet models -- the HP / HP2 / SP "VR arch" v4-v5.0 checkpoints -- and VR 5.1 CascadedNet models).
+"""H100 VR architecture plugin (CascadedASPPNet models -- the HP / HP2 / SP "VR arch" v4-v5.0 checkpoints -- and VR 5.1 CascadedNet models).
 
 Plugin contract of the reference's VRSeparator (audio_separator/separator/architectures/vr_separator.py:26-253): ctor
 `(common_config, arch_config)` with arch keys batch_size / window_size / aggression / enable_tta / enable_post_process /
@@ -34,7 +34,7 @@ class VRSeparator(CommonSeparator):
         self.aggression_setting = int(arch_config.get("aggression", 5))
         self.aggression = float(self.aggression_setting / 100)
         if not torch.cuda.is_available():
-            raise RuntimeError("VRSeparator (B200 build) needs a CUDA device: there is no CPU path in this package")
+            raise RuntimeError("VRSeparator (H100 build) needs a CUDA device: there is no CPU path in this package")
         self.torch_device = torch.device("cuda", torch.cuda.current_device())
         self.model_samplerate = self.model_params["sr"]
         if self.model_samplerate != 44100:

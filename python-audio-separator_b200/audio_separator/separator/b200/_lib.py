@@ -12,7 +12,7 @@ LIB_PATH = os.environ.get("B200SEP_LIB", os.path.join(_PKG_ROOT, "libb200sep.so"
 if not os.path.exists(LIB_PATH):
     raise ImportError(
         f"libb200sep.so not found at {LIB_PATH}: build it with `python python-audio-separator_b200/build.py` "
-        "(the B200 engine has no CPU / PyTorch fallback)"
+        "(the engine has no CPU / PyTorch fallback)"
     )
 lib = C.CDLL(LIB_PATH)
 

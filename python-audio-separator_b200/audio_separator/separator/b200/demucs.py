@@ -61,11 +61,11 @@ class HTDemucsConfig:
 
     def validate(self):
         if self.audio_channels != 2:
-            raise ValueError("the B200 HTDemucs path handles stereo models only")
+            raise ValueError("the H100 HTDemucs path handles stereo models only")
         if self.kernel_size != 8 or self.stride != 4 or self.context != 1:
-            raise ValueError("the B200 HTDemucs path needs kernel_size 8, stride 4, context 1 (the released htdemucs geometry)")
+            raise ValueError("the H100 HTDemucs path needs kernel_size 8, stride 4, context 1 (the released htdemucs geometry)")
         if self.dconv_depth != 2:
-            raise ValueError("the B200 HTDemucs path needs dconv_depth 2 (dilations 1 and 2)")
+            raise ValueError("the H100 HTDemucs path needs dconv_depth 2 (dilations 1 and 2)")
         if self.nfft // 2 != self.stride**self.depth * (self.nfft // 2 // self.stride**self.depth):
             raise ValueError("nfft/2 must be divisible by stride**depth")
 

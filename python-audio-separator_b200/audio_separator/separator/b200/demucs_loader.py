@@ -18,7 +18,7 @@ import yaml
 from .demucs import HTDemucsConfig
 from .hdemucs import HDemucsConfig
 
-# constructor arguments that must keep the value the B200 graph was built for (htdemucs.py:36-98)
+# constructor arguments that must keep the value the H100 graph was built for (htdemucs.py:36-98)
 _REQUIRED = dict(cac=True, wiener_iters=0, end_iters=0, wiener_residual=False, rewrite=True, multi_freqs=None, context_enc=0, t_emb="sin", t_norm_in=True,
                  t_norm_in_group=False, t_group_norm=False, t_norm_first=True, t_norm_out=True, t_layer_scale=True, t_gelu=True, t_weight_pos_embed=1.0,
                  t_sparse_self_attn=False, t_sparse_cross_attn=False, t_cross_first=False, channels_time=None, use_train_segment=True)
@@ -26,7 +26,7 @@ _MAPPED = ("sources", "audio_channels", "channels", "growth", "nfft", "depth", "
            "t_layers", "t_heads", "t_hidden_scale", "freq_emb", "emb_scale", "samplerate", "segment")
 
 
-# HDemucs (v3) constructor arguments (hdemucs.py:360-400): values the B200 graph is built for, and the ones that map onto HDemucsConfig
+# HDemucs (v3) constructor arguments (hdemucs.py:360-400): values the H100 graph is built for, and the ones that map onto HDemucsConfig
 _HD_REQUIRED = dict(cac=True, wiener_iters=0, end_iters=0, wiener_residual=False, rewrite=True, hybrid=True, channels_time=None)
 _HD_MAPPED = ("sources", "audio_channels", "channels", "growth", "nfft", "depth", "hybrid_old", "freq_emb", "emb_scale", "kernel_size", "time_stride", "stride", "context",
               "context_enc", "norm_starts", "norm_groups", "dconv_mode", "dconv_depth", "dconv_comp", "dconv_attn", "dconv_lstm", "samplerate", "segment")
@@ -83,7 +83,7 @@ def config_from_package(package: dict):
     klass = package["klass"]
     name = getattr(klass, "__name__", str(klass))
     if name not in ("HTDemucs", "HDemucs"):
-        raise NotImplementedError(f"model class {name}: the B200 Demucs path covers HTDemucs (v4) and HDemucs (v3 hybrid) packages; Demucs v1 / v2 time-domain models are not built")
+        raise NotImplementedError(f"model class {name}: the H100 Demucs path covers HTDemucs (v4) and HDemucs (v3 hybrid) packages; Demucs v1 / v2 time-domain models are not built")
     kwargs = dict(package.get("kwargs", {}))
     if package.get("args"):
         raise ValueError("positional constructor arguments in a Demucs package are not supported")

@@ -18,7 +18,7 @@ from ._lib import LAYOUT_CFT, LAYOUT_CTF, check, lib
 
 def _require_cuda():
     if not torch.cuda.is_available():
-        raise RuntimeError("the B200 engine needs a CUDA device (sm_100a); there is no CPU fallback")
+        raise RuntimeError("the H100 engine needs a CUDA device (sm_90a); there is no CPU fallback")
 
 
 def _ptr(t: torch.Tensor) -> int:

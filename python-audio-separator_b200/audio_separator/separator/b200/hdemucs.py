@@ -65,11 +65,11 @@ class HDemucsConfig:
 
     def validate(self):
         if self.audio_channels != 2:
-            raise ValueError("the B200 HDemucs path handles stereo models only")
+            raise ValueError("the H100 HDemucs path handles stereo models only")
         if self.kernel_size != 2 * self.stride:
-            raise ValueError("the B200 HDemucs path needs kernel_size == 2 * stride (the transposed convolutions are 2-tap over the coarse index)")
+            raise ValueError("the H100 HDemucs path needs kernel_size == 2 * stride (the transposed convolutions are 2-tap over the coarse index)")
         if self.dconv_depth != 2:
-            raise ValueError("the B200 HDemucs path needs dconv_depth 2 (dilations 1 and 2)")
+            raise ValueError("the H100 HDemucs path needs dconv_depth 2 (dilations 1 and 2)")
 
 
 def layer_plan(cfg: HDemucsConfig):

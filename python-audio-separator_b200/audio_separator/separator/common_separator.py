@@ -1,4 +1,4 @@
-"""Base class contract shared by the B200 architecture plugins.
+"""Base class contract shared by the H100 architecture plugins.
 
 Mirrors what `Separator` and the plugins rely on from the reference's CommonSeparator
 (audio_separator/separator/common_separator.py:57-157 config/stem naming, :217-282 prepare_mix,

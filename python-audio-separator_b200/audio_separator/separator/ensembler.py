@@ -1,4 +1,4 @@
-"""B200 mirror of the reference's Ensembler (audio_separator/separator/ensembler.py): same constructor `(logger, algorithm, weights)` and
+"""H100 mirror of the reference's Ensembler (audio_separator/separator/ensembler.py): same constructor `(logger, algorithm, weights)` and
 `ensemble(waveforms) -> ndarray`, the reductions over the model axis (and the 2048 / 1024 STFTs of the *_fft and uvr_* algorithms) run on the GPU.
 `ensemble_wav` (spec_utils.ensemble_wav: a per-channel pick of the quietest model) is a handful of host comparisons and mirrors the numpy semantics."""
 import numpy as np
@@ -74,7 +74,7 @@ class Ensembler:
             n = max(w.shape[1] for w in waveforms)  # zero-padded to the longest first (ensembler.py:27-29)
             return self._ensemble_wav([np.pad(w, ((0, 0), (0, n - w.shape[1]))) if w.shape[1] < n else w for w in waveforms])
         if not torch.cuda.is_available():
-            raise RuntimeError("Ensembler (B200 build) needs a CUDA device: there is no CPU path in this package")
+            raise RuntimeError("Ensembler (H100 build) needs a CUDA device: there is no CPU path in this package")
         num_channels = waveforms[0].shape[0]
         if any(w.shape[0] != num_channels for w in waveforms):
             raise ValueError("All waveforms must have the same number of channels for ensembling.")

@@ -60,7 +60,7 @@ class Separator:
             raise ValueError(f"The sample rate setting is {self.sample_rate} but it must be a non-zero whole number.")
         self.use_soundfile, self.use_autocast = use_soundfile, use_autocast
         if ensemble_preset or chunk_duration:
-            raise NotImplementedError("ensemble presets (ensemble_presets.json) / file-level chunking are outside the B200 hot-path scope; pass the model list and algorithm explicitly")
+            raise NotImplementedError("ensemble presets (ensemble_presets.json) / file-level chunking are outside the H100 hot-path scope; pass the model list and algorithm explicitly")
         self.ensemble_algorithm = ensemble_algorithm or "avg_wave"  # separator.py:237-238
         self.ensemble_weights = ensemble_weights
         self.ensemble_preset = None
@@ -81,9 +81,9 @@ class Separator:
 
     def setup_accelerated_inferencing_device(self):
         if not torch.cuda.is_available():
-            raise RuntimeError("no CUDA device: this build targets B200 (sm_100a) only and has no CPU / MPS / DirectML path")
+            raise RuntimeError("no CUDA device: this build targets H100 (sm_90a) only and has no CPU / MPS / DirectML path")
         self.torch_device = torch.device("cuda", torch.cuda.current_device())
-        self.logger.info(f"B200 engine on {torch.cuda.get_device_name(self.torch_device)}")
+        self.logger.info(f"H100 engine on {torch.cuda.get_device_name(self.torch_device)}")
 
     def load_model_data(self, model_path):
         if model_path.lower().endswith(".th"):  # a single Demucs package carries its own constructor arguments (demucs/states.py:34-64)

@@ -1,7 +1,7 @@
-"""B200 mirror of the reference's `STFT` helper (audio_separator/separator/uvr_lib_v5/stft.py:4-126).
+"""H100 mirror of the reference's `STFT` helper (audio_separator/separator/uvr_lib_v5/stft.py:4-126).
 
 Same constructor, `__call__` and `inverse` contract -- (B, C, T) <-> (B, 2C, dim_f, T//hop+1), planes
-[L_re, L_im, R_re, R_im] -- but both directions are single launches of the hand-written sm_100a FFT kernels
+[L_re, L_im, R_re, R_im] -- but both directions are single launches of the hand-written sm_90a FFT kernels
 (csrc/stft.cu) instead of torch.stft / torch.istft.  CUDA tensors in, CUDA tensors out; anything else raises.
 """
 import torch
@@ -18,7 +18,7 @@ class STFT:
         if not isinstance(t, torch.Tensor):
             raise TypeError("STFT expects a torch.Tensor")
         if not t.is_cuda:
-            raise RuntimeError("the B200 STFT only runs on CUDA tensors (no CPU fallback); move the input to the GPU")
+            raise RuntimeError("the H100 STFT only runs on CUDA tensors (no CPU fallback); move the input to the GPU")
         return t.to(torch.float32)
 
     def __call__(self, input_tensor):

@@ -1,4 +1,4 @@
-"""Build libb200sep.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Build libb200sep.so in-tree with nvcc for sm_90a (cross-compiles without a GPU).
 
     python python-audio-separator_b200/build.py [--force]
 """
@@ -11,7 +11,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libb200sep.so")
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "-shared", "-lcuda", "--threads", "0",
 ]
 

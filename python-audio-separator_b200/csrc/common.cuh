@@ -1,4 +1,4 @@
-// Shared helpers for libb200sep (sm_100a).  Error plumbing, launch accounting, small device utilities.
+// Shared helpers for libb200sep (sm_90a).  Error plumbing, launch accounting, small device utilities.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -43,6 +43,6 @@ void count_launch(int n = 1);
 
 static inline int cdiv(int64_t a, int64_t b) { return (int)((a + b - 1) / b); }
 
-constexpr int kNumSMs = 148;  // B200
+constexpr int kNumSMs = 132;  // H100 SXM
 
 }  // namespace b200sep

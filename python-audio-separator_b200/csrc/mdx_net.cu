@@ -133,7 +133,7 @@ static int upload_u16(b200sep_mdxnet* net, void** dst, const std::vector<uint16_
   return B200SEP_OK;
 }
 
-// tcgen05 B operand of a 3x3 conv (see umma_conv_block_weights)
+// wgmma B operand of a 3x3 conv (see umma_conv_block_weights)
 static int make_conv_umma(b200sep_mdxnet* net, ConvW& cw, const float* w /*(Cout,Cin,3,3)*/) {
   umma_conv_choose(cw.cin, cw.n, &cw.kc, &cw.n_tile);
   std::vector<uint16_t> hi, lo;

@@ -1,4 +1,4 @@
-// STFT / iSTFT / overlap-add kernels (sm_100a).  Not cuFFT: one CTA transforms one stereo frame as a single
+// STFT / iSTFT / overlap-add kernels (sm_90a).  Not cuFFT: one CTA transforms one stereo frame as a single
 // complex FFT (z = L + iR) with shared-memory Stockham autosort stages of radix 8/4/2/3/5, the two real
 // spectra are separated in the epilogue, which also applies the dim_f crop, the low-bin zeroing and the
 // complex-as-channels plane split of the reference (uvr_lib_v5/stft.py:20-56).  These kernels are HBM/latency

@@ -1,17 +1,16 @@
-// fp32-in / fp32-out GEMM and implicit-GEMM convolution on the 5th-generation tensor cores (tcgen05, sm_100a).
+// fp32-in / fp32-out GEMM and implicit-GEMM convolution on the Hopper tensor cores (wgmma, sm_90a).
 //
 // The operands stay plain fp32 tensors in HBM (any strides, batched).  Producer warps read them, split every value on the fly into a
 // bf16 "hi" and a bf16 "lo" part (x ~= hi + lo, 16 mantissa bits) and write both into shared memory in the canonical K-major
-// SWIZZLE_128B layout; one elected thread then issues, per 64-wide k-block, the three products  Ah*Bh + Ah*Bl + Al*Bh  as
-// tcgen05.mma.kind::f16 instructions accumulating in fp32 in TMEM (relative error ~1e-5 per contraction, see DESIGN.md); eight
-// epilogue warps drain the accumulator (tcgen05.ld), apply bias / activation / residual and store fp32.
+// SWIZZLE_128B layout; two consumer warpgroups (64 rows of the 128-row tile each) then issue, per 64-wide k-block, the three products
+// Ah*Bh + Ah*Bl + Al*Bh as wgmma instructions accumulating in fp32 registers (relative error ~1e-5 per contraction, see DESIGN.md) and
+// apply bias / activation / residual to their accumulator fragments before storing fp32.
 //
-//   warp 0        : MMA issuer (lane 0) + TMEM allocation
-//   warps 1..8    : producers: global fp32 -> registers -> split -> swizzled st.shared -> fence.proxy.async -> mbarrier arrive
-//   warps 9..16   : epilogue; warp w owns TMEM lanes 32*(w%4).., the two warps of a lane quadrant split the columns
+//   warps 0..7    : consumers (wgmma issue + epilogue)
+//   warps 8..15   : producers: global fp32 -> registers -> split -> swizzled st.shared -> fence.proxy.async -> mbarrier arrive
 //
-// Persistent CTAs (one per SM) walk the (batch, m-tile, n-tile) list; the shared-memory ring (full/empty mbarriers) and the two TMEM
-// accumulators (tmem_full/tmem_empty) run continuously across tiles, so the epilogue of tile i overlaps the main loop of tile i+1.
+// Persistent CTAs (one per SM) walk the (batch, m-tile, n-tile) list; the shared-memory ring (full/empty mbarriers) runs continuously
+// across tiles, so the producers fill the next tile's stages while the consumers run an epilogue.
 //
 // Used by b200sep_gemm_f32 (nn.Linear / attention of the HTDemucs cross-transformer) and b200sep_conv2d_f32 (Demucs encoders /
 // DConv / rewrite convolutions, the VR CascadedASPPNet convolutions) when the shape is large enough; the SIMT kernels in ops_f32.cu /
@@ -29,10 +28,11 @@ namespace b200sep {
 
 namespace {
 
-constexpr int kTM = 128, kTK = 64;
-constexpr int kProducerWarps = 8, kEpilogueWarps = 8;
-constexpr int kThreads = 32 * (1 + kProducerWarps + kEpilogueWarps);  // 544
+constexpr int kTM = 128, kTN = 128, kTK = 64;
+constexpr int kProducerWarps = 8;
+constexpr int kConsThreads = 256;  // two consumer warpgroups
 constexpr int kProdThreads = 32 * kProducerWarps;
+constexpr int kThreads = kConsThreads + kProdThreads;  // 512
 
 struct TcParams {
   // A operand (M rows): mode 0 GEMM  a[z*a_sz + m*a_rs + k]  (k contiguous);  mode 1 convolution gather (see below)
@@ -42,7 +42,7 @@ struct TcParams {
   const float* b;
   int64_t b_sz, b_rs, b_ks;
   int M, N, K, batch;
-  int n_tile, stages, tmem_cols;
+  int n_tile, stages;
   int m_tiles, n_tiles, num_tiles, num_iters;
   uint32_t a_bytes, b_bytes, stage_bytes;
   int a_vec, b_vec;  // 16-byte aligned K-major sources: float4 loads
@@ -196,74 +196,52 @@ __device__ __forceinline__ void fill_conv_weights(uint8_t* hi, uint8_t* lo, cons
   }
 }
 
+// one output element of the generic epilogue: v = acc*alpha + bias_m[m] + bias_n[n] (+ add before act); act; (+ add after act | res + res_scale[n]*v)
+__device__ __forceinline__ void tc_store(const TcParams& p, int z, int m, int n, float v) {
+  if (p.up_axis) {
+    // ConvTranspose as a 2-tap convolution over the coarse index: column n is phase r of real channel co
+    const int r = n / p.up_cout, co = n - r * p.up_cout;
+    const int hq = m / p.Wo, wq = m - hq * p.Wo;
+    const int pos = ((p.up_axis == 1) ? hq : wq) * p.up + r - p.trim;
+    if (pos < 0 || pos >= p.out_len) return;
+    const int64_t cs = (p.up_axis == 1) ? (int64_t)p.out_len * p.Wo : (int64_t)p.Ho * p.out_len;
+    float x = v;
+    if (p.bias_n) x += __ldg(&p.bias_n[co]);
+    p.out[(int64_t)z * p.o_sz + (int64_t)co * cs + ((p.up_axis == 1) ? (int64_t)pos * p.Wo + wq : (int64_t)hq * p.out_len + pos)] = tc_act(x, p.act);
+    return;
+  }
+  float x = fmaf(v, p.alpha, p.bias_m ? __ldg(&p.bias_m[m]) : 0.f);
+  if (p.bias_n) x += __ldg(&p.bias_n[n]);
+  const float* rrow = p.res ? p.res + (int64_t)z * p.r_sz + (int64_t)m * p.r_sm : nullptr;
+  if (rrow && p.add_before_act) x += __ldg(&rrow[(int64_t)n * p.r_sn]);
+  x = tc_act(x, p.act);
+  if (rrow && !p.add_before_act) {
+    if (p.res_scale) x = __ldg(&rrow[(int64_t)n * p.r_sn]) + __ldg(&p.res_scale[n]) * x;
+    else x += __ldg(&rrow[(int64_t)n * p.r_sn]);
+  }
+  p.out[(int64_t)z * p.o_sz + (int64_t)m * p.o_sm + (int64_t)n * p.o_sn] = x;
+}
+
 __global__ void __launch_bounds__(kThreads, 1) tc_f32_kernel(const TcParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (ptx::smem_u32(smem_raw) & 1023u)) & 1023u);
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + (size_t)p.stages * p.stage_bytes);
   uint64_t* empty_bar = full_bar + p.stages;
-  uint64_t* tmem_full_bar = empty_bar + p.stages;  // [2]
-  uint64_t* tmem_empty_bar = tmem_full_bar + 2;    // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_empty_bar + 2);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
     for (int s = 0; s < p.stages; ++s) {
       ptx::mbar_init(&full_bar[s], kProducerWarps + (p.b_packed ? 1 : 0));
-      ptx::mbar_init(&empty_bar[s], 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      ptx::mbar_init(&tmem_full_bar[a], 1);
-      ptx::mbar_init(&tmem_empty_bar[a], kEpilogueWarps);
+      ptx::mbar_init(&empty_bar[s], kConsThreads);
     }
     ptx::fence_barrier_init();
   }
-  if (warp == 0) ptx::tmem_alloc(tmem_slot, (uint32_t)p.tmem_cols);
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t acc_stride = (uint32_t)p.tmem_cols / 2;
   const int tiles_per_z = p.m_tiles * p.n_tiles;
 
-  if (warp == 0) {
-    if (lane == 0) {
-      // ===== MMA issuer =====
-      const uint32_t idesc = ptx::instr_desc_bf16(kTM, p.n_tile, 0, 0);
-      int s = 0, acc = 0;
-      uint32_t phase = 0, acc_phase = 0;
-      for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-        ptx::mbar_wait(&tmem_empty_bar[acc], acc_phase ^ 1, 400 + acc);
-        ptx::tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)acc * acc_stride;
-        for (int i = 0; i < p.num_iters; ++i) {
-          ptx::mbar_wait(&full_bar[s], phase, 200 + i);
-          ptx::tc_fence_after();
-          const uint32_t st = ptx::smem_u32(smem + (size_t)s * p.stage_bytes);
-          const uint32_t a_hi = st, a_lo = st + p.a_bytes, b_hi = st + 2 * p.a_bytes, b_lo = b_hi + p.b_bytes;
-#pragma unroll
-          for (int j = 0; j < kTK / 16; ++j) {
-            const uint64_t dah = ptx::smem_desc(a_hi + j * 32, 16, 1024, ptx::kLayoutSW128);
-            const uint64_t dal = ptx::smem_desc(a_lo + j * 32, 16, 1024, ptx::kLayoutSW128);
-            const uint64_t dbh = ptx::smem_desc(b_hi + j * 32, 16, 1024, ptx::kLayoutSW128);
-            const uint64_t dbl = ptx::smem_desc(b_lo + j * 32, 16, 1024, ptx::kLayoutSW128);
-            ptx::umma_bf16(d_tmem, dah, dbh, idesc, (i | j) != 0 ? 1u : 0u);
-            ptx::umma_bf16(d_tmem, dah, dbl, idesc, 1u);
-            ptx::umma_bf16(d_tmem, dal, dbh, idesc, 1u);
-          }
-          ptx::umma_commit(&empty_bar[s]);
-          if (++s == p.stages) {
-            s = 0;
-            phase ^= 1;
-          }
-        }
-        ptx::umma_commit(&tmem_full_bar[acc]);
-        acc ^= 1;
-        if (acc == 0) acc_phase ^= 1;
-      }
-    }
-  } else if (warp <= kProducerWarps) {
+  if (warp >= kConsThreads / 32) {
     // ===== producers =====
-    const int pt = threadIdx.x - 32;
+    const int pt = threadIdx.x - kConsThreads;
     int s = 0;
     uint32_t phase = 0;
     const int taps = p.KH * p.KW;
@@ -343,146 +321,60 @@ __global__ void __launch_bounds__(kThreads, 1) tc_f32_kernel(const TcParams p) {
         }
       }
     }
-  } else {
-    // ===== epilogue =====
-    const int q = warp & 3;
-    const int half = (warp - 1 - kProducerWarps) >> 2;
-    const int mrow = q * 32 + lane;
-    const int nchunks = p.n_tile / 16;
-    const int ch_begin = half ? nchunks / 2 : 0, ch_end = half ? nchunks : nchunks / 2;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-      const int z = tile / tiles_per_z, rem = tile - z * tiles_per_z;
-      const int m = (rem / p.n_tiles) * kTM + mrow, n0 = (rem % p.n_tiles) * p.n_tile;
-      const bool row_ok = m < p.M;
-      const float bm = (row_ok && p.bias_m) ? __ldg(&p.bias_m[m]) : 0.f;
-      float* orow = p.out + (int64_t)z * p.o_sz + (int64_t)m * p.o_sm;
-      const float* rrow = p.res ? p.res + (int64_t)z * p.r_sz + (int64_t)m * p.r_sm : nullptr;
-      ptx::mbar_wait_opt(&tmem_full_bar[acc], acc_phase, p.sleep_ns, 300 + acc);
-      ptx::tc_fence_after();
-      const uint32_t trow = tmem_base + (uint32_t)acc * acc_stride + ((uint32_t)(q * 32) << 16);
-      for (int ch = ch_begin; ch < ch_end; ++ch) {
-        const int c0 = ch * 16;
-        if (n0 + c0 >= p.N) break;  // warp-uniform
-        uint32_t v[16];
-        ptx::tmem_ld16(trow + (uint32_t)c0, v);
-        ptx::tmem_ld_wait();
-        if (!row_ok) continue;
-        if (p.up_axis) {
-          // ConvTranspose as a 2-tap convolution over the coarse index: this 16-column group is one phase r and 16 consecutive real channels
-          const int nb = n0 + c0;
-          const int r = nb / p.up_cout, co0 = nb - r * p.up_cout;
-          const int hq = m / p.Wo, wq = m - hq * p.Wo;
-          const int pos = ((p.up_axis == 1) ? hq : wq) * p.up + r - p.trim;
-          if (pos < 0 || pos >= p.out_len) continue;
-          const int64_t cs = (p.up_axis == 1) ? (int64_t)p.out_len * p.Wo : (int64_t)p.Ho * p.out_len;
-          float* o = p.out + (int64_t)z * p.o_sz + (int64_t)co0 * cs + ((p.up_axis == 1) ? (int64_t)pos * p.Wo + wq : (int64_t)hq * p.out_len + pos);
-          float x[16];
-#pragma unroll
-          for (int j = 0; j < 16; ++j) x[j] = __uint_as_float(v[j]);
-          if (p.bias_n) {
-#pragma unroll
-            for (int j4 = 0; j4 < 4; ++j4) {
-              const float4 bv = __ldg(reinterpret_cast<const float4*>(p.bias_n + co0) + j4);  // co0 is a multiple of 16
-              x[4 * j4] += bv.x; x[4 * j4 + 1] += bv.y; x[4 * j4 + 2] += bv.z; x[4 * j4 + 3] += bv.w;
-            }
-          }
-          switch (p.act) {
-            case 0: break;
-            case 1:
-#pragma unroll
-              for (int j = 0; j < 16; ++j) x[j] = fmaxf(x[j], 0.f);
-              break;
-            default:
-#pragma unroll
-              for (int j = 0; j < 16; ++j) x[j] = tc_act(x[j], p.act);
-          }
-#pragma unroll
-          for (int j = 0; j < 16; ++j) o[(int64_t)j * cs] = x[j];
-          continue;
-        }
-        // Everything that does not depend on the column is decided OUTSIDE the 16-column loops (the first version re-tested bias / residual /
-        // activation per column: ~25 instructions per output, 48 k warp-instructions per tile, which made K = 64 attention GEMMs epilogue-bound).
-        float x[16];
-        const int nb0 = n0 + c0;
-        const bool full = nb0 + 15 < p.N;
-#pragma unroll
-        for (int j = 0; j < 16; ++j) x[j] = fmaf(__uint_as_float(v[j]), p.alpha, bm);
-        if (p.bias_n) {
-          if (full) {
-#pragma unroll
-            for (int j4 = 0; j4 < 4; ++j4) {
-              const float4 bv = __ldg(reinterpret_cast<const float4*>(p.bias_n + nb0) + j4);  // nb0 is a multiple of 16
-              x[4 * j4] += bv.x; x[4 * j4 + 1] += bv.y; x[4 * j4 + 2] += bv.z; x[4 * j4 + 3] += bv.w;
-            }
-          } else {
-#pragma unroll
-            for (int j = 0; j < 16; ++j)
-              if (nb0 + j < p.N) x[j] += __ldg(&p.bias_n[nb0 + j]);
-          }
-        }
-        if (rrow && p.add_before_act) {
-#pragma unroll
-          for (int j = 0; j < 16; ++j)
-            if (full || nb0 + j < p.N) x[j] += __ldg(&rrow[(int64_t)(nb0 + j) * p.r_sn]);
-        }
-        switch (p.act) {
-          case 1:
-#pragma unroll
-            for (int j = 0; j < 16; ++j) x[j] = fmaxf(x[j], 0.f);
-            break;
-          case 0: break;
-          default:
-#pragma unroll
-            for (int j = 0; j < 16; ++j) x[j] = tc_act(x[j], p.act);
-        }
-        if (rrow && !p.add_before_act) {
-          if (p.res_scale) {
-#pragma unroll
-            for (int j = 0; j < 16; ++j)
-              if (full || nb0 + j < p.N) x[j] = __ldg(&rrow[(int64_t)(nb0 + j) * p.r_sn]) + __ldg(&p.res_scale[nb0 + j]) * x[j];
-          } else if (p.r_sn == 1 && full && ((reinterpret_cast<uintptr_t>(rrow + nb0) & 15) == 0)) {
-#pragma unroll
-            for (int j4 = 0; j4 < 4; ++j4) {
-              const float4 rv = __ldg(reinterpret_cast<const float4*>(rrow + nb0) + j4);
-              x[4 * j4] += rv.x; x[4 * j4 + 1] += rv.y; x[4 * j4 + 2] += rv.z; x[4 * j4 + 3] += rv.w;
-            }
-          } else {
-#pragma unroll
-            for (int j = 0; j < 16; ++j)
-              if (full || nb0 + j < p.N) x[j] += __ldg(&rrow[(int64_t)(nb0 + j) * p.r_sn]);
-          }
-        }
-        const int n = n0 + c0;
-        if (p.o_sn == 1 && n + 15 < p.N && ((reinterpret_cast<uintptr_t>(orow + n) & 15) == 0)) {
-          float4* d = reinterpret_cast<float4*>(orow + n);
-          d[0] = make_float4(x[0], x[1], x[2], x[3]);
-          d[1] = make_float4(x[4], x[5], x[6], x[7]);
-          d[2] = make_float4(x[8], x[9], x[10], x[11]);
-          d[3] = make_float4(x[12], x[13], x[14], x[15]);
-        } else {
-#pragma unroll
-          for (int j = 0; j < 16; ++j)
-            if (n + j < p.N) orow[(int64_t)(n + j) * p.o_sn] = x[j];
-        }
-      }
-      ptx::tc_fence_before();
-      __syncwarp();
-      if (lane == 0) ptx::mbar_arrive(&tmem_empty_bar[acc]);
-      acc ^= 1;
-      if (acc == 0) acc_phase ^= 1;
-    }
+    return;
   }
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    ptx::tc_fence_after();
-    ptx::tmem_dealloc(tmem_base, (uint32_t)p.tmem_cols);
+  // ===== consumers: wgmma main loop into registers, then the epilogue from the accumulator fragments =====
+  const int wg = warp >> 2, g = lane >> 2, cq = lane & 3;
+  const int mrow0 = wg * 64 + (warp & 3) * 16 + g;  // tile rows mrow0 and mrow0 + 8
+  int s = 0;
+  uint32_t phase = 0;
+  float acc[kTN / 2];
+  for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+    const int z = tile / tiles_per_z, rem = tile - z * tiles_per_z;
+    const int m0 = (rem / p.n_tiles) * kTM, n0 = (rem % p.n_tiles) * kTN;
+    int prev = -1;
+    for (int i = 0; i < p.num_iters; ++i) {
+      ptx::mbar_wait(&full_bar[s], phase, 200 + i);
+      const uint32_t st = ptx::smem_u32(smem + (size_t)s * p.stage_bytes);
+      const uint32_t a_hi = st + (uint32_t)wg * 8192u, a_lo = a_hi + p.a_bytes, b_hi = st + 2 * p.a_bytes, b_lo = b_hi + p.b_bytes;
+      ptx::wgmma_fence();
+#pragma unroll
+      for (int j = 0; j < kTK / 16; ++j) {
+        const uint64_t dah = ptx::smem_desc(a_hi + j * 32, 16, 1024, ptx::kLayoutSW128);
+        const uint64_t dal = ptx::smem_desc(a_lo + j * 32, 16, 1024, ptx::kLayoutSW128);
+        const uint64_t dbh = ptx::smem_desc(b_hi + j * 32, 16, 1024, ptx::kLayoutSW128);
+        const uint64_t dbl = ptx::smem_desc(b_lo + j * 32, 16, 1024, ptx::kLayoutSW128);
+        ptx::wgmma_ss_n128<0>(acc, dah, dbh, (i | j) != 0 ? 1 : 0);
+        ptx::wgmma_ss_n128<0>(acc, dah, dbl, 1);
+        ptx::wgmma_ss_n128<0>(acc, dal, dbh, 1);
+      }
+      ptx::wgmma_commit();
+      ptx::wgmma_wait<1>();  // the previous stage's group has completed: release it
+      if (prev >= 0) ptx::mbar_arrive(&empty_bar[prev]);
+      prev = s;
+      if (++s == p.stages) {
+        s = 0;
+        phase ^= 1;
+      }
+    }
+    ptx::wgmma_wait<0>();
+    if (prev >= 0) ptx::mbar_arrive(&empty_bar[prev]);
+    ptx::fence_regs(acc);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int m = m0 + mrow0 + 8 * h;
+      if (m >= p.M) continue;
+#pragma unroll
+      for (int i = 0; i < kTN / 8; ++i) {
+        const int n = n0 + 8 * i + 2 * cq;
+        if (n < p.N) tc_store(p, z, m, n, acc[4 * i + 2 * h]);
+        if (n + 1 < p.N) tc_store(p, z, m, n + 1, acc[4 * i + 2 * h + 1]);
+      }
+    }
   }
 }
 
-static int pick_n_tile(int N) { return (N > 128) ? 256 : 128; }
+static int pick_n_tile(int) { return kTN; }
 
 // one thread per 16-byte chunk of the packed image: (n-tile, k-block, row, chunk)
 __global__ void tc_pack_kernel(const float* __restrict__ src, int conv, int64_t rs, int64_t ks, int N, int K, int Cin, int Cin8, int taps, int n_tile, int num_iters,
@@ -522,8 +414,7 @@ int wait_sleep_ns() {
 int tc_launch(TcParams& p, cudaStream_t st) {
   p.sleep_ns = wait_sleep_ns();
   p.n_tile = pick_n_tile(p.N);
-  p.stages = (p.n_tile == 256) ? 2 : 3;
-  p.tmem_cols = 2 * p.n_tile;
+  p.stages = 3;
   p.a_bytes = kTM * 128;
   p.b_bytes = (uint32_t)p.n_tile * 128;
   p.stage_bytes = 2 * p.a_bytes + 2 * p.b_bytes;
@@ -536,7 +427,7 @@ int tc_launch(TcParams& p, cudaStream_t st) {
   const size_t smem = (size_t)p.stages * p.stage_bytes + 1024 + 256;
   static bool attr_set = false;
   if (!attr_set) {
-    B2_CUDA(cudaFuncSetAttribute(tc_f32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    B2_CUDA(cudaFuncSetAttribute(tc_f32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     attr_set = true;
   }
   const int grid = std::min(p.num_tiles, kNumSMs);
@@ -549,27 +440,23 @@ bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 
 
 // ===================================================================================================================================
 // Fused attention for head dimension 64:  O = softmax(alpha * Q K^T) V  per (batch, head), fp32 in / out, every product as bf16 hi/lo x3 on
-// tcgen05 with fp32 accumulation in TMEM -- the score matrix never reaches HBM (the unfused form wrote, re-read, normalised and re-read
-// B*H*Lq*Lk floats: 0.9 GB per HTDemucs frequency layer at batch 4).
+// wgmma with fp32 accumulation in registers -- the score matrix never reaches HBM (the unfused form wrote, re-read, normalised and re-read
+// B*H*Lq*Lk floats: 0.9 GB per HTDemucs frequency layer at batch 4).  Q / K / V^T arrive as pre-split tile images (att_pack_kernel).
 //
 //   one CTA per (128-query tile, batch*head);  key tiles of 128:
-//   warp 0       : MMA issuer: S_j = Q K_j^T (128 x 128, K = 64) into one of two TMEM score buffers, then R_{j-1} = P_{j-1} V_{j-1}
-//                  (128 x 64, K = 128) into one of two TMEM output-tile buffers -- S_{j+1} is in flight while the softmax of tile j runs
-//   warps 1..4   : K producers: Q once, then K_j (keys x 64) fp32 -> bf16 hi/lo -> SWIZZLE_128B shared memory (2 slots, freed when S_j completes)
-//   warps 5..8   : V producers: V^T_j (64 x keys), 2 slots freed when R_j completes
-//   warps 9..12  : softmax, one thread per query row: row maximum, exp, running sum, P_j split into bf16 hi/lo and written as the A operand
-//                  of the second product; the 64 output accumulators of the row live in registers and are rescaled when the maximum moves
-//                  (R_j is folded in one tile late, so the fold never waits for the tensor core)
-constexpr int kAttProdWarps = 8, kAttSoftWarps = 4;
-constexpr int kAttThreads = 32 * (1 + kAttProdWarps + kAttSoftWarps);  // 416
+//   warps 0..7 : two consumer warpgroups, 64 query rows each: S_j = Q K_j^T (64 x 128, K = 64) into registers, online softmax on the
+//                fragments (row max / sum over the 4 lanes of a quad), P_j split into bf16 hi/lo in registers and fed as the A operand of
+//                O += P_j V_j (64 x 64, K = 128); O lives in registers and is rescaled when the row maximum moves
+//   warp 8     : loader: one thread, bulk copies of the 32 KB tile images into a two-slot ring (K and V slots freed independently)
+constexpr int kAttConsumers = 256;
+constexpr int kAttThreads = kAttConsumers + 32;
 constexpr int kAttQ = 128, kAttKeys = 128, kAttD = 64;
 constexpr uint32_t kAttQBytes = kAttQ * 128;            // one plane of Q: 128 rows x 64 bf16
-constexpr uint32_t kAttPBlk = kAttQ * 128;              // one plane of one 64-key block of P
 constexpr uint32_t kAttKBytes = kAttKeys * 128;         // one plane of K_j
 constexpr uint32_t kAttVBlk = kAttD * 128;              // one plane of one 64-key block of V^T_j
 constexpr uint32_t kAttStage = 2 * kAttKBytes + 4 * kAttVBlk;  // 64 KB
-constexpr uint32_t kAttOffP = 2 * kAttQBytes, kAttOffStage = kAttOffP + 4 * kAttPBlk;
-constexpr uint32_t kAttSmem = kAttOffStage + 2 * kAttStage;  // 224 KB
+constexpr uint32_t kAttOffStage = 2 * kAttQBytes;
+constexpr uint32_t kAttSmem = kAttOffStage + 2 * kAttStage;  // 160 KB
 
 struct AttParams {
   const float* q;   // q[b * q_bs + m * q_rs + h * 64 + d]
@@ -579,9 +466,9 @@ struct AttParams {
   int64_t q_bs, q_rs, k_bs, k_rs, vt_bs, vt_rs, o_bs, o_rs;
   int H, Lq, Lk;
   float alpha;
-  int q_vec, k_vec, v_vec, o_vec;
-  int v_kn;  // 1: V given untransposed, v[b * vt_bs + n * vt_rs + h * 64 + d] (the producers gather it d-major)
-  // PACKED variant: Q / K / V^T already split into bf16 hi / lo and laid out as the kernel's shared-memory tiles by att_pack_kernel, 32 KB per tile:
+  int o_vec;
+  int v_kn;  // 1: V given untransposed, v[b * vt_bs + n * vt_rs + h * 64 + d] (the pack kernel gathers it d-major)
+  // Q / K / V^T split into bf16 hi / lo and laid out as the kernel's shared-memory tiles by att_pack_kernel, 32 KB per tile:
   //   qimg[(z * mq_tiles + mt)] = [hi 128 x 128 B | lo],  kimg[(z * nk + j)] = [hi | lo],  vimg[(z * nk + j)] = [hi kb0 | hi kb1 | lo kb0 | lo kb1] (64 rows x 128 B each)
   const uint8_t* qimg;
   const uint8_t* kimg;
@@ -594,8 +481,6 @@ __device__ __forceinline__ float ex2_approx(float x) {
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
-
-constexpr int kAttThreadsPacked = 32 * (2 + kAttSoftWarps);  // MMA issuer warp, loader warp, 4 softmax warps
 
 // one 16-byte chunk (8 values) of a tile image per thread; see AttParams for the image layouts
 __global__ void att_pack_kernel(const AttParams p, uint8_t* __restrict__ qimg, uint8_t* __restrict__ kimg, uint8_t* __restrict__ vimg, int nk, int64_t nq_chunks,
@@ -637,130 +522,39 @@ __global__ void att_pack_kernel(const AttParams p, uint8_t* __restrict__ qimg, u
   }
 }
 
-template <bool PACKED>
-__global__ void __launch_bounds__(PACKED ? kAttThreadsPacked : kAttThreads, 1) tc_attention_kernel(const AttParams p) {
+__global__ void __launch_bounds__(kAttThreads, 1) tc_attention_kernel(const AttParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (ptx::smem_u32(smem_raw) & 1023u)) & 1023u);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kAttSmem);
-  uint64_t* q_full = bars;            // [1]
-  uint64_t* k_full = bars + 1;        // [2]  K_j converted            (K producer warps -> MMA)
-  uint64_t* k_empty = bars + 3;       // [2]  S_j done: K slot free     (MMA commit -> K producers)
-  uint64_t* v_full = bars + 5;        // [2]
-  uint64_t* v_empty = bars + 7;       // [2]  R_j done: V slot free
-  uint64_t* s_full = bars + 9;        // [2]
-  uint64_t* s_empty = bars + 11;      // [2]
-  uint64_t* p_full = bars + 13;       // [1]
-  uint64_t* p_empty = bars + 14;      // [1]
-  uint64_t* o_full = bars + 15;       // [2]
-  uint64_t* o_empty = bars + 17;      // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 19);
+  uint64_t* q_full = bars;       // [1]
+  uint64_t* k_full = bars + 1;   // [2]  K_j landed
+  uint64_t* k_empty = bars + 3;  // [2]  S_j done: K slot free
+  uint64_t* v_full = bars + 5;   // [2]
+  uint64_t* v_empty = bars + 7;  // [2]  O += P_j V_j done: V slot free
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
-    constexpr uint32_t kFillArrivals = PACKED ? 1 : kAttProdWarps / 2;  // PACKED: the loader thread's arrive.expect_tx (the bulk copy completes the bytes)
-    ptx::mbar_init(q_full, kFillArrivals);
+    ptx::mbar_init(q_full, 1);
     for (int a = 0; a < 2; ++a) {
-      ptx::mbar_init(&k_full[a], kFillArrivals);
-      ptx::mbar_init(&k_empty[a], 1);
-      ptx::mbar_init(&v_full[a], kFillArrivals);
-      ptx::mbar_init(&v_empty[a], 1);
-      ptx::mbar_init(&s_full[a], 1);
-      ptx::mbar_init(&s_empty[a], kAttSoftWarps);
-      ptx::mbar_init(&o_full[a], 1);
-      ptx::mbar_init(&o_empty[a], kAttSoftWarps);
+      ptx::mbar_init(&k_full[a], 1);
+      ptx::mbar_init(&k_empty[a], kAttConsumers);
+      ptx::mbar_init(&v_full[a], 1);
+      ptx::mbar_init(&v_empty[a], kAttConsumers);
     }
-    ptx::mbar_init(p_full, kAttSoftWarps);
-    ptx::mbar_init(p_empty, 1);
     ptx::fence_barrier_init();
   }
-  if (warp == 0) ptx::tmem_alloc(tmem_slot, 512);
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;  // columns [0, 256): two score buffers; [256, 384): two output-tile buffers
 
   const int z = blockIdx.y, b = z / p.H, h = z - b * p.H;
   const int m0 = blockIdx.x * kAttQ;
   const int nk = (p.Lk + kAttKeys - 1) / kAttKeys;
-  uint8_t* q_hi = smem;
-  uint8_t* q_lo = smem + kAttQBytes;
-  uint8_t* p_hi = smem + kAttOffP;                 // [2 key blocks][128 rows x 128 B]
-  uint8_t* p_lo = smem + kAttOffP + 2 * kAttPBlk;
 
-  if (warp == 0) {
-    if (lane == 0) {
-      // ===== MMA issuer =====
-      const uint32_t idesc_s = ptx::instr_desc_bf16(kAttQ, kAttKeys, 0, 0), idesc_o = ptx::instr_desc_bf16(kAttQ, kAttD, 0, 0);
-      const uint32_t qh = ptx::smem_u32(q_hi), ql = ptx::smem_u32(q_lo), ph_ = ptx::smem_u32(p_hi), pl_ = ptx::smem_u32(p_lo);
-      ptx::mbar_wait(q_full, 0, 500);
-      // Two instruction streams, issued in whatever order their inputs arrive: S_js = Q K_js^T needs K_js and a free score buffer, R_jo = P_jo V_jo needs
-      // P_jo, V_jo and a free output-tile buffer.  (A fixed S, R, S, R order made R_{j-1} wait for the K_j conversion and serialised the pipeline.)
-      int js = 0, jo = 0;
-      uint32_t idle = 0;
-      while (jo < nk) {
-        bool did = false;
-        if (js < nk) {
-          const int st = js & 1;
-          const uint32_t ph = (uint32_t)(js >> 1) & 1u;
-          if (ptx::mbar_try_wait(&k_full[st], ph) && ptx::mbar_try_wait(&s_empty[st], ph ^ 1u)) {
-            ptx::tc_fence_after();
-            const uint32_t d = tmem_base + (uint32_t)st * kAttKeys;
-            const uint32_t kh = ptx::smem_u32(smem + kAttOffStage + (size_t)st * kAttStage), kl = kh + kAttKBytes;
-#pragma unroll
-            for (int jj = 0; jj < kAttD / 16; ++jj) {
-              const uint64_t dqh = ptx::smem_desc(qh + jj * 32, 16, 1024, ptx::kLayoutSW128), dql = ptx::smem_desc(ql + jj * 32, 16, 1024, ptx::kLayoutSW128);
-              const uint64_t dkh = ptx::smem_desc(kh + jj * 32, 16, 1024, ptx::kLayoutSW128), dkl = ptx::smem_desc(kl + jj * 32, 16, 1024, ptx::kLayoutSW128);
-              ptx::umma_bf16(d, dqh, dkh, idesc_s, jj != 0 ? 1u : 0u);
-              ptx::umma_bf16(d, dqh, dkl, idesc_s, 1u);
-              ptx::umma_bf16(d, dql, dkh, idesc_s, 1u);
-            }
-            ptx::umma_commit(&s_full[st]);
-            ptx::umma_commit(&k_empty[st]);
-            ++js;
-            did = true;
-          }
-        }
-        if (jo < js) {
-          const int st = jo & 1;
-          const uint32_t ph = (uint32_t)(jo >> 1) & 1u;
-          if (ptx::mbar_try_wait(p_full, (uint32_t)jo & 1u) && ptx::mbar_try_wait(&v_full[st], ph) && ptx::mbar_try_wait(&o_empty[st], ph ^ 1u)) {
-            ptx::tc_fence_after();
-            const uint32_t d = tmem_base + 2 * kAttKeys + (uint32_t)st * kAttD;
-            const uint32_t vh = ptx::smem_u32(smem + kAttOffStage + (size_t)st * kAttStage) + 2 * kAttKBytes, vl = vh + 2 * kAttVBlk;
-#pragma unroll
-            for (int kb = 0; kb < 2; ++kb) {
-#pragma unroll
-              for (int jj = 0; jj < 4; ++jj) {
-                const uint64_t dph = ptx::smem_desc(ph_ + kb * kAttPBlk + jj * 32, 16, 1024, ptx::kLayoutSW128);
-                const uint64_t dpl = ptx::smem_desc(pl_ + kb * kAttPBlk + jj * 32, 16, 1024, ptx::kLayoutSW128);
-                const uint64_t dvh = ptx::smem_desc(vh + kb * kAttVBlk + jj * 32, 16, 1024, ptx::kLayoutSW128);
-                const uint64_t dvl = ptx::smem_desc(vl + kb * kAttVBlk + jj * 32, 16, 1024, ptx::kLayoutSW128);
-                ptx::umma_bf16(d, dph, dvh, idesc_o, (kb | jj) != 0 ? 1u : 0u);
-                ptx::umma_bf16(d, dph, dvl, idesc_o, 1u);
-                ptx::umma_bf16(d, dpl, dvh, idesc_o, 1u);
-              }
-            }
-            ptx::umma_commit(&o_full[st]);
-            ptx::umma_commit(&v_empty[st]);
-            ptx::umma_commit(p_empty);
-            ++jo;
-            did = true;
-          }
-        }
-        if (did) {
-          idle = 0;
-        } else if (__nanosleep(40), ++idle > (1u << 22)) {
-          printf("b200sep: attention MMA issuer stalled block=(%d,%d) js=%d jo=%d\n", blockIdx.x, blockIdx.y, js, jo);
-          __trap();
-        }
-      }
-    }
-  } else if (PACKED && warp == 1) {
-    // ===== loader (PACKED): one thread, bulk copies of the pre-split 32 KB tile images; K and V streams polled independently =====
+  if (warp == kAttConsumers / 32) {
+    // ===== loader: K and V streams polled independently =====
     if (lane == 0) {
       const int64_t zq = (int64_t)z * p.mq_tiles + blockIdx.x, zk = (int64_t)z * nk;
       ptx::mbar_arrive_expect_tx(q_full, 32768);
-      ptx::bulk_load_1d(q_hi, p.qimg + zq * 32768, 32768, q_full);
+      ptx::bulk_load_1d(smem, p.qimg + zq * 32768, 32768, q_full);
       int jk = 0, jv = 0;
       uint32_t idle = 0;
       while (jk < nk || jv < nk) {
@@ -786,158 +580,126 @@ __global__ void __launch_bounds__(PACKED ? kAttThreadsPacked : kAttThreads, 1) t
         if (did) {
           idle = 0;
         } else if (__nanosleep(100), ++idle > (1u << 22)) {
-          printf("b200sep: attention loader stalled block=(%d,%d) jk=%d jv=%d\n", blockIdx.x, blockIdx.y, jk, jv);
-          __trap();
+          __trap();  // stalled pipeline
         }
       }
     }
-  } else if (!PACKED && warp <= kAttProdWarps / 2) {
-    // ===== K producers (warps 1..4): Q once, then K_j into the K half of stage j % 2 as soon as S_{j-2} has consumed it =====
-    constexpr int NT = 32 * (kAttProdWarps / 2);
-    const int pt = threadIdx.x - 32;
-    const float* qb = p.q + (int64_t)b * p.q_bs + (int64_t)h * kAttD;
-    const float* kb_ = p.k + (int64_t)b * p.k_bs + (int64_t)h * kAttD;
-    fill_kmajor<NT>(q_hi, q_lo, qb, p.q_rs, kAttQ, m0, p.Lq, 0, kAttD, p.q_vec, pt);
-    ptx::fence_proxy_async();
-    __syncwarp();
-    if (lane == 0) ptx::mbar_arrive(q_full);
-    for (int j = 0; j < nk; ++j) {
-      const int st = j & 1;
-      const uint32_t ph = (uint32_t)(j >> 1) & 1u;
-      ptx::mbar_wait_backoff(&k_empty[st], ph ^ 1u, 200, 550 + st);
-      uint8_t* sb = smem + kAttOffStage + (size_t)st * kAttStage;
-      fill_kmajor<NT>(sb, sb + kAttKBytes, kb_, p.k_rs, kAttKeys, j * kAttKeys, p.Lk, 0, kAttD, p.k_vec, pt);
-      ptx::fence_proxy_async();
-      __syncwarp();
-      if (lane == 0) ptx::mbar_arrive(&k_full[st]);
-    }
-  } else if (!PACKED && warp <= kAttProdWarps) {
-    // ===== V producers (warps 5..8): V^T_j (64 x 128 keys as two 64-key blocks) into the V half of stage j % 2 once R_{j-2} has consumed it =====
-    constexpr int NT = 32 * (kAttProdWarps / 2);
-    const int pt = threadIdx.x - 32 - NT;
-    const float* vb = p.vt + (int64_t)b * p.vt_bs + (p.v_kn ? (int64_t)h * kAttD : (int64_t)h * kAttD * p.vt_rs);
-    for (int j = 0; j < nk; ++j) {
-      const int st = j & 1;
-      const uint32_t ph = (uint32_t)(j >> 1) & 1u;
-      ptx::mbar_wait_backoff(&v_empty[st], ph ^ 1u, 200, 555 + st);
-      uint8_t* vh = smem + kAttOffStage + (size_t)st * kAttStage + 2 * kAttKBytes;
-      uint8_t* vl = vh + 2 * kAttVBlk;
-#pragma unroll
-      for (int kb = 0; kb < 2; ++kb) {
-        if (p.v_kn) fill_nmajor<NT>(vh + kb * kAttVBlk, vl + kb * kAttVBlk, vb, p.vt_rs, kAttD, 0, kAttD, j * kAttKeys + kb * 64, p.Lk, pt);
-        else fill_kmajor<NT>(vh + kb * kAttVBlk, vl + kb * kAttVBlk, vb, p.vt_rs, kAttD, 0, kAttD, j * kAttKeys + kb * 64, p.Lk, p.v_vec, pt);
-      }
-      ptx::fence_proxy_async();
-      __syncwarp();
-      if (lane == 0) ptx::mbar_arrive(&v_full[st]);
-    }
-  } else {
-    // ===== softmax: thread = query row (TMEM lane quadrant = warp % 4) =====
-    const int qd = warp & 3;
-    const int row = qd * 32 + lane;
-    const int m = m0 + row;
-    const uint32_t tlane = tmem_base + ((uint32_t)(qd * 32) << 16);
-    // base-2 domain: p = 2^(s * a2 - m2) with a2 = alpha * log2(e): one FFMA + one MUFU.EX2 per score (expf() costs ~10 instructions, and this warp is
-    // the only softmax warp of its scheduler: its instruction count is the kernel's critical path)
-    const float a2 = p.alpha * 1.4426950408889634f;
-    float mrun = -INFINITY, l = 0.f, corr_prev = 1.f;
-    float O[kAttD];
-#pragma unroll
-    for (int e = 0; e < kAttD; ++e) O[e] = 0.f;
-    for (int j = 0; j <= nk; ++j) {
-      float corr = 1.f;
-      if (j < nk) {
-        const int st = j & 1;
-        const uint32_t ph = (uint32_t)(j >> 1) & 1u;
-        ptx::mbar_wait_backoff(&s_full[st], ph, 20, 560 + st);
-        ptx::tc_fence_after();
-        const uint32_t ts = tlane + (uint32_t)st * kAttKeys;
-        const int nvalid = min(kAttKeys, p.Lk - j * kAttKeys);
-        const bool full = nvalid == kAttKeys;  // warp-uniform
-        float mx = -INFINITY;
-#pragma unroll 1
-        for (int c = 0; c < 4; ++c) {
-          uint32_t v[32];
-          ptx::tmem_ld32(ts + c * 32, v);
-          ptx::tmem_ld_wait();
-          if (full) {
-#pragma unroll
-            for (int e = 0; e < 32; e += 2) mx = fmaxf(mx, fmaxf(__uint_as_float(v[e]), __uint_as_float(v[e + 1])));
-          } else {
-#pragma unroll
-            for (int e = 0; e < 32; ++e)
-              if (c * 32 + e < nvalid) mx = fmaxf(mx, __uint_as_float(v[e]));
-          }
-        }
-        const float mnew = fmaxf(mrun, mx * a2);
-        corr = ex2_approx(mrun - mnew);  // first tile: 2^(-inf) = 0
-        mrun = mnew;
-        ptx::mbar_wait_backoff(p_empty, ((uint32_t)j & 1u) ^ 1u, 20, 570);  // P_{j-1} consumed by the tensor core
-        float lsum = 0.f;
-#pragma unroll 1
-        for (int c = 0; c < 4; ++c) {
-          uint32_t v[32];
-          ptx::tmem_ld32(ts + c * 32, v);
-          ptx::tmem_ld_wait();
-#pragma unroll
-          for (int ch = 0; ch < 4; ++ch) {
-            float pv[8];
-#pragma unroll
-            for (int e = 0; e < 8; ++e) {
-              const float x = ex2_approx(fmaf(__uint_as_float(v[ch * 8 + e]), a2, -mnew));
-              pv[e] = (full || c * 32 + ch * 8 + e < nvalid) ? x : 0.f;
-              lsum += pv[e];
-            }
-            const int chunk = c * 4 + ch;  // 16 chunks of 8 keys; chunks 0..7 = key block 0
-            store_chunk(p_hi + (chunk >> 3) * kAttPBlk, p_lo + (chunk >> 3) * kAttPBlk, row, chunk & 7, pv);
-          }
-        }
-        l = l * corr + lsum;
-        ptx::tc_fence_before();
-        ptx::fence_proxy_async();
-        __syncwarp();
-        if (lane == 0) {
-          ptx::mbar_arrive(&s_empty[st]);
-          ptx::mbar_arrive(p_full);
-        }
-      }
-      if (j > 0) {  // fold R_{j-1} (relative to the maximum after tile j-1) into the accumulators (relative to the maximum after tile j-2)
-        const int jp = j - 1, st = jp & 1;
-        const uint32_t ph = (uint32_t)(jp >> 1) & 1u;
-        ptx::mbar_wait_backoff(&o_full[st], ph, 20, 580 + st);
-        ptx::tc_fence_after();
-        const uint32_t to = tlane + 2 * kAttKeys + (uint32_t)st * kAttD;
-#pragma unroll
-        for (int c = 0; c < 2; ++c) {
-          uint32_t v[32];
-          ptx::tmem_ld32(to + c * 32, v);
-          ptx::tmem_ld_wait();
-#pragma unroll
-          for (int e = 0; e < 32; ++e) O[c * 32 + e] = fmaf(O[c * 32 + e], corr_prev, __uint_as_float(v[e]));
-        }
-        ptx::tc_fence_before();
-        __syncwarp();
-        if (lane == 0) ptx::mbar_arrive(&o_empty[st]);
-      }
-      corr_prev = corr;
-    }
-    if (m < p.Lq) {
-      const float inv = 1.f / l;
-      float* o = p.out + (int64_t)b * p.o_bs + (int64_t)m * p.o_rs + (int64_t)h * kAttD;
-      if (p.o_vec) {
-#pragma unroll
-        for (int e = 0; e < kAttD; e += 4) *reinterpret_cast<float4*>(o + e) = make_float4(O[e] * inv, O[e + 1] * inv, O[e + 2] * inv, O[e + 3] * inv);
-      } else {
-#pragma unroll
-        for (int e = 0; e < kAttD; ++e) o[e] = O[e] * inv;
-      }
-    }
+    return;
   }
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    ptx::tc_fence_after();
-    ptx::tmem_dealloc(tmem_base, 512);
+
+  // ===== consumers: thread = rows r0 and r0 + 8 of the query tile, columns 8i + 2*cq + {0, 1} of every fragment =====
+  const int wg = warp >> 2, g = lane >> 2, cq = lane & 3;
+  const int r0 = wg * 64 + (warp & 3) * 16 + g;
+  // base-2 domain: p = 2^(s * a2 - m2) with a2 = alpha * log2(e): one FFMA + one MUFU.EX2 per score
+  const float a2 = p.alpha * 1.4426950408889634f;
+  float mrun[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+  float O[kAttD / 2];
+#pragma unroll
+  for (int e = 0; e < kAttD / 2; ++e) O[e] = 0.f;
+  const uint32_t qh = ptx::smem_u32(smem) + (uint32_t)wg * 8192u, ql = qh + kAttQBytes;
+  ptx::mbar_wait(q_full, 0, 500);
+  for (int j = 0; j < nk; ++j) {
+    const int st = j & 1;
+    const uint32_t ph = (uint32_t)(j >> 1) & 1u;
+    const uint32_t kh = ptx::smem_u32(smem + kAttOffStage + (size_t)st * kAttStage), kl = kh + kAttKBytes;
+    ptx::mbar_wait(&k_full[st], ph, 560 + st);
+    float S[kAttKeys / 2];
+    ptx::wgmma_fence();
+#pragma unroll
+    for (int jj = 0; jj < kAttD / 16; ++jj) {
+      const uint64_t dqh = ptx::smem_desc(qh + jj * 32, 16, 1024, ptx::kLayoutSW128), dql = ptx::smem_desc(ql + jj * 32, 16, 1024, ptx::kLayoutSW128);
+      const uint64_t dkh = ptx::smem_desc(kh + jj * 32, 16, 1024, ptx::kLayoutSW128), dkl = ptx::smem_desc(kl + jj * 32, 16, 1024, ptx::kLayoutSW128);
+      ptx::wgmma_ss_n128<0>(S, dqh, dkh, jj != 0 ? 1 : 0);
+      ptx::wgmma_ss_n128<0>(S, dqh, dkl, 1);
+      ptx::wgmma_ss_n128<0>(S, dql, dkh, 1);
+    }
+    ptx::wgmma_commit();
+    ptx::wgmma_wait<0>();
+    ptx::fence_regs(S);
+    ptx::mbar_arrive(&k_empty[st]);
+
+    const int nvalid = min(kAttKeys, p.Lk - j * kAttKeys);
+    float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+    for (int i = 0; i < kAttKeys / 8; ++i)
+#pragma unroll
+      for (int e = 0; e < 2; ++e)
+        if (8 * i + 2 * cq + e < nvalid) {
+          mx[0] = fmaxf(mx[0], S[4 * i + e]);
+          mx[1] = fmaxf(mx[1], S[4 * i + 2 + e]);
+        }
+    float mnew[2], corr[2];
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 1));
+      mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 2));
+      mnew[hh] = fmaxf(mrun[hh], mx[hh] * a2);
+      corr[hh] = ex2_approx(mrun[hh] - mnew[hh]);  // first tile: 2^(-inf) = 0
+      mrun[hh] = mnew[hh];
+    }
+    // P_j as the register A operand of the second product: k-step kk covers keys 16kk..16kk+15; A register q holds row r0 + 8*(q & 1),
+    // keys 16kk + 8*(q >> 1) + 2*cq + {0, 1} -- exactly S[8kk + 2q], S[8kk + 2q + 1]
+    uint32_t ah[kAttKeys / 16][4], al[kAttKeys / 16][4];
+    float lsum[2] = {0.f, 0.f};
+#pragma unroll
+    for (int kk = 0; kk < kAttKeys / 16; ++kk)
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        const int hh = q & 1, col = 16 * kk + 8 * (q >> 1) + 2 * cq;
+        float x0 = ex2_approx(fmaf(S[8 * kk + 2 * q], a2, -mnew[hh])), x1 = ex2_approx(fmaf(S[8 * kk + 2 * q + 1], a2, -mnew[hh]));
+        if (col >= nvalid) x0 = 0.f;
+        if (col + 1 >= nvalid) x1 = 0.f;
+        lsum[hh] += x0 + x1;
+        split2(x0, x1, ah[kk][q], al[kk][q]);
+      }
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) l[hh] = l[hh] * corr[hh] + lsum[hh];
+#pragma unroll
+    for (int i = 0; i < kAttD / 8; ++i) {
+      O[4 * i] *= corr[0];
+      O[4 * i + 1] *= corr[0];
+      O[4 * i + 2] *= corr[1];
+      O[4 * i + 3] *= corr[1];
+    }
+    ptx::mbar_wait(&v_full[st], ph, 580 + st);
+    const uint32_t vh = kh + 2 * kAttKBytes, vl = vh + 2 * kAttVBlk;
+    ptx::wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < kAttKeys / 16; ++kk) {
+      const uint32_t off = (uint32_t)(kk >> 2) * kAttVBlk + (uint32_t)(kk & 3) * 32u;
+      const uint64_t dvh = ptx::smem_desc(vh + off, 16, 1024, ptx::kLayoutSW128), dvl = ptx::smem_desc(vl + off, 16, 1024, ptx::kLayoutSW128);
+      ptx::wgmma_rs_n64(O, ah[kk], dvh);
+      ptx::wgmma_rs_n64(O, ah[kk], dvl);
+      ptx::wgmma_rs_n64(O, al[kk], dvh);
+    }
+    ptx::wgmma_commit();
+    ptx::wgmma_wait<0>();
+    ptx::fence_regs(O);
+#pragma unroll
+    for (int kk = 0; kk < kAttKeys / 16; ++kk) {
+      ptx::fence_regs(ah[kk]);
+      ptx::fence_regs(al[kk]);
+    }
+    ptx::mbar_arrive(&v_empty[st]);
+  }
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    l[hh] += __shfl_xor_sync(0xffffffffu, l[hh], 1);
+    l[hh] += __shfl_xor_sync(0xffffffffu, l[hh], 2);
+    const int m = m0 + r0 + 8 * hh;
+    if (m >= p.Lq) continue;
+    const float inv = 1.f / l[hh];
+    float* o = p.out + (int64_t)b * p.o_bs + (int64_t)m * p.o_rs + (int64_t)h * kAttD;
+#pragma unroll
+    for (int i = 0; i < kAttD / 8; ++i) {
+      const int col = 8 * i + 2 * cq;
+      if (p.o_vec) {
+        *reinterpret_cast<float2*>(o + col) = make_float2(O[4 * i + 2 * hh] * inv, O[4 * i + 2 * hh + 1] * inv);
+      } else {
+        o[col] = O[4 * i + 2 * hh] * inv;
+        o[col + 1] = O[4 * i + 2 * hh + 1] * inv;
+      }
+    }
   }
 }
 
@@ -957,47 +719,38 @@ int tc_attention_f32(const float* q, const float* k, const float* vt, float* out
   p.q = q; p.k = k; p.vt = vt; p.out = out;
   p.q_bs = q_bs; p.q_rs = q_rs; p.k_bs = k_bs; p.k_rs = k_rs; p.vt_bs = vt_bs; p.vt_rs = vt_rs; p.o_bs = o_bs; p.o_rs = o_rs;
   p.H = H; p.Lq = Lq; p.Lk = Lk; p.alpha = alpha;
-  p.q_vec = (q_rs % 4 == 0) && (q_bs % 4 == 0) && aligned16(q);
-  p.k_vec = (k_rs % 4 == 0) && (k_bs % 4 == 0) && aligned16(k);
-  p.v_vec = (vt_rs % 4 == 0) && (vt_bs % 4 == 0) && aligned16(vt);
   p.o_vec = (o_rs % 4 == 0) && (o_bs % 4 == 0) && aligned16(out);
   const size_t smem = (size_t)kAttSmem + 1024 + 256;
   B2_CHECK_ARG((int64_t)B * H <= 65535, "attention_f32: batch * heads too large");
   dim3 grid((unsigned)cdiv(Lq, kAttQ), (unsigned)(B * H));
-  if (work) {
-    // Every K / V tile is consumed by all query tiles of its (batch, head): split it into bf16 hi / lo ONCE here, not once per consumer inside the attention
-    // kernel (ncu: the in-kernel producers were 40 % of its instructions and took the schedulers from the softmax warps).
-    B2_CHECK_ARG(aligned16(work), "attention_f32: work must be 16-byte aligned");
-    static bool attr_packed = false;
-    if (!attr_packed) {
-      B2_CUDA(cudaFuncSetAttribute(tc_attention_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-      attr_packed = true;
-    }
-    const int nk = cdiv(Lk, kAttKeys);
-    p.mq_tiles = cdiv(Lq, kAttQ);
-    uint8_t* qimg = (uint8_t*)work;
-    uint8_t* kimg = qimg + (int64_t)B * H * p.mq_tiles * 32768;
-    uint8_t* vimg = kimg + (int64_t)B * H * nk * 32768;
-    p.qimg = qimg; p.kimg = kimg; p.vimg = vimg;
-    const int64_t nq_chunks = (int64_t)B * H * p.mq_tiles * 1024, nk_chunks = (int64_t)B * H * nk * 1024;
-    att_pack_kernel<<<(int)std::min<int64_t>(cdiv(nq_chunks + 2 * nk_chunks, 256), kNumSMs * 32), 256, 0, st>>>(p, qimg, kimg, vimg, nk, nq_chunks, nk_chunks);
-    B2_LAUNCHED();
-    tc_attention_kernel<true><<<grid, kAttThreadsPacked, smem, st>>>(p);
-    B2_LAUNCHED();
-    return B200SEP_OK;
+  // Every K / V tile is consumed by all query tiles of its (batch, head): it is split into bf16 hi / lo ONCE, here, not once per consumer inside the
+  // attention kernel.  Without caller scratch the images live in a stream-ordered allocation for the duration of the call.
+  void* scratch = nullptr;
+  if (!work) {
+    B2_CUDA(cudaMallocAsync(&scratch, (size_t)tc_attention_work_bytes(B, H, Lq, Lk), st));
+    work = scratch;
   }
+  B2_CHECK_ARG(aligned16(work), "attention_f32: work must be 16-byte aligned");
   static bool attr_set = false;
   if (!attr_set) {
-    B2_CUDA(cudaFuncSetAttribute(tc_attention_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    B2_CUDA(cudaFuncSetAttribute(tc_attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     attr_set = true;
   }
-  tc_attention_kernel<false><<<grid, kAttThreads, smem, st>>>(p);
+  const int nk = cdiv(Lk, kAttKeys);
+  p.mq_tiles = cdiv(Lq, kAttQ);
+  uint8_t* qimg = (uint8_t*)work;
+  uint8_t* kimg = qimg + (int64_t)B * H * p.mq_tiles * 32768;
+  uint8_t* vimg = kimg + (int64_t)B * H * nk * 32768;
+  p.qimg = qimg; p.kimg = kimg; p.vimg = vimg;
+  const int64_t nq_chunks = (int64_t)B * H * p.mq_tiles * 1024, nk_chunks = (int64_t)B * H * nk * 1024;
+  att_pack_kernel<<<(int)std::min<int64_t>(cdiv(nq_chunks + 2 * nk_chunks, 256), kNumSMs * 32), 256, 0, st>>>(p, qimg, kimg, vimg, nk, nq_chunks, nk_chunks);
   B2_LAUNCHED();
+  tc_attention_kernel<<<grid, kAttThreads, smem, st>>>(p);
+  B2_LAUNCHED();
+  if (scratch) B2_CUDA(cudaFreeAsync(scratch, st));
   return B200SEP_OK;
 }
 
-namespace {
-}  // namespace
 
 bool tc_enabled() {
   static const bool on = [] {

@@ -1,6 +1,6 @@
 // TFC_TDF_net forward plan (MDX23C; audio_separator/separator/uvr_lib_v5/tfc_tdf_v3.py:110-267 of the reference).
 // InstanceNorm2d(affine)+GELU pre-activations, 3x3 / 1x1 / 2x2-strided convolutions, TDF linears, concat skips.
-// Every contraction runs on the tcgen05 "pair" pipeline (umma_ops.cu); normalisation + GELU is one fused
+// Every contraction runs on the wgmma "pair" pipeline (umma_ops.cu); normalisation + GELU is one fused
 // per-plane kernel between them (elementwise.cu); TDF layers too small for TMA fall back to the pair-aware SIMT GEMM.
 // Activation layout: (B, C, T, F) pair tensors, F innermost (the network's own layout after transpose(-1,-2), :236).
 #include <math.h>

@@ -1,9 +1,9 @@
-// tcgen05 tensor-core operators on "pair" tensors (fp32 values stored as two bf16 planes, hi + lo).
+// Hopper (sm_90a) tensor-core operators on "pair" tensors (fp32 values stored as two bf16 planes, hi + lo).
 //
 // Why pairs: the reference computes the networks in fp32 and parity is gated at 1e-4 on PCM samples; a single
 // TF32/BF16 pass misses that (measured 5e-4 / 3e-3 relative on the ConvTDFNet), so every contraction is evaluated as
 //      A*B ~= Ah*Bh + Ah*Bl + Al*Bh          (Ah = bf16(A), Al = bf16(A - Ah); dropped terms <= 2^-16 |A||B|)
-// with fp32 accumulation in TMEM: three kind::f16 UMMAs per k-step at the bf16 rate (measured error 7e-6 relative,
+// with fp32 accumulation: three bf16 wgmma products per k-step at the bf16 rate (measured error 7e-6 relative,
 // DESIGN.md).  Producers write activations already split, so a pair tensor costs the same 4 bytes/element as fp32
 // and its planes are fed to the tensor cores straight from TMA-written shared memory, no register staging.
 //
@@ -11,13 +11,12 @@
 //   GEMM : D[M][N] = A[M][K] * W[N][K]^T     (TDF linears; A, W K-major, TMA SWIZZLE_128B tiles of 64 k)
 //   CONV : implicit GEMM for the 3x3 stride-1 convolution on (B,C,T,F) pairs.  The A tile of one filter ROW dy is a
 //          TMA box [kc channels][128 pixels along F] at row t+dy-1 (out-of-bounds rows zero-filled = the padding); it
-//          lands MN-major (pixels contiguous), which tcgen05 consumes directly (a_major = MN).  TMA cannot shift a box
-//          by one bf16 along the innermost axis (box starts must be 16-byte aligned -- measured: illegal instruction),
-//          so the horizontal taps are moved to the OUTPUT side: B holds the three dx filter columns side by side
-//          (N = 3*n_c accumulator columns, P_dx[m] = W[dy][dx] . x[f0+m]) and the epilogue forms
-//          out[f0+j] = P_0[j-1] + P_1[j] + P_2[j+1] with warp shuffles (+ a small smem exchange at warp edges).
-//          Tiles advance by 120 pixels so that every output has both neighbours inside the same 128-row tile.
-// Warp roles per CTA (192 threads): warp 0 = TMA producer, warp 1 = TMEM alloc + MMA issuer, warps 2-5 = epilogue.
+//          lands MN-major (pixels contiguous), which wgmma consumes directly (transposed A).  TMA cannot shift a box
+//          by one bf16 along the innermost axis (box starts must be 16-byte aligned), so the horizontal taps are moved
+//          to the OUTPUT side: B holds the three dx filter columns side by side (N = 3*n_c accumulator columns,
+//          P_dx[m] = W[dy][dx] . x[f0+m]) and the epilogue forms out[f0+j] = P_0[j-1] + P_1[j] + P_2[j+1] with warp
+//          shuffles (+ a small smem exchange at warp edges).
+// Warp roles per CTA (288 threads): warps 0-7 = two consumer warpgroups (wgmma issue + epilogue), warp 8 = TMA producer.
 #include <cuda_bf16.h>
 #include <stdlib.h>
 #include <string.h>
@@ -34,30 +33,27 @@
 namespace b200sep {
 
 using bf16 = __nv_bfloat16;
-constexpr int kEpiParts = 2;  // epilogue warps per TMEM lane quadrant: the epilogue is latency-bound (0.48 eligible warps per scheduler with 2), so more warps = more overlap
-constexpr int kUmmaThreads = 64 + 128 * kEpiParts;  // warp 0 TMA, warp 1 MMA, then 4 * kEpiParts epilogue warps
+constexpr int kConsumerThreads = 256;                 // two consumer warpgroups: rows 0-63 and 64-127 of a 128-row tile
+constexpr int kUmmaThreads = kConsumerThreads + 32;   // + the TMA producer warp (warp 8)
 constexpr int kMaxChannels = 1024;  // per-channel scale/shift staged in shared memory (conv modes)
 constexpr int kTileM = 128;
-constexpr int kConv3Parts = 2;  // CONV3x3 kernel: epilogue warps per TMEM lane quadrant.  Measured with 4 (16 epilogue warps, 88 registers): 530 us vs 477 us per scale-0 launch under ncu -- the epilogue is not what paces the kernel (profiles/README.md, round 2)
-constexpr int kConv3Threads = 64 + 128 * kConv3Parts;
-constexpr int kConvStride = 112;  // output pixels per 3x3 tile: TMEM rows 8..119 of the 128 loaded pixels [f0 - 8, f0 + 120), so that loads AND stores start 16-byte aligned
+constexpr int kMaxNTile = 128;      // accumulator columns of umma_pair_kernel: n_tile / 2 fp32 registers per consumer thread
+constexpr int kConvStride = 112;    // output pixels per 3x3 tile: rows 8..119 of the 128 loaded pixels [f0 - 8, f0 + 120), so that loads AND stores start 16-byte aligned
+constexpr int kEpiBar = 1;          // named barrier of the 256 consumer threads
 
 struct UmmaParams {
   int mode;  // 0 GEMM, 1 CONV3x3, 2 UP (ConvTranspose2d k2 s2), 3 DOWN (Conv2d k2 s2), 4 PW (Conv2d 1x1)
   int f_stride, t_mul, t_off;  // implicit-GEMM addressing: tile f0 = blockIdx.x*f_stride, input row = t*t_mul + r + t_off
   int f_off;                   // first input pixel of a tile = f0 + f_off (CONV3x3: -8, so that the 112 outputs of a tile start 16-byte aligned)
-  int n_sbuf;                  // CONV3x3: output staging buffers per epilogue half (2 when shared memory allows)
   int b_resident;              // CONV3x3 with one weight tile that fits (Cin = Cout = 48: 83 KB): the whole B operand is loaded ONCE per CTA and the ring carries only A
   uint32_t b_res_off;          //   byte offset of the resident image [num_iters][hi | lo] from the start of dynamic shared memory (after alignment)
-  int cluster;                 // conv modes: CTAs per cluster walking tiles of the same weight tile in lockstep; each loads 1/cluster of every B stage and multicasts it
-  int n_tile, n_total, tmem_cols;
+  int n_tile, n_total;
   int num_iters, ksteps, stages;
-  int dbg;  // development switches from env B200SEP_DBG (0 in production): see launch()
-  int sleep_ns;  // > 0: waiting producer / epilogue warps sleep between polls (B200SEP_WAIT_SLEEP_NS)
+  int sleep_ns;  // > 0: the waiting producer sleeps between polls (B200SEP_WAIT_SLEEP_NS)
   int num_tiles, n_ftiles, t_tiles;  // persistent tile walk (n_tiles below = tiles along N / output channels)
   uint32_t a_bytes, b_bytes, stage_bytes;
   // CONV
-  int n_chunks, kc, T, F, Cin, Cout, n_tiles, n_c;  // n_c = output channels per CTA; n_tile = 3*n_c accumulator columns
+  int n_chunks, kc, T, F, Cin, Cout, n_tiles, n_c;  // n_c = output channels per CTA
   const bf16* wb_hi;
   const bf16* wb_lo;
   // GEMM
@@ -76,24 +72,17 @@ struct UmmaParams {
   int out_c_total, out_c_off;  // conv modes: the output occupies channels [out_c_off, out_c_off + Cout) of a (B, out_c_total, T', F') tensor
 };
 
-
-// activation of a whole register group with ONE test of the (kernel-uniform) activation code: inside the unrolled column loops the per-column
-// form cost a uniform branch (and, for GELU, an inlined erf with its own selects) per output
-template <int N>
-__device__ __forceinline__ void act_group(float (&x)[N], int act) {
-  if (act == 1) {
-#pragma unroll
-    for (int j = 0; j < N; ++j) x[j] = fmaxf(x[j], 0.f);
-  } else if (act == 2) {
-#pragma unroll
-    for (int j = 0; j < N; ++j) x[j] = 0.5f * x[j] * (1.f + erff(x[j] * 0.70710678118654752440f));
-  }
+__device__ __forceinline__ float act1(float x, int act) {
+  if (act == 1) return fmaxf(x, 0.f);
+  if (act == 2) return 0.5f * x * (1.f + erff(x * 0.70710678118654752440f));
+  return x;
 }
 
 __device__ __forceinline__ void split_store2(float v, bf16& hi, bf16& lo) {
   hi = __float2bfloat16_rn(v);
   lo = __float2bfloat16_rn(v - __bfloat162float(hi));
 }
+__device__ __forceinline__ float pair_at(const bf16* hi, const bf16* lo, size_t o) { return __bfloat162float(hi[o]) + __bfloat162float(lo[o]); }
 
 struct TileCoord {
   int m0, n_idx, f0, t, b;
@@ -139,44 +128,23 @@ __device__ __forceinline__ void umma_producer_loop(const CUtensorMap& tmA_hi, co
       uint8_t* a_lo = st + p.a_bytes;
       uint8_t* b_hi = st + 2 * p.a_bytes;
       uint8_t* b_lo = b_hi + p.b_bytes;
-      ptx::mbar_arrive_expect_tx(&full_bar[s], ((p.dbg & 8) ? 0 : 2 * p.a_bytes) + (((p.dbg & 16) || p.b_resident) ? 0 : 2 * p.b_bytes));
+      ptx::mbar_arrive_expect_tx(&full_bar[s], 2 * p.a_bytes + (p.b_resident ? 0 : 2 * p.b_bytes));
       if (p.mode == 0) {
         const int k0 = i * 64;
-        if (p.cluster > 1) {
-          // the CTAs of a cluster sit on the same 128 activation rows (consecutive weight tiles): this one fetches 128/cluster rows for all of them
-          // (tmA_* are then the maps with a [64 k][128/cluster rows] box; rows are 128 bytes, so a slice is whole 1024-byte swizzle atoms)
-          const uint32_t rows = 128u / (uint32_t)p.cluster, r0 = ptx::cluster_ctarank() * rows;
-          const uint16_t mask = (uint16_t)((1u << p.cluster) - 1u);
-          ptx::tma_load_2d_multicast(a_hi + r0 * 128u, &tmA_hi, &full_bar[s], k0, tc.m0 + (int)r0, mask);
-          ptx::tma_load_2d_multicast(a_lo + r0 * 128u, &tmA_lo, &full_bar[s], k0, tc.m0 + (int)r0, mask);
-        } else if (!(p.dbg & 8)) {
-          ptx::tma_load_2d(a_hi, &tmA_hi, &full_bar[s], k0, tc.m0);
-          ptx::tma_load_2d(a_lo, &tmA_lo, &full_bar[s], k0, tc.m0);
-        }
-        if (!(p.dbg & 16)) {
-          ptx::tma_load_2d(b_hi, &tmB_hi, &full_bar[s], k0, n0);
-          ptx::tma_load_2d(b_lo, &tmB_lo, &full_bar[s], k0, n0);
-        }
+        ptx::tma_load_2d(a_hi, &tmA_hi, &full_bar[s], k0, tc.m0);
+        ptx::tma_load_2d(a_lo, &tmA_lo, &full_bar[s], k0, tc.m0);
+        ptx::tma_load_2d(b_hi, &tmB_hi, &full_bar[s], k0, n0);
+        ptx::tma_load_2d(b_lo, &tmB_lo, &full_bar[s], k0, n0);
       } else {
         const int r = i / p.n_chunks, chunk = i - r * p.n_chunks;
         const int cf = tc.f0 + p.f_off, ct = tc.t * p.t_mul + r + p.t_off, cc = tc.b * p.Cin + chunk * p.kc;
         const uint32_t box = (uint32_t)p.kc * 128u;
-        if (!(p.dbg & 8)) {
-          ptx::tma_load_3d(a_hi, &tmA_hi, &full_bar[s], cf, ct, cc);
-          ptx::tma_load_3d(a_hi + box, &tmA_hi, &full_bar[s], cf + 64, ct, cc);
-          ptx::tma_load_3d(a_lo, &tmA_lo, &full_bar[s], cf, ct, cc);
-          ptx::tma_load_3d(a_lo + box, &tmA_lo, &full_bar[s], cf + 64, ct, cc);
-        }
-        const size_t woff = ((size_t)tc.n_idx * p.num_iters + i) * (size_t)(p.b_bytes / 2);
-        if (p.b_resident) {
-          // nothing to fetch: the weights are resident
-        } else if (p.cluster > 1) {
-          // the CTAs of a cluster are at the same (weight tile, iteration): this one fetches its 1/cluster share of the stage for all of them
-          const uint32_t slice = p.b_bytes / (uint32_t)p.cluster, off = ptx::cluster_ctarank() * slice;
-          const uint16_t mask = (uint16_t)((1u << p.cluster) - 1u);
-          ptx::bulk_load_1d_multicast(b_hi + off, p.wb_hi + woff + off / 2, slice, &full_bar[s], mask);
-          ptx::bulk_load_1d_multicast(b_lo + off, p.wb_lo + woff + off / 2, slice, &full_bar[s], mask);
-        } else if (!(p.dbg & 16)) {
+        ptx::tma_load_3d(a_hi, &tmA_hi, &full_bar[s], cf, ct, cc);
+        ptx::tma_load_3d(a_hi + box, &tmA_hi, &full_bar[s], cf + 64, ct, cc);
+        ptx::tma_load_3d(a_lo, &tmA_lo, &full_bar[s], cf, ct, cc);
+        ptx::tma_load_3d(a_lo + box, &tmA_lo, &full_bar[s], cf + 64, ct, cc);
+        if (!p.b_resident) {
+          const size_t woff = ((size_t)tc.n_idx * p.num_iters + i) * (size_t)(p.b_bytes / 2);
           ptx::bulk_load_1d(b_hi, p.wb_hi + woff, p.b_bytes, &full_bar[s]);
           ptx::bulk_load_1d(b_lo, p.wb_lo + woff, p.b_bytes, &full_bar[s]);
         }
@@ -189,72 +157,60 @@ __device__ __forceinline__ void umma_producer_loop(const CUtensorMap& tmA_hi, co
   }
 }
 
-// ===== MMA issuer (one thread): three bf16 UMMAs per k-step into one of two TMEM accumulators =====
-__device__ __forceinline__ void umma_mma_loop(const UmmaParams& p, uint8_t* smem, uint64_t* full_bar, uint64_t* empty_bar, uint64_t* tmem_full_bar,
-                                              uint64_t* tmem_empty_bar, uint32_t tmem_base, uint32_t acc_stride, uint64_t* wres_bar = nullptr) {
-  const uint32_t idesc = ptx::instr_desc_bf16(kTileM, p.n_tile, p.mode != 0 ? 1 : 0, 0);
-  if (p.b_resident) ptx::mbar_wait(wres_bar, 0, 500);  // the resident weight image has landed
-  int s = 0, acc = 0;
-  uint32_t phase = 0, acc_phase = 0;
-  for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-    ptx::mbar_wait(&tmem_empty_bar[acc], acc_phase ^ 1, 400 + acc);  // epilogue has drained this accumulator
-    ptx::tc_fence_after();
-    const uint32_t d_tmem = tmem_base + (uint32_t)acc * acc_stride;
-    for (int i = 0; i < p.num_iters; ++i) {
-      ptx::mbar_wait(&full_bar[s], phase, 200 + i);
-      ptx::tc_fence_after();
-      const uint32_t st = ptx::smem_u32(smem + (size_t)s * p.stage_bytes);
-      const uint32_t a_hi = st, a_lo = st + p.a_bytes;
-      const uint32_t b_hi = p.b_resident ? ptx::smem_u32(smem + p.b_res_off + (size_t)i * 2 * p.b_bytes) : st + 2 * p.a_bytes, b_lo = b_hi + p.b_bytes;
-      for (int j = 0; j < ((p.dbg & 4) ? 0 : p.ksteps); ++j) {
-        uint64_t dah, dal, dbh, dbl;
-        if (p.mode == 0) {
-          dah = ptx::smem_desc(a_hi + j * 32, 16, 1024, ptx::kLayoutSW128);
-          dal = ptx::smem_desc(a_lo + j * 32, 16, 1024, ptx::kLayoutSW128);
-          dbh = ptx::smem_desc(b_hi + j * 32, 16, 1024, ptx::kLayoutSW128);
-          dbl = ptx::smem_desc(b_lo + j * 32, 16, 1024, ptx::kLayoutSW128);
-        } else {
-          const uint32_t lbo = (uint32_t)p.kc * 128u;  // next 64 pixels (second TMA box)
-          dah = ptx::smem_desc(a_hi + j * 2048, lbo, 1024, ptx::kLayoutSW128);
-          dal = ptx::smem_desc(a_lo + j * 2048, lbo, 1024, ptx::kLayoutSW128);
-          const uint32_t bstep = (uint32_t)p.n_tile * 32u;  // one [n_tile][16] block of 8x8 core matrices
-          dbh = ptx::smem_desc(b_hi + j * bstep, 128, 256, ptx::kLayoutNone);
-          dbl = ptx::smem_desc(b_lo + j * bstep, 128, 256, ptx::kLayoutNone);
-        }
-        ptx::umma_bf16(d_tmem, dah, dbh, idesc, (i | j) != 0 ? 1u : 0u);
-        ptx::umma_bf16(d_tmem, dah, dbl, idesc, 1u);
-        ptx::umma_bf16(d_tmem, dal, dbh, idesc, 1u);
-      }
-      // frees the smem stage once these MMAs have read it -- in every CTA of the cluster when the stage was filled by multicast
-      if (p.cluster > 1) ptx::umma_commit_multicast(&empty_bar[s], (uint16_t)((1u << p.cluster) - 1u));
-      else ptx::umma_commit(&empty_bar[s]);
-      if (++s == p.stages) {
-        s = 0;
-        phase ^= 1;
-      }
+// ===== one tile's main loop of a consumer warpgroup =====
+// Per ring stage and 16-deep k-step, mma() issues the three products Ah*Bh + Ah*Bl + Al*Bh into the register accumulator.  A stage is released
+// (one arrive per consumer thread) when the wgmma group that read it has completed, one stage late, so the tensor core always has the next group queued.
+template <class Mma>
+__device__ __forceinline__ void consumer_mainloop(const UmmaParams& p, uint8_t* smem, uint64_t* full_bar, uint64_t* empty_bar, int& s, uint32_t& phase, Mma mma) {
+  int prev = -1;
+  for (int i = 0; i < p.num_iters; ++i) {
+    ptx::mbar_wait(&full_bar[s], phase, 200 + i);
+    const uint32_t st = ptx::smem_u32(smem + (size_t)s * p.stage_bytes);
+    const uint32_t a_hi = st, a_lo = st + p.a_bytes;
+    const uint32_t b_hi = p.b_resident ? ptx::smem_u32(smem + p.b_res_off + (size_t)i * 2 * p.b_bytes) : st + 2 * p.a_bytes, b_lo = b_hi + p.b_bytes;
+    ptx::wgmma_fence();
+    for (int j = 0; j < p.ksteps; ++j) mma(a_hi, a_lo, b_hi, b_lo, j, (i | j) != 0 ? 1 : 0);
+    ptx::wgmma_commit();
+    ptx::wgmma_wait<1>();
+    if (prev >= 0) ptx::mbar_arrive(&empty_bar[prev]);
+    prev = s;
+    if (++s == p.stages) {
+      s = 0;
+      phase ^= 1;
     }
-    ptx::umma_commit(&tmem_full_bar[acc]);
-    acc ^= 1;
-    if (acc == 0) acc_phase ^= 1;
   }
+  ptx::wgmma_wait<0>();
+  if (prev >= 0) ptx::mbar_arrive(&empty_bar[prev]);
 }
 
-// Persistent kernel: grid = min(#tiles, #SMs); every CTA walks tiles blockIdx.x, +gridDim.x, ...  Three pipelines run
-// concurrently: TMA producer -> smem ring (full/empty mbarriers, continuous across tiles), MMA issuer -> one of two TMEM
-// accumulators (tmem_full/tmem_empty), epilogue warps draining the other accumulator.
+// A operand descriptors of consumer warpgroup wg (rows 64*wg..): GEMM = K-major 128-byte-swizzled rows of 64 k; conv modes = the two TMA boxes of
+// 64 pixels (MN-major, pixels contiguous), box wg; k-step j
+__device__ __forceinline__ uint64_t a_desc(const UmmaParams& p, uint32_t a, int wg, int j) {
+  if (p.mode == 0) return ptx::smem_desc(a + (uint32_t)wg * 8192u + (uint32_t)j * 32u, 16, 1024, ptx::kLayoutSW128);
+  const uint32_t lbo = (uint32_t)p.kc * 128u;
+  return ptx::smem_desc(a + (uint32_t)wg * lbo + (uint32_t)j * 2048u, lbo, 1024, ptx::kLayoutSW128);
+}
+// B operand: GEMM = K-major swizzled rows of 64 k; conv modes = one [n_tile][16] block of 8x8 core matrices per k-step
+__device__ __forceinline__ uint64_t b_desc(const UmmaParams& p, uint32_t b, int j) {
+  if (p.mode == 0) return ptx::smem_desc(b + (uint32_t)j * 32u, 16, 1024, ptx::kLayoutSW128);
+  return ptx::smem_desc(b + (uint32_t)j * (uint32_t)p.n_tile * 32u, 128, 256, ptx::kLayoutNone);
+}
+
+// Persistent kernel: grid = min(#tiles, #SMs); every CTA walks tiles blockIdx.x, +gridDim.x, ...  The producer warp keeps the shared-memory ring
+// (full/empty mbarriers) filled across tiles while the two consumer warpgroups multiply (wgmma, fp32 accumulators in registers) and run the
+// epilogue straight from their accumulator fragments.
+// Accumulator column layouts (the weight blocking below produces them): GEMM n; UP co*4 + (dy*2 + dx); DOWN co*2 + dx; PW co -- so the
+// columns a thread holds in one register pair (2c, 2c + 1) always belong together.
 __global__ void __launch_bounds__(kUmmaThreads, 1) umma_pair_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
                                                                     const __grid_constant__ CUtensorMap tmB_hi, const __grid_constant__ CUtensorMap tmB_lo,
                                                                     const UmmaParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // 1024-byte alignment for SWIZZLE_128B tiles.  The offset is applied to the __shared__ array itself (not through an integer
-  // round trip) so every derived pointer keeps the shared address space: LDS/STS instead of generic LD/ST in the epilogue.
+  // round trip) so every derived pointer keeps the shared address space.
   uint8_t* smem = smem_raw + ((1024u - (ptx::smem_u32(smem_raw) & 1023u)) & 1023u);
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + (size_t)p.stages * p.stage_bytes);
   uint64_t* empty_bar = full_bar + p.stages;
-  uint64_t* tmem_full_bar = empty_bar + p.stages;  // [2]
-  uint64_t* tmem_empty_bar = tmem_full_bar + 2;    // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_empty_bar + 2);
-  float* sc_s = reinterpret_cast<float*>(tmem_slot + 4);  // conv modes: folded BatchNorm scale / shift per output channel
+  float* sc_s = reinterpret_cast<float*>(empty_bar + p.stages + 2);  // conv modes: folded BatchNorm scale / shift per output channel
   float* sh_s = sc_s + kMaxChannels;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -262,11 +218,7 @@ __global__ void __launch_bounds__(kUmmaThreads, 1) umma_pair_kernel(const __grid
   if (threadIdx.x == 0) {
     for (int s = 0; s < p.stages; ++s) {
       ptx::mbar_init(&full_bar[s], 1);
-      ptx::mbar_init(&empty_bar[s], p.cluster > 1 ? p.cluster : 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      ptx::mbar_init(&tmem_full_bar[a], 1);
-      ptx::mbar_init(&tmem_empty_bar[a], 4 * kEpiParts);  // one arrive per epilogue warp
+      ptx::mbar_init(&empty_bar[s], kConsumerThreads);
     }
     ptx::fence_barrier_init();
     ptx::prefetch_tensormap(&tmA_hi);
@@ -276,326 +228,198 @@ __global__ void __launch_bounds__(kUmmaThreads, 1) umma_pair_kernel(const __grid
       ptx::prefetch_tensormap(&tmB_lo);
     }
   }
-  if (warp == 1) ptx::tmem_alloc(tmem_slot, (uint32_t)p.tmem_cols);
   if (p.mode != 0) {
     for (int i = threadIdx.x; i < p.Cout; i += blockDim.x) {
       sc_s[i] = p.scale ? __ldg(&p.scale[i]) : 1.f;
       sh_s[i] = p.shift ? __ldg(&p.shift[i]) : 0.f;
     }
   }
-  ptx::tc_fence_before();
   __syncthreads();
-  if (p.cluster > 1) ptx::cluster_sync();  // every CTA's barriers exist before a peer multicasts into them
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t acc_stride = (uint32_t)p.tmem_cols / 2;
 
-  if (warp == 0) {
+  if (warp == kConsumerThreads / 32) {
     if (lane == 0) umma_producer_loop(tmA_hi, tmA_lo, tmB_hi, tmB_lo, p, smem, full_bar, empty_bar);
-  } else if (warp == 1) {
-    if (lane == 0) umma_mma_loop(p, smem, full_bar, empty_bar, tmem_full_bar, tmem_empty_bar, tmem_base, acc_stride);
-  } else {
-    // ===== epilogue: TMEM -> registers -> BN/ReLU(/+res, *skip) -> split into bf16 hi/lo -> global =====
-    // Eight warps: warp w may only touch TMEM lanes 32*(w%4)..+31, so two warps share each lane quadrant and split
-    // the accumulator columns between them (two warps per scheduler also hide the ALU latency of the conversion chain).
-    const int q = warp & 3;
-    const int half = (warp - 2) >> 2;
-    const int m = q * 32 + lane;
-    const int ncol = (p.mode == 0) ? p.n_tile : p.n_c;  // columns of ONE logical output group
-    // GEMM: 16-column groups; conv modes: 8-column groups (n_c = 48 splits 24/24 between the two warps of a quadrant)
-    const int cw = (p.mode == 0) ? 16 : 8;
-    const int nchunks = ncol / cw;
-    const int ch_begin = half * nchunks / kEpiParts, ch_end = (half + 1) * nchunks / kEpiParts;  // `half` = which of the kEpiParts column parts
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-      const TileCoord tc = decode_tile(p, tile);
-      const int m0 = tc.m0, f0 = tc.f0, t = tc.t, b = tc.b;
-      const int n0 = tc.n_idx * ncol;
-      // GEMM: the residual does not depend on the accumulator -> fetch it while the MMAs of this tile are still running
-      uint4 rh[4][2], rl[4][2];
-      if (p.mode == 0 && p.res_hi && !(p.dbg & 1)) {
-        const int r = m0 + m;
+    return;
+  }
+  const int wg = warp >> 2, g = lane >> 2, cq = lane & 3;
+  const int mrow0 = wg * 64 + (warp & 3) * 16 + g;  // tile rows of this thread: mrow0 and mrow0 + 8
+  int s = 0;
+  uint32_t phase = 0;
+  float acc[kMaxNTile / 2];
+  for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+    const TileCoord tc = decode_tile(p, tile);
+    if (p.mode == 0) {
+      consumer_mainloop(p, smem, full_bar, empty_bar, s, phase, [&](uint32_t ah, uint32_t al, uint32_t bh, uint32_t bl, int j, int accum) {
+        const uint64_t dah = a_desc(p, ah, wg, j), dal = a_desc(p, al, wg, j), dbh = b_desc(p, bh, j), dbl = b_desc(p, bl, j);
+        ptx::wgmma_ss<0>(p.n_tile, acc, dah, dbh, accum);
+        ptx::wgmma_ss<0>(p.n_tile, acc, dah, dbl, 1);
+        ptx::wgmma_ss<0>(p.n_tile, acc, dal, dbh, 1);
+      });
+    } else {
+      consumer_mainloop(p, smem, full_bar, empty_bar, s, phase, [&](uint32_t ah, uint32_t al, uint32_t bh, uint32_t bl, int j, int accum) {
+        const uint64_t dah = a_desc(p, ah, wg, j), dal = a_desc(p, al, wg, j), dbh = b_desc(p, bh, j), dbl = b_desc(p, bl, j);
+        ptx::wgmma_ss<1>(p.n_tile, acc, dah, dbh, accum);
+        ptx::wgmma_ss<1>(p.n_tile, acc, dah, dbl, 1);
+        ptx::wgmma_ss<1>(p.n_tile, acc, dal, dbh, 1);
+      });
+    }
+    ptx::fence_regs(acc);
+
+    // ===== epilogue: accumulator fragments -> BN/act(/+res, *skip) -> split into bf16 hi/lo -> global =====
+    if (p.mode == 0) {
+      const int n0 = tc.n_idx * p.n_tile;
+      float sc[2], sh[2];
 #pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          const int n = n0 + (ch_begin + k) * 16;
-          if (ch_begin + k < ch_end && r < p.M && n < p.n_total) {
-            const size_t o = (size_t)r * p.n_total + n;
-            rh[k][0] = __ldg(reinterpret_cast<const uint4*>(p.res_hi + o));
-            rh[k][1] = __ldg(reinterpret_cast<const uint4*>(p.res_hi + o) + 1);
-            rl[k][0] = __ldg(reinterpret_cast<const uint4*>(p.res_lo + o));
-            rl[k][1] = __ldg(reinterpret_cast<const uint4*>(p.res_lo + o) + 1);
+      for (int h = 0; h < 2; ++h) {
+        const int r = tc.m0 + mrow0 + 8 * h;
+        sc[h] = 1.f;
+        sh[h] = 0.f;
+        if (r < p.M) {
+          const int c = (r / p.rows_per_channel) % p.channels;
+          sc[h] = p.scale ? __ldg(&p.scale[c]) : 1.f;
+          sh[h] = p.shift ? __ldg(&p.shift[c]) : 0.f;
+        }
+      }
+#pragma unroll
+      for (int i = 0; i < kMaxNTile / 8; ++i) {
+        if (8 * i >= p.n_tile) break;
+        const int n = n0 + 8 * i + 2 * cq;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int r = tc.m0 + mrow0 + 8 * h;
+          if (r >= p.M) continue;
+          const size_t o = (size_t)r * p.n_total + n;
+          float y0 = act1(fmaf(acc[4 * i + 2 * h], sc[h], sh[h]), p.act), y1 = act1(fmaf(acc[4 * i + 2 * h + 1], sc[h], sh[h]), p.act);
+          if (p.res_hi) {
+            y0 += pair_at(p.res_hi, p.res_lo, o);
+            y1 += pair_at(p.res_hi, p.res_lo, o + 1);
+          }
+          __nv_bfloat162 oh, ol;
+          split_store2(y0, oh.x, ol.x);
+          split_store2(y1, oh.y, ol.y);
+          *reinterpret_cast<__nv_bfloat162*>(p.out_hi + o) = oh;
+          *reinterpret_cast<__nv_bfloat162*>(p.out_lo + o) = ol;
+        }
+      }
+    } else if (p.mode == 2) {
+      // ConvTranspose2d k2 s2: the register pair (col, col + 1), col = co*4 + dy*2, holds output pixels (2t+dy, 2f) and (2t+dy, 2f+1) of channel co,
+      // f = f0 + row; then BN + ReLU, times the skip tensor (uvr_lib_v5/mdxnet.py:111-112), stored as one 4-byte pair per plane.
+      const int c0 = tc.n_idx * p.n_c;
+      const int T2 = 2 * p.T, F2 = 2 * p.F;
+      const size_t plane = (size_t)T2 * F2;
+#pragma unroll
+      for (int i = 0; i < kMaxNTile / 8; ++i) {
+        if (8 * i >= p.n_tile) break;
+        const int col = 8 * i + 2 * cq, co = c0 + (col >> 2), dy = (col >> 1) & 1;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int f = tc.f0 + mrow0 + 8 * h;
+          if (f >= p.F) continue;
+          const size_t pix = (size_t)(2 * tc.t + dy) * F2 + 2 * f;
+          const size_t o = ((size_t)tc.b * p.out_c_total + p.out_c_off + co) * plane + pix;
+          float x0 = act1(fmaf(acc[4 * i + 2 * h], sc_s[co], sh_s[co]), p.act), x1 = act1(fmaf(acc[4 * i + 2 * h + 1], sc_s[co], sh_s[co]), p.act);
+          if (p.res_hi) {  // skip tensor: own channel count; bf16 -> fp32 is a 16-bit shift: low half = dx 0, high half = dx 1
+            const size_t so = ((size_t)tc.b * p.Cout + co) * plane + pix;
+            const uint32_t sk_h = __ldg(reinterpret_cast<const unsigned int*>(p.res_hi + so)), sk_l = __ldg(reinterpret_cast<const unsigned int*>(p.res_lo + so));
+            x0 *= __uint_as_float(sk_h << 16) + __uint_as_float(sk_l << 16);
+            x1 *= __uint_as_float(sk_h & 0xffff0000u) + __uint_as_float(sk_l & 0xffff0000u);
+          }
+          __nv_bfloat162 oh, ol;
+          split_store2(x0, oh.x, ol.x);
+          split_store2(x1, oh.y, ol.y);
+          *reinterpret_cast<__nv_bfloat162*>(p.out_hi + o) = oh;
+          *reinterpret_cast<__nv_bfloat162*>(p.out_lo + o) = ol;
+        }
+      }
+    } else if (p.mode == 3) {
+      // Conv2d k2 s2: the register pair (col, col + 1), col = co*2, holds P_0 and P_1 of channel co, the partial sums over (ci, dy) at INPUT pixel
+      // f0 + row; out[(f0+row)/2] = P_0[row] + P_1[row+1] for even rows (row + 1 is lane + 4: same register, same warp).
+      const int c0 = tc.n_idx * p.n_c;
+      const int Fo = p.F >> 1, To = p.T >> 1;
+      const size_t plane = (size_t)To * Fo;
+#pragma unroll
+      for (int i = 0; i < kMaxNTile / 8; ++i) {
+        if (8 * i >= p.n_tile) break;
+        const int co = c0 + 4 * i + cq;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const float p1 = __shfl_down_sync(0xffffffffu, acc[4 * i + 2 * h + 1], 4);
+          const int fo = (tc.f0 + mrow0 + 8 * h) >> 1;
+          if ((g & 1) == 0 && fo < Fo) {
+            const float y = act1(fmaf(acc[4 * i + 2 * h] + p1, sc_s[co], sh_s[co]), p.act);
+            const size_t o = ((size_t)tc.b * p.out_c_total + p.out_c_off + co) * plane + (size_t)tc.t * Fo + fo;
+            split_store2(y, p.out_hi[o], p.out_lo[o]);
           }
         }
       }
-      ptx::mbar_wait_opt(&tmem_full_bar[acc], acc_phase, p.sleep_ns, 300 + acc);
-      ptx::tc_fence_after();
-      const uint32_t trow = tmem_base + (uint32_t)acc * acc_stride + ((uint32_t)(q * 32) << 16);
-      if (p.dbg & 32) {
-        // development: handshake only
-      } else if (p.mode == 0) {
-        const int r = m0 + m;
-        float sc = 1.f, sh = 0.f;
-        if (r < p.M) {
-          const int c = (r / p.rows_per_channel) % p.channels;
-          sc = p.scale ? __ldg(&p.scale[c]) : 1.f;
-          sh = p.shift ? __ldg(&p.shift[c]) : 0.f;
-        }
+    } else if (p.mode == 4) {
+      // 1x1 convolution: column co is channel c0 + co at output pixel f0 + row
+      const int c0 = tc.n_idx * p.n_c;
+      const size_t plane = (size_t)p.T * p.F;
 #pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          const int ch = ch_begin + k;
-          if (ch >= ch_end) break;
-          const int c0 = ch * 16;
-          uint32_t v[16];
-          ptx::tmem_ld16(trow + (uint32_t)c0, v);
-          ptx::tmem_ld_wait();
-          const int n = n0 + c0;
-          if (r < p.M && n < p.n_total) {
-            const size_t o = (size_t)r * p.n_total + n;
-            float x[16];
+      for (int i = 0; i < kMaxNTile / 8; ++i) {
+        if (8 * i >= p.n_tile) break;
 #pragma unroll
-            for (int j = 0; j < 16; ++j) x[j] = fmaf(__uint_as_float(v[j]), sc, sh);
-            act_group(x, p.act);
-            if (p.res_hi && !(p.dbg & 1)) {
-              const bf16* h = reinterpret_cast<const bf16*>(rh[k]);
-              const bf16* l = reinterpret_cast<const bf16*>(rl[k]);
+        for (int h = 0; h < 2; ++h) {
+          const int f = tc.f0 + mrow0 + 8 * h;
+          if (f >= p.F) continue;
 #pragma unroll
-              for (int j = 0; j < 16; ++j) x[j] += __bfloat162float(h[j]) + __bfloat162float(l[j]);
-            }
-            __align__(16) bf16 oh[16];
-            __align__(16) bf16 ol[16];
-#pragma unroll
-            for (int j = 0; j < 16; ++j) split_store2(x[j], oh[j], ol[j]);
-            uint4* dh = reinterpret_cast<uint4*>(p.out_hi + o);
-            uint4* dl = reinterpret_cast<uint4*>(p.out_lo + o);
-            dh[0] = reinterpret_cast<const uint4*>(oh)[0];
-            dh[1] = reinterpret_cast<const uint4*>(oh)[1];
-            dl[0] = reinterpret_cast<const uint4*>(ol)[0];
-            dl[1] = reinterpret_cast<const uint4*>(ol)[1];
+          for (int e = 0; e < 2; ++e) {
+            const int co = c0 + 8 * i + 2 * cq + e;
+            float y = act1(fmaf(acc[4 * i + 2 * h + e], sc_s[co], sh_s[co]), p.act);
+            const size_t ro = ((size_t)tc.b * p.Cout + co) * plane + (size_t)tc.t * p.F + f;
+            if (p.res_hi) y += pair_at(p.res_hi, p.res_lo, ro);
+            if (p.mul_hi) y *= pair_at(p.mul_hi, p.mul_lo, ro);
+            const size_t o = ((size_t)tc.b * p.out_c_total + p.out_c_off + co) * plane + (size_t)tc.t * p.F + f;
+            if (p.out_f32) p.out_f32[o] = y;
+            else split_store2(y, p.out_hi[o], p.out_lo[o]);
           }
         }
-      } else if (p.mode == 2) {
-        // ConvTranspose2d k2 s2: column (dy*2+dx)*n_c + co of lane m is the output pixel (2t+dy, 2(f0+m)+dx) of channel co;
-        // then BN + ReLU, times the skip tensor (uvr_lib_v5/mdxnet.py:111-112).  The two dx values are stored as one 4-byte pair.
-        constexpr int CW = 8;
-        const int nc = p.n_c;
-        const int f = f0 + m;
-        const bool row_ok = f < p.F;
-        const int T2 = 2 * p.T, F2 = 2 * p.F;
-        const size_t plane = (size_t)T2 * F2;
-        for (int dy = 0; dy < 2; ++dy) {
-          const size_t base = ((size_t)b * p.out_c_total + p.out_c_off + n0) * plane + (size_t)(2 * t + dy) * F2 + 2 * f;
-          const size_t sbase = ((size_t)b * p.Cout + n0) * plane + (size_t)(2 * t + dy) * F2 + 2 * f;  // skip tensor: own channel count
-          for (int ch = ch_begin; ch < ch_end; ++ch) {
-            const int c0 = ch * CW;
-            uint32_t v0[CW], v1[CW];
-            ptx::tmem_ld8(trow + (uint32_t)((dy * 2 + 0) * nc + c0), v0);
-            ptx::tmem_ld8(trow + (uint32_t)((dy * 2 + 1) * nc + c0), v1);
-            ptx::tmem_ld_wait();
-            if (row_ok) {
-              const size_t o0 = base + (size_t)c0 * plane, s0 = sbase + (size_t)c0 * plane;
-              // all skip loads of this group are issued before any store (read-only path)
-              uint32_t sk_h[CW], sk_l[CW];
-#pragma unroll
-              for (int j = 0; j < CW; ++j) {
-                sk_h[j] = 0x3f803f80u;  // bf16 (1.0, 1.0)
-                sk_l[j] = 0u;
-                if (p.res_hi && !(p.dbg & 1)) {
-                  sk_h[j] = __ldg(reinterpret_cast<const unsigned int*>(p.res_hi + s0 + (size_t)j * plane));
-                  sk_l[j] = __ldg(reinterpret_cast<const unsigned int*>(p.res_lo + s0 + (size_t)j * plane));
-                }
-              }
-              float scv[CW], shv[CW];
-#pragma unroll
-              for (int j4 = 0; j4 < CW / 4; ++j4) {
-                const float4 s4 = *reinterpret_cast<const float4*>(&sc_s[n0 + c0 + 4 * j4]);
-                const float4 h4 = *reinterpret_cast<const float4*>(&sh_s[n0 + c0 + 4 * j4]);
-                scv[4 * j4] = s4.x; scv[4 * j4 + 1] = s4.y; scv[4 * j4 + 2] = s4.z; scv[4 * j4 + 3] = s4.w;
-                shv[4 * j4] = h4.x; shv[4 * j4 + 1] = h4.y; shv[4 * j4 + 2] = h4.z; shv[4 * j4 + 3] = h4.w;
-              }
-              bf16* ph = p.out_hi + o0;
-              bf16* pl = p.out_lo + o0;
-              float xa[CW], xb[CW];
-#pragma unroll
-              for (int j = 0; j < CW; ++j) {
-                xa[j] = fmaf(__uint_as_float(v0[j]), scv[j], shv[j]);
-                xb[j] = fmaf(__uint_as_float(v1[j]), scv[j], shv[j]);
-              }
-              act_group(xa, p.act);
-              act_group(xb, p.act);
-#pragma unroll
-              for (int j = 0; j < CW; ++j) {
-                // bf16 -> fp32 is a 16-bit shift: low half = element 0 (dx = 0), high half = element 1 (dx = 1)
-                float x0 = xa[j] * (__uint_as_float(sk_h[j] << 16) + __uint_as_float(sk_l[j] << 16));
-                float x1 = xb[j] * (__uint_as_float(sk_h[j] & 0xffff0000u) + __uint_as_float(sk_l[j] & 0xffff0000u));
-                __nv_bfloat162 oh, ol;
-                split_store2(x0, oh.x, ol.x);
-                split_store2(x1, oh.y, ol.y);
-                *reinterpret_cast<__nv_bfloat162*>(ph) = oh;  // 32 lanes -> 128 contiguous bytes
-                *reinterpret_cast<__nv_bfloat162*>(pl) = ol;
-                ph += plane;
-                pl += plane;
-              }
-            }
-          }
-        }
-      } else if (p.mode == 3) {
-        // Conv2d k2 s2: P_dx[m] (column dx*n_c + co) is the partial sum over (ci, dy) at INPUT pixel f0+m;
-        // out[(f0+m)/2] = P_0[m] + P_1[m+1] for even m (odd rows of P_0 / even rows of P_1 are computed but unused).
-        constexpr int CW = 8;
-        const int nc = p.n_c;
-        const int fo = (f0 + m) >> 1, Fo = p.F >> 1, To = p.T >> 1;
-        const bool row_ok = ((m & 1) == 0) && fo < Fo;
-        const size_t plane = (size_t)To * Fo;
-        const size_t base = ((size_t)b * p.out_c_total + p.out_c_off + n0) * plane + (size_t)t * Fo + fo;
-        for (int ch = ch_begin; ch < ch_end; ++ch) {
-          const int c0 = ch * CW;
-          uint32_t v0[CW], v1[CW];
-          ptx::tmem_ld8(trow + (uint32_t)c0, v0);
-          ptx::tmem_ld8(trow + (uint32_t)(nc + c0), v1);
-          ptx::tmem_ld_wait();
-          float x[CW];
-#pragma unroll
-          for (int j = 0; j < CW; ++j) x[j] = __uint_as_float(v0[j]) + __shfl_down_sync(0xffffffffu, __uint_as_float(v1[j]), 1);  // + P_1 of row m+1
-          float sc[CW], sh[CW];
-#pragma unroll
-          for (int j4 = 0; j4 < CW / 4; ++j4) {
-            const float4 s4 = *reinterpret_cast<const float4*>(&sc_s[n0 + c0 + 4 * j4]);
-            const float4 h4 = *reinterpret_cast<const float4*>(&sh_s[n0 + c0 + 4 * j4]);
-            sc[4 * j4] = s4.x; sc[4 * j4 + 1] = s4.y; sc[4 * j4 + 2] = s4.z; sc[4 * j4 + 3] = s4.w;
-            sh[4 * j4] = h4.x; sh[4 * j4 + 1] = h4.y; sh[4 * j4 + 2] = h4.z; sh[4 * j4 + 3] = h4.w;
-          }
-          if (row_ok) {
-            bf16* ph = p.out_hi + base + (size_t)c0 * plane;
-            bf16* pl = p.out_lo + base + (size_t)c0 * plane;
-            float y[CW];
-#pragma unroll
-            for (int j = 0; j < CW; ++j) y[j] = fmaf(x[j], sc[j], sh[j]);
-            act_group(y, p.act);
-#pragma unroll
-            for (int j = 0; j < CW; ++j) {
-              bf16 h, l;
-              split_store2(y[j], h, l);
-              *ph = h;
-              *pl = l;
-              ph += plane;
-              pl += plane;
-            }
-          }
-        }
-      } else if (p.mode == 4) {
-        // 1x1 convolution: column co of lane m is output pixel f0+m of channel n0+co.
-        constexpr int CW = 8;
-        const int f = f0 + m;
-        const bool row_ok = f < p.F;
-        const size_t plane = (size_t)p.T * p.F;
-        const size_t base = ((size_t)b * p.out_c_total + p.out_c_off + n0) * plane + (size_t)t * p.F + f;
-        const size_t rbase = ((size_t)b * p.Cout + n0) * plane + (size_t)t * p.F + f;
-        for (int ch = ch_begin; ch < ch_end; ++ch) {
-          const int c0 = ch * CW;
-          uint32_t v[CW];
-          ptx::tmem_ld8(trow + (uint32_t)c0, v);
-          ptx::tmem_ld_wait();
-          float sc[CW], sh[CW];
-#pragma unroll
-          for (int j4 = 0; j4 < CW / 4; ++j4) {
-            const float4 s4 = *reinterpret_cast<const float4*>(&sc_s[n0 + c0 + 4 * j4]);
-            const float4 h4 = *reinterpret_cast<const float4*>(&sh_s[n0 + c0 + 4 * j4]);
-            sc[4 * j4] = s4.x; sc[4 * j4 + 1] = s4.y; sc[4 * j4 + 2] = s4.z; sc[4 * j4 + 3] = s4.w;
-            sh[4 * j4] = h4.x; sh[4 * j4 + 1] = h4.y; sh[4 * j4 + 2] = h4.z; sh[4 * j4 + 3] = h4.w;
-          }
-          if (row_ok) {
-            float y[CW];
-#pragma unroll
-            for (int j = 0; j < CW; ++j) y[j] = fmaf(__uint_as_float(v[j]), sc[j], sh[j]);
-            act_group(y, p.act);
-            if (p.res_hi) {
-#pragma unroll
-              for (int j = 0; j < CW; ++j) {
-                const size_t ro = rbase + (size_t)(c0 + j) * plane;
-                y[j] += __bfloat162float(p.res_hi[ro]) + __bfloat162float(p.res_lo[ro]);
-              }
-            }
-            if (p.mul_hi) {
-#pragma unroll
-              for (int j = 0; j < CW; ++j) {
-                const size_t ro = rbase + (size_t)(c0 + j) * plane;
-                y[j] *= __bfloat162float(p.mul_hi[ro]) + __bfloat162float(p.mul_lo[ro]);
-              }
-            }
-            if (p.out_f32) {
-#pragma unroll
-              for (int j = 0; j < CW; ++j) p.out_f32[base + (size_t)(c0 + j) * plane] = y[j];
-            } else {
-#pragma unroll
-              for (int j = 0; j < CW; ++j) {
-                const size_t o = base + (size_t)(c0 + j) * plane;
-                bf16 h, l;
-                split_store2(y[j], h, l);
-                p.out_hi[o] = h;
-                p.out_lo[o] = l;
-              }
-            }
-          }
-        }
-      }  // (CONV3x3 has its own kernel, umma_conv3_kernel)
-      // this warp is done reading the accumulator: hand it back to the MMA issuer
-      ptx::tc_fence_before();
-      __syncwarp();
-      if (lane == 0) ptx::mbar_arrive(&tmem_empty_bar[acc]);
-      acc ^= 1;
-      if (acc == 0) acc_phase ^= 1;
-    }
-  }
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (p.cluster > 1) ptx::cluster_sync();  // no CTA leaves while a peer may still signal its barriers
-  if (warp == 1) {
-    ptx::tc_fence_after();
-    ptx::tmem_dealloc(tmem_base, (uint32_t)p.tmem_cols);
+      }
+    }  // (CONV3x3 has its own kernel, umma_conv3_kernel)
   }
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// CONV3x3 kernel.  Same producer / MMA pipelines as umma_pair_kernel; the epilogue is specialised (NC = output channels per CTA):
+// CONV3x3 kernel (NC = output channels per CTA).  Same producer / ring as umma_pair_kernel; accumulator column dx*NC + co holds
+// P_dx[row] = W[dy][dx] . x[f0 - 8 + row] summed over (ci, dy), and the epilogue forms out[j] = P_0[j-1] + P_1[j] + P_2[j+1]:
 //   * a tile loads the 128 pixels [f0 - 8, f0 + 120) (TMA zero-fills the left / right padding) and produces the 112 outputs
-//     [f0, f0 + 112) = TMEM rows 8..119, so both the loads and the STORES start 16-byte aligned (TMA faults on any other
-//     innermost coordinate, measured: tests/dev/tma_probe2.cu);
-//   * each of the 8 epilogue warps pulls ALL its accumulator columns (3 * NC/2) into registers with one tcgen05.wait::ld and
-//     hands the accumulator back to the MMA issuer at once -- the arithmetic below overlaps the next tiles' MMAs;
-//   * out[j] = P_0[j-1] + P_1[j] + P_2[j+1] by warp shuffles, the three warp-boundary rows through a 128-thread exchange
-//     (no second pass over TMEM), folded BatchNorm + activation (+ residual, * multiplier), bf16 hi/lo split;
-//   * the tile is staged in shared memory as [channel][pixel] bf16 planes and written with two cp.async.bulk.tensor stores per half
-//     (UTMASTG): no per-thread global stores, no 64-bit address arithmetic, full 224-byte rows per channel.
+//     [f0, f0 + 112) = rows 8..119, so both the loads and the STORES start 16-byte aligned (TMA faults on any other innermost coordinate);
+//   * row +-1 of a fragment row is lane +-4 (warp shuffles); the rows across a warp boundary go through a small shared-memory exchange;
+//   * folded BatchNorm + activation (+ residual, * multiplier), bf16 hi/lo split, staged in shared memory as [channel][pixel] planes
+//     and written with one cp.async.bulk.tensor store per plane: full 224-byte rows per channel.
 template <int NC>
-__global__ void __launch_bounds__(kConv3Threads, 1) umma_conv3_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
+__device__ __forceinline__ void conv3_mma(float (&acc)[3 * NC / 2], uint64_t da, uint64_t db, int accum) {
+  if constexpr (NC == 16) ptx::wgmma_ss_n48<1>(acc, da, db, accum);
+  else if constexpr (NC == 32) ptx::wgmma_ss_n96<1>(acc, da, db, accum);
+  else if constexpr (NC == 48) ptx::wgmma_ss_n144<1>(acc, da, db, accum);
+  else if constexpr (NC == 64) ptx::wgmma_ss_n192<1>(acc, da, db, accum);
+  else ptx::wgmma_ss_n240<1>(acc, da, db, accum);
+}
+
+template <int NC>
+__global__ void __launch_bounds__(kUmmaThreads, 1) umma_conv3_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
                                                                      const __grid_constant__ CUtensorMap tmO_hi, const __grid_constant__ CUtensorMap tmO_lo,
                                                                      const UmmaParams p) {
-  constexpr int H = NC / kConv3Parts;       // channels per epilogue warp
-  constexpr int kPlane = H * kConvStride;   // bf16 elements of one staged plane [H][112]
+  constexpr int kPlane = NC * kConvStride;  // bf16 elements of one staged plane [NC][112]
+  constexpr int G = NC / 8;                 // 8-column groups per dx
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (ptx::smem_u32(smem_raw) & 1023u)) & 1023u);
-  // [ring: stages x stage_bytes][resident weights, when b_resident][output staging][barriers, BN coefficients, edge rows]
-  bf16* stage_out = reinterpret_cast<bf16*>(smem + (size_t)p.stages * p.stage_bytes + (p.b_resident ? (size_t)2 * p.b_bytes * p.num_iters : 0));  // [n_sbuf][parts][hi, lo][H][112]
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(stage_out) + (size_t)p.n_sbuf * 2 * kConv3Parts * kPlane * sizeof(bf16));
+  // [ring: stages x stage_bytes][resident weights, when b_resident][output staging hi | lo][barriers][BN coefficients][edge rows]
+  bf16* s_hi = reinterpret_cast<bf16*>(smem + (size_t)p.stages * p.stage_bytes + (p.b_resident ? (size_t)2 * p.b_bytes * p.num_iters : 0));
+  bf16* s_lo = s_hi + kPlane;
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(s_lo + kPlane);
   uint64_t* empty_bar = full_bar + p.stages;
-  uint64_t* tmem_full_bar = empty_bar + p.stages;  // [2]
-  uint64_t* tmem_empty_bar = tmem_full_bar + 2;    // [2]
-  uint64_t* wres_bar = tmem_empty_bar + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(wres_bar + 2);  // (+2: keeps everything behind it 16-byte aligned -- sc_s / sh_s / the edge rows are read as float4)
-  float* sc_s = reinterpret_cast<float*>(tmem_slot + 4);
+  uint64_t* wres_bar = empty_bar + p.stages;
+  float* sc_s = reinterpret_cast<float*>(wres_bar + 2);
   float* sh_s = sc_s + kMaxChannels;
-  float* edge_base = sh_s + kMaxChannels;  // [kConv3Parts][P_0 row 31 | P_2 row 0][4 quadrants][H]
+  float* edge0 = sh_s + kMaxChannels;  // [8 warps][NC]: P_0 of the warp's last row (row 16w + 15)
+  float* edge2 = edge0 + 8 * NC;       // [8 warps][NC]: P_2 of the warp's first row (row 16w)
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
     for (int s = 0; s < p.stages; ++s) {
       ptx::mbar_init(&full_bar[s], 1);
-      ptx::mbar_init(&empty_bar[s], p.cluster > 1 ? p.cluster : 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      ptx::mbar_init(&tmem_full_bar[a], 1);
-      ptx::mbar_init(&tmem_empty_bar[a], 4 * kConv3Parts);
+      ptx::mbar_init(&empty_bar[s], kConsumerThreads);
     }
     ptx::mbar_init(wres_bar, 1);
     ptx::fence_barrier_init();
@@ -604,135 +428,84 @@ __global__ void __launch_bounds__(kConv3Threads, 1) umma_conv3_kernel(const __gr
     ptx::prefetch_tensormap(&tmO_hi);
     ptx::prefetch_tensormap(&tmO_lo);
   }
-  if (warp == 1) ptx::tmem_alloc(tmem_slot, (uint32_t)p.tmem_cols);
   for (int i = threadIdx.x; i < p.Cout; i += blockDim.x) {
     sc_s[i] = p.scale ? __ldg(&p.scale[i]) : 1.f;
     sh_s[i] = p.shift ? __ldg(&p.shift[i]) : 0.f;
   }
-  ptx::tc_fence_before();
   __syncthreads();
-  if (p.cluster > 1) ptx::cluster_sync();  // every CTA's barriers exist before a peer multicasts into them
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t acc_stride = (uint32_t)p.tmem_cols / 2;
 
-  if (warp == 0) {
+  if (warp == kConsumerThreads / 32) {
     if (lane == 0) umma_producer_loop(tmA_hi, tmA_lo, tmA_hi, tmA_lo, p, smem, full_bar, empty_bar, wres_bar);
-  } else if (warp == 1) {
-    if (lane == 0) umma_mma_loop(p, smem, full_bar, empty_bar, tmem_full_bar, tmem_empty_bar, tmem_base, acc_stride, wres_bar);
-  } else {
-    const int q = warp & 3;           // TMEM lane quadrant
-    const int half = (warp - 2) >> 2;  // which NC/kConv3Parts channels
-    const int m = q * 32 + lane;
-    const bool issuer = (q == 0) && (lane == 0);  // the thread of this half that owns the bulk store groups
-    const bool out_row = (m >= 8) && (m < 8 + kConvStride);
-    float* edge0 = edge_base + half * 8 * H;  // [q][H]: P_0 of row 32q+31
-    float* edge2 = edge0 + 4 * H;             // [q][H]: P_2 of row 32q
-    const int bar_a = 1 + 2 * half, bar_b = 2 + 2 * half;
-    int acc = 0, it = 0;
-    uint32_t acc_phase = 0;
-    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++it) {
-      const TileCoord tc = decode_tile(p, tile);
-      const int n0 = tc.n_idx * NC + half * H;  // first output channel of this warp
-      ptx::mbar_wait_opt(&tmem_full_bar[acc], acc_phase, p.sleep_ns, 300 + acc);
-      ptx::tc_fence_after();
-      const uint32_t trow = tmem_base + (uint32_t)acc * acc_stride + ((uint32_t)(q * 32) << 16) + (uint32_t)(half * H);
-      uint32_t v0[H], v1[H], v2[H];
-      ptx::tmem_ld_n<H>(trow, v0);
-      ptx::tmem_ld_n<H>(trow + NC, v1);
-      ptx::tmem_ld_n<H>(trow + 2 * NC, v2);
-      ptx::tmem_ld_wait();
-      // the accumulator now lives in registers: hand it back to the MMA issuer
-      ptx::tc_fence_before();
-      __syncwarp();
-      if (lane == 0) ptx::mbar_arrive(&tmem_empty_bar[acc]);
-      acc ^= 1;
-      if (acc == 0) acc_phase ^= 1;
-      // boundary rows for the neighbouring quadrants
-      if (lane == 31) {
+    return;
+  }
+  const int wg = warp >> 2, g = lane >> 2, cq = lane & 3;
+  const int mrow0 = wg * 64 + (warp & 3) * 16 + g;  // tile rows mrow0 and mrow0 + 8
+  const bool issuer = threadIdx.x == 0;             // owns the bulk store groups
+  if (p.b_resident) ptx::mbar_wait(wres_bar, 0, 500);  // the resident weight image has landed
+  int s = 0;
+  uint32_t phase = 0;
+  float acc[3 * NC / 2];
+  for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+    const TileCoord tc = decode_tile(p, tile);
+    consumer_mainloop(p, smem, full_bar, empty_bar, s, phase, [&](uint32_t ah, uint32_t al, uint32_t bh, uint32_t bl, int j, int accum) {
+      const uint64_t dah = a_desc(p, ah, wg, j), dal = a_desc(p, al, wg, j), dbh = b_desc(p, bh, j), dbl = b_desc(p, bl, j);
+      conv3_mma<NC>(acc, dah, dbh, accum);
+      conv3_mma<NC>(acc, dah, dbl, 1);
+      conv3_mma<NC>(acc, dal, dbh, 1);
+    });
+    ptx::fence_regs(acc);
+    // boundary rows for the neighbouring warps
 #pragma unroll
-        for (int j = 0; j < H; j += 4) *reinterpret_cast<uint4*>(&edge0[q * H + j]) = make_uint4(v0[j], v0[j + 1], v0[j + 2], v0[j + 3]);
-      }
-      if (lane == 0) {
+    for (int i = 0; i < G; ++i) {
+      const int col = 8 * i + 2 * cq;
+      if (g == 7) *reinterpret_cast<float2*>(&edge0[warp * NC + col]) = make_float2(acc[4 * i + 2], acc[4 * i + 3]);
+      if (g == 0) *reinterpret_cast<float2*>(&edge2[warp * NC + col]) = make_float2(acc[4 * (2 * G + i)], acc[4 * (2 * G + i) + 1]);
+    }
+    // the staging planes must have been read out by the previous tile's store
+    if (issuer) ptx::bulk_wait_read<0>();
+    asm volatile("bar.sync %0, %1;" ::"n"(kEpiBar), "n"(kConsumerThreads) : "memory");
+    const int n0 = tc.n_idx * NC;
 #pragma unroll
-        for (int j = 0; j < H; j += 4) *reinterpret_cast<uint4*>(&edge2[q * H + j]) = make_uint4(v2[j], v2[j + 1], v2[j + 2], v2[j + 3]);
-      }
-      // the staging buffer of this tile must have been read out by the store issued n_sbuf tiles ago
-      if (issuer) {
-        if (p.n_sbuf == 2) ptx::bulk_wait_read<1>();
-        else ptx::bulk_wait_read<0>();
-      }
-      asm volatile("bar.sync %0, 128;" ::"r"(bar_a) : "memory");
-      float x[H];
+    for (int i = 0; i < G; ++i) {
 #pragma unroll
-      for (int j = 0; j < H; ++j) {
-        const float a = __shfl_up_sync(0xffffffffu, __uint_as_float(v0[j]), 1);    // P_0 of row m-1
-        const float c = __shfl_down_sync(0xffffffffu, __uint_as_float(v2[j]), 1);  // P_2 of row m+1
-        x[j] = __uint_as_float(v1[j]) + ((lane == 0) ? 0.f : a) + ((lane == 31) ? 0.f : c);
-      }
-      if (lane == 0 && q > 0) {
+      for (int e = 0; e < 2; ++e) {
+        const int col = 8 * i + 2 * cq + e;
+        const float p0a = acc[4 * i + e], p0b = acc[4 * i + 2 + e];
+        const float p1a = acc[4 * (G + i) + e], p1b = acc[4 * (G + i) + 2 + e];
+        const float p2a = acc[4 * (2 * G + i) + e], p2b = acc[4 * (2 * G + i) + 2 + e];
+        const float up_a = __shfl_sync(0xffffffffu, p0a, (lane + 28) & 31), up_b = __shfl_sync(0xffffffffu, p0b, (lane + 28) & 31);
+        const float dn_a = __shfl_sync(0xffffffffu, p2a, (lane + 4) & 31), dn_b = __shfl_sync(0xffffffffu, p2b, (lane + 4) & 31);
+        const float prev = (g == 0 && warp > 0) ? edge0[(warp - 1) * NC + col] : 0.f;
+        const float next = (g == 7 && warp < 7) ? edge2[(warp + 1) * NC + col] : 0.f;
+        float x[2];
+        x[0] = p1a + ((g > 0) ? up_a : prev) + ((g < 7) ? dn_a : dn_b);
+        x[1] = p1b + ((g > 0) ? up_b : up_a) + ((g < 7) ? dn_b : next);
 #pragma unroll
-        for (int j = 0; j < H; j += 4) {
-          const float4 e = *reinterpret_cast<const float4*>(&edge0[(q - 1) * H + j]);
-          x[j] += e.x; x[j + 1] += e.y; x[j + 2] += e.z; x[j + 3] += e.w;
+        for (int h = 0; h < 2; ++h) {
+          const int m = mrow0 + 8 * h;
+          if (m < 8 || m >= 8 + kConvStride) continue;
+          float y = act1(fmaf(x[h], sc_s[n0 + col], sh_s[n0 + col]), p.act);
+          const int f = tc.f0 + m - 8;
+          if ((p.res_hi || p.mul_hi) && f < p.F) {
+            const size_t plane = (size_t)p.T * p.F;
+            const size_t ro = ((size_t)tc.b * p.Cout + n0 + col) * plane + (size_t)tc.t * p.F + f;  // residual / multiplier: (B, Cout, T, F)
+            if (p.res_hi) y += pair_at(p.res_hi, p.res_lo, ro);
+            if (p.mul_hi) y *= pair_at(p.mul_hi, p.mul_lo, ro);
+          }
+          split_store2(y, s_hi[col * kConvStride + (m - 8)], s_lo[col * kConvStride + (m - 8)]);
         }
-      }
-      if (lane == 31 && q < 3) {
-#pragma unroll
-        for (int j = 0; j < H; j += 4) {
-          const float4 e = *reinterpret_cast<const float4*>(&edge2[(q + 1) * H + j]);
-          x[j] += e.x; x[j + 1] += e.y; x[j + 2] += e.z; x[j + 3] += e.w;
-        }
-      }
-#pragma unroll
-      for (int j = 0; j < H; j += 4) {
-        const float4 s4 = *reinterpret_cast<const float4*>(&sc_s[n0 + j]);
-        const float4 h4 = *reinterpret_cast<const float4*>(&sh_s[n0 + j]);
-        x[j] = fmaf(x[j], s4.x, h4.x); x[j + 1] = fmaf(x[j + 1], s4.y, h4.y); x[j + 2] = fmaf(x[j + 2], s4.z, h4.z); x[j + 3] = fmaf(x[j + 3], s4.w, h4.w);
-      }
-      act_group(x, p.act);
-      const int f = tc.f0 + m - 8;
-      if ((p.res_hi || p.mul_hi) && out_row && f < p.F) {
-        const size_t plane = (size_t)p.T * p.F;
-        const size_t rbase = ((size_t)tc.b * p.Cout + n0) * plane + (size_t)tc.t * p.F + f;  // residual / multiplier: (B, Cout, T, F)
-        if (p.res_hi) {
-#pragma unroll
-          for (int j = 0; j < H; ++j) x[j] += __bfloat162float(p.res_hi[rbase + (size_t)j * plane]) + __bfloat162float(p.res_lo[rbase + (size_t)j * plane]);
-        }
-        if (p.mul_hi) {
-#pragma unroll
-          for (int j = 0; j < H; ++j) x[j] *= __bfloat162float(p.mul_hi[rbase + (size_t)j * plane]) + __bfloat162float(p.mul_lo[rbase + (size_t)j * plane]);
-        }
-      }
-      bf16* s_hi = stage_out + (size_t)(((p.n_sbuf == 2) ? (it & 1) : 0) * kConv3Parts + half) * 2 * kPlane;
-      bf16* s_lo = s_hi + kPlane;
-      if (out_row) {
-#pragma unroll
-        for (int j = 0; j < H; ++j) {
-          bf16 h, l;
-          split_store2(x[j], h, l);
-          s_hi[j * kConvStride + (m - 8)] = h;
-          s_lo[j * kConvStride + (m - 8)] = l;
-        }
-      }
-      ptx::fence_proxy_async();
-      asm volatile("bar.sync %0, 128;" ::"r"(bar_b) : "memory");
-      if (issuer) {
-        const int cc = tc.b * p.out_c_total + p.out_c_off + n0;
-        ptx::tma_store_3d(&tmO_hi, s_hi, tc.f0, tc.t, cc);
-        ptx::tma_store_3d(&tmO_lo, s_lo, tc.f0, tc.t, cc);
-        ptx::bulk_commit();
       }
     }
-    if (issuer) ptx::bulk_wait_all();
+    ptx::fence_proxy_async();
+    asm volatile("bar.sync %0, %1;" ::"n"(kEpiBar), "n"(kConsumerThreads) : "memory");
+    if (issuer) {
+      const int cc = tc.b * p.out_c_total + p.out_c_off + n0;
+      ptx::tma_store_3d(&tmO_hi, s_hi, tc.f0, tc.t, cc);
+      ptx::tma_store_3d(&tmO_lo, s_lo, tc.f0, tc.t, cc);
+      ptx::bulk_commit();
+    }
   }
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (p.cluster > 1) ptx::cluster_sync();  // no CTA leaves while a peer may still signal its barriers
-  if (warp == 1) {
-    ptx::tc_fence_after();
-    ptx::tmem_dealloc(tmem_base, (uint32_t)p.tmem_cols);
-  }
+  if (issuer) ptx::bulk_wait_all();
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -777,12 +550,6 @@ static int make_map(CUtensorMap* map, const void* base, int rank, const uint64_t
   return B200SEP_OK;
 }
 
-static int pow2_cols(int n) {
-  int c = 32;
-  while (c < n) c <<= 1;
-  return c;
-}
-
 static int num_sms() {
   static int n = 0;
   if (n == 0) {
@@ -793,15 +560,6 @@ static int num_sms() {
   return n;
 }
 
-// Cluster size for the operand multicast.  Conv modes: the CTAs of a cluster must sit on the same weight tile at every step of their tile walk, which holds
-// when tile ids, the grid and the number of tiles per weight tile are all multiples of the cluster size; GEMM: `cs` consecutive tiles share their activation rows
-// when cs divides the tiles along N.  Measured on B200 (profiles/README.md, round 2): the conv kernels gain nothing from it (they are not L2-bound), so it is
-// off by default there; B200SEP_CLUSTER / B200SEP_CLUSTER_GEMM (1, 2, 4, 8) select it for A/B runs.
-static int env_cluster(const char* name, int dflt) {
-  const char* e = getenv(name);
-  const int v = e ? atoi(e) : dflt;
-  return (v == 1 || v == 2 || v == 4 || v == 8) ? v : dflt;
-}
 static int umma_wait_sleep_ns() {
   static const int ns = [] {
     const char* e = getenv("B200SEP_WAIT_SLEEP_NS");
@@ -810,76 +568,28 @@ static int umma_wait_sleep_ns() {
   return ns;
 }
 
-static int choose_cluster(const UmmaParams& p) {
-  static const int want_conv = env_cluster("B200SEP_CLUSTER", 1), want_gemm = env_cluster("B200SEP_CLUSTER_GEMM", 1);
-  if (p.mode == 0) {
-    for (int cs = std::min(want_gemm, 4); cs > 1; cs >>= 1)
-      if (p.n_tiles % cs == 0) return cs;
-    return 1;
-  }
-  for (int cs = want_conv; cs > 1; cs >>= 1)
-    if (p.num_tiles % cs == 0 && (p.n_ftiles * p.t_tiles) % cs == 0 && p.b_bytes % (16u * cs) == 0) return cs;
-  return 1;
-}
-
-// Persistent launch: one CTA per SM, as clusters of `cs` when the weight operand is multicast (the grid is then the number of co-resident clusters x cs).
+// Persistent launch: one CTA per SM.
 template <class Kernel, class... Args>
-static int launch_persistent(Kernel kernel, int threads, int cs, int num_tiles, size_t smem, cudaStream_t st, Args... args) {
-  cudaLaunchConfig_t cfg{};
-  cfg.blockDim = dim3((unsigned)threads);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = (unsigned)cs;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  int grid = std::min(num_tiles, num_sms());
-  if (cs > 1) {
-    static std::map<std::tuple<const void*, int, size_t>, int> cache;
-    static std::mutex mu;
-    int nclusters = 0;
-    {
-      std::lock_guard<std::mutex> lock(mu);
-      const auto key = std::make_tuple((const void*)kernel, cs, smem);
-      auto it = cache.find(key);
-      if (it == cache.end()) {
-        cfg.gridDim = dim3((unsigned)(num_sms() / cs * cs));
-        B2_CUDA(cudaOccupancyMaxActiveClusters(&nclusters, kernel, &cfg));
-        cache[key] = nclusters;
-      } else {
-        nclusters = it->second;
-      }
-    }
-    B2_CHECK_ARG(nclusters >= 1, "umma: no cluster of %d CTAs with %zu bytes of shared memory can be resident", cs, smem);
-    grid = std::min(num_tiles, nclusters * cs) / cs * cs;
-  }
-  cfg.gridDim = dim3((unsigned)grid);
-  B2_CUDA(cudaLaunchKernelEx(&cfg, kernel, args...));
-  count_launch();
+static int launch_persistent(Kernel kernel, int num_tiles, size_t smem, cudaStream_t st, Args... args) {
+  const int grid = std::min(num_tiles, num_sms());
+  kernel<<<grid, kUmmaThreads, smem, st>>>(args...);
+  B2_LAUNCHED();
   return B200SEP_OK;
 }
 
 // `tiles` is the logical tile grid: GEMM (n tiles, m tiles, 1); conv modes (f tiles, output rows, batch * channel tiles).
 static int launch(const CUtensorMap& a_hi, const CUtensorMap& a_lo, const CUtensorMap& b_hi, const CUtensorMap& b_lo, UmmaParams& p, dim3 tiles,
-                  cudaStream_t st, const CUtensorMap* a_slices = nullptr /* GEMM: {hi, lo} with 64-row boxes, {hi, lo} with 32-row boxes */) {
-  {
-    const char* e = getenv("B200SEP_DBG");  // development only: selectively disable parts of the kernel (results become wrong)
-    p.dbg = e ? atoi(e) : 0;
-    p.sleep_ns = umma_wait_sleep_ns();
-  }
+                  cudaStream_t st) {
+  p.sleep_ns = umma_wait_sleep_ns();
+  B2_CHECK_ARG(p.n_tile % 16 == 0 && p.n_tile >= 16 && p.n_tile <= kMaxNTile, "umma: n_tile=%d is not a multiple of 16 in [16, %d]", p.n_tile, kMaxNTile);
   p.stage_bytes = ((2 * p.a_bytes + 2 * p.b_bytes + 1023) / 1024) * 1024;
-  p.tmem_cols = 2 * pow2_cols(p.n_tile);  // two accumulators: the epilogue of tile i overlaps the MMAs of tile i+1
-  B2_CHECK_ARG(p.tmem_cols <= 512, "umma: n_tile=%d needs more than 512 TMEM columns", p.n_tile);
   if (p.mode == 0) p.n_tiles = (int)tiles.x;
   p.n_ftiles = (int)tiles.x;
   p.t_tiles = (int)tiles.y;
   p.num_tiles = (int)(tiles.x * tiles.y * tiles.z);
-  const size_t fixed = 1024 /*alignment slack*/ + 64 * sizeof(uint64_t) + 64 + 2 * kMaxChannels * sizeof(float) + (p.mode != 0 ? (size_t)16 * p.n_c * sizeof(float) : 0);
+  const size_t fixed = 1024 /*alignment slack*/ + 64 * sizeof(uint64_t) + 64 + 2 * kMaxChannels * sizeof(float);
   B2_CHECK_ARG(p.mode == 0 || p.Cout <= kMaxChannels, "umma: more than %d output channels", kMaxChannels);
-  const size_t budget = 220 * 1024 - fixed;  // one persistent CTA per SM
+  const size_t budget = 227 * 1024 - fixed;  // one persistent CTA per SM
   int stages = (int)(budget / p.stage_bytes);
   if (stages > 8) stages = 8;
   B2_CHECK_ARG(stages >= 2, "umma: a pipeline stage of %u bytes does not fit twice in shared memory", p.stage_bytes);
@@ -890,13 +600,7 @@ static int launch(const CUtensorMap& a_hi, const CUtensorMap& a_lo, const CUtens
     B2_CUDA(cudaFuncSetAttribute(umma_pair_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     attr_set = true;
   }
-  p.cluster = choose_cluster(p);
-  if (p.mode == 0 && p.cluster > 1) {
-    B2_CHECK_ARG(a_slices != nullptr, "umma: GEMM multicast needs the sliced activation maps");
-    const CUtensorMap* sl = a_slices + (p.cluster == 4 ? 2 : 0);
-    return launch_persistent(umma_pair_kernel, kUmmaThreads, p.cluster, p.num_tiles, smem, st, sl[0], sl[1], b_hi, b_lo, p);
-  }
-  return launch_persistent(umma_pair_kernel, kUmmaThreads, p.cluster, p.num_tiles, smem, st, a_hi, a_lo, b_hi, b_lo, p);
+  return launch_persistent(umma_pair_kernel, p.num_tiles, smem, st, a_hi, a_lo, b_hi, b_lo, p);
 }
 
 bool umma_gemm_supported(int M, int N, int K) { return M >= 1 && N % 16 == 0 && K % 8 == 0 && N >= 16 && K >= 16; }
@@ -908,10 +612,6 @@ int umma_gemm_plan_create(UmmaGemmPlan* pl, const void* a_hi, const void* a_lo, 
     for (n_tile = 128; n_tile >= 16; n_tile -= 16)
       if (N % n_tile == 0) break;
   }
-  // prefer a tile width whose tile count along N is a multiple of 4 (then of 2): those tiles run as one cluster and share the activation rows by multicast
-  auto share = [&](int nt) { const int t = N / nt; return t % 4 == 0 ? 4 : (t % 2 == 0 ? 2 : 1); };
-  for (int cand : {96, 64})
-    if (N % cand == 0 && N >= cand && share(cand) > share(n_tile)) n_tile = cand;
   pl->n_tile = n_tile;
   const uint64_t da[2] = {(uint64_t)K, (uint64_t)M}, sa[1] = {(uint64_t)K * 2};
   const uint32_t ba[2] = {64, 128};
@@ -919,11 +619,6 @@ int umma_gemm_plan_create(UmmaGemmPlan* pl, const void* a_hi, const void* a_lo, 
   const uint32_t bb[2] = {64, (uint32_t)n_tile};
   int rc = make_map(&pl->a_hi, a_hi, 2, da, sa, ba);
   if (!rc) rc = make_map(&pl->a_lo, a_lo, 2, da, sa, ba);
-  const uint32_t ba2[2] = {64, 64}, ba4[2] = {64, 32};
-  if (!rc) rc = make_map(&pl->a_slices[0], a_hi, 2, da, sa, ba2);
-  if (!rc) rc = make_map(&pl->a_slices[1], a_lo, 2, da, sa, ba2);
-  if (!rc) rc = make_map(&pl->a_slices[2], a_hi, 2, da, sa, ba4);
-  if (!rc) rc = make_map(&pl->a_slices[3], a_lo, 2, da, sa, ba4);
   if (!rc) rc = make_map(&pl->b_hi, w_hi, 2, db, sa, bb);
   if (!rc) rc = make_map(&pl->b_lo, w_lo, 2, db, sa, bb);
   return rc;
@@ -956,9 +651,8 @@ int umma_gemm_run_ex(const UmmaGemmPlan& pl, int rows_per_channel, int channels,
   p.M = M_active; p.K = pl.K; p.rows_per_channel = rows_per_channel; p.channels = channels;
   p.scale = scale; p.shift = shift; p.act = relu;
   p.out_hi = (bf16*)out_hi; p.out_lo = (bf16*)out_lo; p.res_hi = (const bf16*)res_hi; p.res_lo = (const bf16*)res_lo;
-  B2_CHECK_ARG(pl.n_tile <= 128, "umma_gemm: n_tile=%d exceeds the epilogue's 8 column groups", pl.n_tile);
   dim3 grid(pl.N / pl.n_tile, cdiv(M_active, kTileM));
-  return launch(pl.a_hi, pl.a_lo, pl.b_hi, pl.b_lo, p, grid, st, pl.a_slices);
+  return launch(pl.a_hi, pl.a_lo, pl.b_hi, pl.b_lo, p, grid, st);
 }
 
 bool umma_conv_supported(int Cin, int Cout, int F, int kh, int kw) {
@@ -981,7 +675,7 @@ int umma_conv_choose(int Cin, int Cout, int* kc, int* n_c) {
   // (n_c = 80 with 64 channels per stage is a 92 KB stage: MDX23C's 640-channel scale)
   auto fits = [&](int kk) {
     const size_t stage = ((size_t)2 * kk * 256 + (size_t)2 * (kk / 16) * (3 * nc) * 32 + 1023) / 1024 * 1024;
-    const size_t staging = (size_t)2 * kConv3Parts * (nc / kConv3Parts) * kConvStride * 2;
+    const size_t staging = (size_t)2 * nc * kConvStride * 2;  // hi + lo output planes
     return 2 * stage + staging + 16 * 1024 <= 227 * 1024;
   };
   while (!fits(k) && k > 16) {
@@ -1013,7 +707,7 @@ int umma_conv_run(const UmmaConvPlan& pl, const void* wb_hi, const void* wb_lo, 
   return umma_conv_run_ex(pl, wb_hi, wb_lo, B, Cout, n_c, e, st);
 }
 
-// TMA store maps of a conv3x3 output: the (F, T, B * C_total) bf16 planes with a [112 px][1 row][NC/2 channels] box, no swizzle.  Encoding a map costs a few
+// TMA store maps of a conv3x3 output: the (F, T, B * C_total) bf16 planes with a [112 px][1 row][NC channels] box, no swizzle.  Encoding a map costs a few
 // microseconds on the host and the same activation buffers are written forward after forward, so the maps are cached by (plane address, geometry).
 struct StoreMapKey {
   const void* base; int F, T, C, box_c;
@@ -1046,9 +740,8 @@ static int launch_conv3(const CUtensorMap& a_hi, const CUtensorMap& a_lo, const 
     B2_CUDA(cudaFuncSetAttribute(umma_conv3_kernel<NC>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     attr_set = true;
   }
-  p.cluster = choose_cluster(p);
   p.sleep_ns = umma_wait_sleep_ns();
-  return launch_persistent(umma_conv3_kernel<NC>, kConv3Threads, p.cluster, p.num_tiles, smem, st, a_hi, a_lo, o_hi, o_lo, p);
+  return launch_persistent(umma_conv3_kernel<NC>, p.num_tiles, smem, st, a_hi, a_lo, o_hi, o_lo, p);
 }
 
 int umma_conv_run_ex(const UmmaConvPlan& pl, const void* wb_hi, const void* wb_lo, int B, int Cout, int n_c, const UmmaEpilogue& e, cudaStream_t st) {
@@ -1069,31 +762,23 @@ int umma_conv_run_ex(const UmmaConvPlan& pl, const void* wb_hi, const void* wb_l
   static const bool allow_res = !(getenv("B200SEP_WRES") && atoi(getenv("B200SEP_WRES")) == 0);
   p.b_resident = (allow_res && p.n_tiles == 1 && b_all <= 96 * 1024) ? 1 : 0;
   p.stage_bytes = ((2 * p.a_bytes + (p.b_resident ? 0 : 2 * p.b_bytes) + 1023) / 1024) * 1024;
-  p.tmem_cols = 2 * pow2_cols(p.n_tile);
-  B2_CHECK_ARG(p.tmem_cols <= 512, "umma_conv: n_c=%d needs more than 512 TMEM columns", n_c);
   p.n_ftiles = cdiv(pl.F, kConvStride);
   p.t_tiles = pl.T;
   p.num_tiles = p.n_ftiles * pl.T * B * p.n_tiles;
-  B2_CHECK_ARG(n_c % (4 * kConv3Parts) == 0, "umma_conv: n_c=%d is not a multiple of %d", n_c, 4 * kConv3Parts);
-  const size_t stage_plane = (size_t)(n_c / kConv3Parts) * kConvStride * 2;  // bytes of one staged [n_c/parts][112] bf16 plane
-  const size_t fixed = 1024 /*alignment slack*/ + 64 * sizeof(uint64_t) + 64 + 2 * kMaxChannels * sizeof(float) + (size_t)8 * n_c * sizeof(float) +
+  B2_CHECK_ARG(n_c % 16 == 0 && n_c <= 80, "umma_conv: n_c=%d is not a multiple of 16 up to 80", n_c);
+  const size_t sbuf_bytes = (size_t)2 * n_c * kConvStride * 2;  // staged output: hi + lo planes [n_c][112] bf16
+  const size_t fixed = 1024 /*alignment slack*/ + 64 * sizeof(uint64_t) + 64 + 2 * kMaxChannels * sizeof(float) + (size_t)16 * n_c * sizeof(float) +
                        (p.b_resident ? b_all : 0);
   const size_t budget = 227 * 1024 - fixed;
-  p.n_sbuf = 2;
-  const size_t sbuf_bytes = 2 * kConv3Parts * stage_plane;  // hi + lo plane per column part
-  int stages = (int)((budget - 2 * sbuf_bytes) / p.stage_bytes);
-  if (stages < 3) {  // deep layers with 80 KB stages: one staging buffer leaves room for the ring
-    p.n_sbuf = 1;
-    stages = (int)((budget - sbuf_bytes) / p.stage_bytes);
-  }
+  int stages = (int)((budget - sbuf_bytes) / p.stage_bytes);
   if (stages > 8) stages = 8;
   B2_CHECK_ARG(stages >= 2, "umma_conv: a pipeline stage of %u bytes does not fit twice in shared memory", p.stage_bytes);
   p.stages = stages;
   p.b_res_off = (uint32_t)((size_t)stages * p.stage_bytes);
-  const size_t smem = (size_t)stages * p.stage_bytes + (size_t)p.n_sbuf * sbuf_bytes + fixed;
+  const size_t smem = (size_t)stages * p.stage_bytes + sbuf_bytes + fixed;
   CUtensorMap o_hi, o_lo;
-  int rc = store_map(p.out_hi, pl.F, pl.T, B * p.out_c_total, n_c / kConv3Parts, &o_hi);
-  if (!rc) rc = store_map(p.out_lo, pl.F, pl.T, B * p.out_c_total, n_c / kConv3Parts, &o_lo);
+  int rc = store_map(p.out_hi, pl.F, pl.T, B * p.out_c_total, n_c, &o_hi);
+  if (!rc) rc = store_map(p.out_lo, pl.F, pl.T, B * p.out_c_total, n_c, &o_lo);
   if (rc) return rc;
   switch (n_c) {
     case 16: return launch_conv3<16>(pl.a_hi, pl.a_lo, o_hi, o_lo, p, smem, st);
@@ -1112,15 +797,14 @@ static int pick_nc(int Cout, int mult, int limit) {  // largest n_c | Cout with 
   return 0;
 }
 bool umma_updown_supported(int Cin, int Cout, int F_in, int up) {
-  return Cin % 16 == 0 && F_in % 8 == 0 && pick_nc(Cout, up ? 4 : 2, 256) > 0 && (up || F_in % 2 == 0);
+  return Cin % 16 == 0 && F_in % 8 == 0 && pick_nc(Cout, up ? 4 : 2, kMaxNTile) > 0 && (up || F_in % 2 == 0);
 }
 int umma_updown_choose(int Cin, int Cout, int up, int* kc, int* n_c) {
   int k = 64;
   while (k > 16 && Cin % k != 0) k -= 16;
   if (Cin % 48 == 0) k = 48;
   *kc = k;
-  *n_c = pick_nc(Cout, up ? 4 : 2, up ? 192 : 256);
-  if (*n_c == 0) *n_c = pick_nc(Cout, up ? 4 : 2, 256);
+  *n_c = pick_nc(Cout, up ? 4 : 2, kMaxNTile);
   return 0;
 }
 
@@ -1199,17 +883,17 @@ static void block_weights(int n_tiles, int n_r, int Cin, int kc, int rows, F val
           pos += (size_t)rows * 16;
         }
 }
-// ConvTranspose2d weight (Cin, Cout, 2, 2): B rows = (q = dy*2+dx, co_local)
+// ConvTranspose2d weight (Cin, Cout, 2, 2): B rows = (co_local, q = dy*2+dx)
 void umma_up_block_weights(const float* w, int Cin, int Cout, int kc, int n_c, std::vector<uint16_t>& hi, std::vector<uint16_t>& lo) {
   block_weights(Cout / n_c, 1, Cin, kc, 4 * n_c, [&](int nt, int row, int, int ci) {
-    const int q = row / n_c, co = nt * n_c + row % n_c;
+    const int q = row & 3, co = nt * n_c + (row >> 2);
     return w[((size_t)ci * Cout + co) * 4 + q];
   }, hi, lo);
 }
-// Conv2d weight (Cout, Cin, 2, 2) stride 2: row taps r = dy, B rows = (dx, co_local)
+// Conv2d weight (Cout, Cin, 2, 2) stride 2: row taps r = dy, B rows = (co_local, dx)
 void umma_down_block_weights(const float* w, int Cout, int Cin, int kc, int n_c, std::vector<uint16_t>& hi, std::vector<uint16_t>& lo) {
   block_weights(Cout / n_c, 2, Cin, kc, 2 * n_c, [&](int nt, int row, int dy, int ci) {
-    const int dx = row / n_c, co = nt * n_c + row % n_c;
+    const int dx = row & 1, co = nt * n_c + (row >> 1);
     return w[(((size_t)co * Cin + ci) * 2 + dy) * 2 + dx];
   }, hi, lo);
 }
@@ -1224,7 +908,7 @@ int umma_pw_choose(int Cin, int Cout, int* kc, int* n_c) {
   while (k > 16 && Cin % k != 0) k -= 16;
   if (Cin % 48 == 0) k = 48;
   *kc = k;
-  *n_c = pick_nc(Cout, 1, 256);
+  *n_c = pick_nc(Cout, 1, kMaxNTile);
   return 0;
 }
 // x: pair (B, Cin, T, F) -> Conv2d 1x1 (+affine, act, +res, *mul) -> pair or fp32 (B, Cout, T, F)
@@ -1302,7 +986,7 @@ int join_pair(const void* hi, const void* lo, float* y, int64_t n, cudaStream_t 
 
 // ---------------------------------------------------------------------------------------------------------
 // self-test entry points (exported through the C ABI so the GPU test-suite can check each tensor-core operator in
-// isolation against a plain fp32 reference): fp32 in -> split -> tcgen05 op -> join -> fp32 out.
+// isolation against a plain fp32 reference): fp32 in -> split -> wgmma op -> join -> fp32 out.
 using namespace b200sep;
 
 extern "C" int b200sep_selftest_umma_gemm(const float* a, const float* w, const float* res, float* out, int M, int N, int K, int rows_per_channel,

@@ -1,4 +1,4 @@
-// Host interface of the tcgen05 "pair" operators (umma_ops.cu).
+// Host interface of the wgmma "pair" operators (umma_ops.cu).
 #pragma once
 #include <cuda.h>
 #include <stdint.h>
@@ -11,7 +11,6 @@ namespace b200sep {
 
 struct UmmaGemmPlan {
   CUtensorMap a_hi, a_lo, b_hi, b_lo;
-  CUtensorMap a_slices[4];  // the activation planes again with 64-row and 32-row boxes: each CTA of a 2 / 4 cluster loads one slice and multicasts it
   int M, N, K, n_tile;
 };
 struct UmmaConvPlan {

@@ -10,7 +10,7 @@ for p in (os.path.join(ROOT, "python-audio-separator_b200"), os.path.join(ROOT, 
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100; run with -m gpu)")
 
 
 @pytest.fixture(scope="session")

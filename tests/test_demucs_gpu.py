@@ -100,7 +100,7 @@ def test_conv_transpose_f32(dm, axis):
 
 @pytest.mark.parametrize("axis", [1, 2])
 def test_conv_transpose_f32_tensor_core_route(dm, axis):
-    """Same operator at shapes the tcgen05 kernel takes (real output channels a multiple of 16, >= 512 coarse pixels): the scatter epilogue of tc_f32.cu."""
+    """Same operator at shapes the wgmma kernel takes (real output channels a multiple of 16, >= 512 coarse pixels): the scatter epilogue of tc_f32.cu."""
     g = torch.Generator().manual_seed(5)
     cin, cout = 96, 48
     if axis == 1:

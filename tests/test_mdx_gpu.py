@@ -16,7 +16,7 @@ import mdx_oracle as O
 pytestmark = pytest.mark.gpu
 
 SMALL = dict(n_fft=1536, hop_length=256, dim_f=768, dim_t=32, segment_size=32, g=8)
-MID = dict(n_fft=1024, hop_length=256, dim_f=512, dim_t=32, segment_size=32, g=16, num_blocks=7)  # channel counts the tcgen05 conv accepts
+MID = dict(n_fft=1024, hop_length=256, dim_f=512, dim_t=32, segment_size=32, g=16, num_blocks=7)  # channel counts the wgmma conv accepts
 
 
 @pytest.fixture(scope="module")

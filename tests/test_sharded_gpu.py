@@ -140,7 +140,7 @@ def test_sharded_engines_world1_equal_plain_engines(lib_built):
 
 
 @pytest.mark.timeout(900)
-@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs two GPUs (gpurun --gpus 2)")
+@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs two GPUs")
 def test_sharded_engines_world2_equal_single_gpu(lib_built):
     for name, same, diff in _run(2):
         # per-sample arithmetic is the single-GPU arithmetic (same contributions, same order).  The ranks batch their segments differently from the

@@ -1,5 +1,5 @@
-"""The fp32-in/fp32-out tensor-core GEMM / implicit-GEMM convolution (csrc/tc_f32.cu: in-kernel bf16 hi/lo split, three tcgen05
-products, fp32 TMEM accumulation) against fp64 ATen on the CPU.  Shapes are chosen to take the tensor-core route
+"""The fp32-in/fp32-out tensor-core GEMM / implicit-GEMM convolution (csrc/tc_f32.cu: in-kernel bf16 hi/lo split, three wgmma
+products, fp32 accumulation in registers) against fp64 ATen on the CPU.  Shapes are chosen to take the tensor-core route
 (tc_gemm_usable / tc_conv_usable) and to hit its edges: ragged M / N / K tiles, unaligned leading dimensions, batched strided
 operands (the attention pattern), output channel slices, every activation."""
 import numpy as np
@@ -108,7 +108,7 @@ def test_tc_conv2d_slice_and_add(dm):
     [(2, 3, 200, 1344, 0), (1, 2, 130, 130, 1), (1, 8, 2688, 2688, 0), (2, 2, 1344, 2688, 0), (3, 1, 1101, 1101, 1), (1, 1, 5, 7, 0), (1, 2, 128, 256, 1)],
 )
 def test_fused_attention_vs_fp64(lib_built, B, H, Lq, Lk, v_kn, packed):
-    """b200sep_attention_f32 (scores in TMEM, running softmax, P V from shared memory) against softmax(q k^T / 8) v in float64; ragged query / key tiles,
+    """b200sep_attention_f32 (scores in registers, running softmax, P as the register operand of P V) against softmax(q k^T / 8) v in float64; ragged query / key tiles,
     both V layouts (transposed with keys contiguous: HTDemucs; plain (keys, d): Roformer)."""
     from audio_separator.separator.b200._lib import check, lib
     from audio_separator.separator.b200.engine import _ptr, _stream

@@ -1,4 +1,4 @@
-"""GPU: the tcgen05 ("bf16x3 pair") operators in isolation against plain fp32 PyTorch references of the same op,
+"""GPU: the wgmma ("bf16x3 pair") operators in isolation against plain fp32 PyTorch references of the same op,
 through the C-ABI self-test entry points.  Tolerance: the split scheme carries ~16 mantissa bits per operand, so
 errors are ~1e-5 of the output scale (measured 7e-6 on the whole network); gate at 5e-5 relative to max|ref|."""
 import ctypes as C
