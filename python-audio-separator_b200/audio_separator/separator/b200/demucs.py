@@ -11,7 +11,6 @@ operator launches; every arithmetic step is a kernel behind the C ABI (include/b
 from __future__ import annotations
 
 import math
-import os
 from dataclasses import dataclass
 from fractions import Fraction
 
@@ -22,7 +21,6 @@ from ._lib import LAYOUT_CFT, check, lib
 from .engine import StftPlan, _ptr, _require_cuda, _stream
 
 ACT_NONE, ACT_RELU, ACT_GELU = 0, 1, 2
-_FUSED_ATTENTION = os.environ.get("B200SEP_FUSED_ATTN", "1") != "0"  # 0: the unfused scores / softmax / P V launches (A/B measurements)
 _DCONV_FUSED_HID = (4, 6, 8, 12, 16, 24, 32, 48)  # hidden widths b200sep_dconv_f32 is instantiated for
 
 
@@ -363,7 +361,7 @@ class HTDemucsNet:
         wv, bv = W[f"{p}.v_weight"], W[f"{p}.v_bias"]
         _gemm_raw(_ptr(wv), _ptr(kv_in), _ptr(vt), D, Lk, D, D, D, Lk, B, 0, Lk * D, D * Lk, bias_m=_ptr(bv))
         o = _new((B, Lq, D), q_in)
-        if hd == 64 and _FUSED_ATTENTION:  # one kernel, the (H, Lq, Lk) scores stay on chip
+        if hd == 64:  # one kernel, the (H, Lq, Lk) scores stay on chip
             work = _new((lib.b200sep_attention_work_floats(B, H, Lq, Lk),), q_in)  # bf16 hi / lo tile images of Q, K, V^T (split once, not once per consumer)
             check(lib.b200sep_attention_f32(_ptr(q), _ptr(k), _ptr(vt), _ptr(o), B, H, Lq, Lk, hd, Lq * D, D, Lk * D, D, D * Lk, Lk, Lq * D, D, 1.0 / math.sqrt(hd),
                                             0, _ptr(work), _stream()), "attention_f32")

@@ -12,22 +12,19 @@ graph are libb200sep's own; nothing is traced or compiled.  A C host does the sa
 """
 from __future__ import annotations
 
-import os
-
 import torch
 
 
 class GraphedForward:
     """fn(x) -> tensor, captured per (shape, dtype) of x.  The returned tensor is the graph's static output buffer: consume (copy) it before the
-    next call.  B200SEP_GRAPHS=0 runs eagerly (A/B measurements)."""
+    next call.  Inside a capture that is already running, fn runs directly and becomes part of the caller's graph."""
 
     def __init__(self, fn, warmup: int = 2, max_graphs: int = 8):
         self.fn, self.warmup, self.max_graphs = fn, warmup, max_graphs
         self.cache = {}
-        self.enabled = os.environ.get("B200SEP_GRAPHS", "1") != "0"
 
     def __call__(self, x: torch.Tensor) -> torch.Tensor:
-        if not self.enabled or torch.cuda.is_current_stream_capturing():
+        if torch.cuda.is_current_stream_capturing():
             return self.fn(x)
         key = (tuple(x.shape), x.dtype, x.device.index)
         ent = self.cache.get(key)

@@ -17,7 +17,7 @@ import numpy as np
 import torch
 
 from ._lib import LAYOUT_CFT, check, lib
-from .demucs import _FUSED_ATTENTION, ACT_GELU, ACT_NONE, _new, _packed_linear
+from .demucs import ACT_GELU, ACT_NONE, _new, _packed_linear
 from .engine import StftPlan, _ptr, _require_cuda, _stream
 
 ACT_TANH = 5
@@ -215,7 +215,7 @@ class BSRoformerNet:
             q, k, v = _new((Bq, H, n, dh), x), _new((Bq, H, n, dh), x), _new((Bq, H, n, dh), x)
             check(lib.b200sep_rope_split_heads_f32(_ptr(qkv), _ptr(W[f"{a}.rotary_embed.freqs"]), _ptr(q), _ptr(k), _ptr(v), Bq, n, H, dh, _stream()), "rope_split_heads_f32")
             o = _new((Bq, H, n, dh), x)
-            if dh == 64 and _FUSED_ATTENTION:  # scores stay on chip (b200sep_attention_f32): every (batch, head) pair is one batch entry of the kernel, V untransposed
+            if dh == 64:  # scores stay on chip (b200sep_attention_f32): every (batch, head) pair is one batch entry of the kernel, V untransposed
                 work = _new((lib.b200sep_attention_work_floats(Bq * H, 1, n, n),), x)
                 check(lib.b200sep_attention_f32(_ptr(q), _ptr(k), _ptr(v), _ptr(o), Bq * H, 1, n, n, dh, n * dh, dh, n * dh, dh, n * dh, dh, n * dh, dh, dh**-0.5, 1,
                                                 _ptr(work), _stream()), "attention_f32")

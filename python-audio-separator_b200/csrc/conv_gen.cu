@@ -239,7 +239,7 @@ extern "C" int b200sep_conv2d_f32(const float* x, const float* w_blocked, const 
   p.up_axis = up_axis; p.up = up; p.trim = trim; p.out_len = out_len; p.CoutReal = up_axis ? Cout / up : Cout;
   B2_CHECK_ARG(up_axis == 0 || (up >= 1 && Cout % up == 0), "conv2d_f32: transposed mode needs Cout divisible by the up factor");
   cudaStream_t st = (cudaStream_t)stream;
-  if (tc_enabled() && tc_conv_usable(Cin, Cout, KH, KW, Ho, Wo, B) && (up_axis == 0 || (p.CoutReal % 16 == 0 && add == nullptr)))
+  if (tc_conv_usable(Cin, Cout, KH, KW, Ho, Wo, B) && (up_axis == 0 || (p.CoutReal % 16 == 0 && add == nullptr)))
     return tc_conv2d_f32(x, w_blocked, bias, add, y, B, Cin, H, W, Cout, p.CoutPad, Ho, Wo, KH, KW, SH, SW, PH, PW, DH, DW, act, add_before_act, out_c_total, out_c_off, w_packed,
                          st, up_axis, up, trim, out_len);
 #define B2_CONV_CASE(kh, kw, sh, sw, dw) \

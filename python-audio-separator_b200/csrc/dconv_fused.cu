@@ -13,8 +13,6 @@
 // with a tiny finalise kernel after K1 and K2 turning the partial sums (double) into (mean, rstd) per sample.
 // All arithmetic is fp32 FMA (no tensor cores: 2*hid*2C flops per position against 4*(2C + C/4) bytes is below the ridge even for
 // fp32 SIMT); thread = P positions, the small weight matrices sit in shared memory and are read as broadcast float4.
-#include <stdlib.h>
-
 #include <algorithm>
 
 #include "common.cuh"
@@ -547,12 +545,8 @@ extern "C" int b200sep_dconv_f32(const float* x, float* y, const float* w0, cons
   p.B = B; p.C = C; p.Fr = Fr; p.L = (int)L; p.dil = dilation;
   cudaStream_t st = (cudaStream_t)stream;
   const bool have_u = u_in != nullptr;
-  // rows that fit in shared memory (the frequency branch) take the single-pass kernel; B200SEP_DCONV_ROW=0 keeps the three-pass form for A/B runs
-  static const bool row_on = [] {
-    const char* e = getenv("B200SEP_DCONV_ROW");
-    return !(e && e[0] == '0');
-  }();
-  if (row_on && !have_u && Fr > 1 && L <= 4096) {
+  // rows that fit in shared memory (the frequency branch) take the single-pass kernel
+  if (!have_u && Fr > 1 && L <= 4096) {
 #define B2_DCONV_ROW_CASE(h) \
   if (hid == h && dconv_row_smem<h>(C, (int)L) <= 216 * 1024) return dconv_row_launch<h>(p, st);
     B2_DCONV_ROW_CASE(6)

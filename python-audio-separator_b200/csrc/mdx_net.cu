@@ -5,11 +5,11 @@
 // Activation layout: (B, C, T, F) float32, F innermost -- the layout the reference network computes on
 // after its transpose(-1,-2) (mdxnet.py:101), which is also what the STFT kernel emits (layout CTF).
 #include <math.h>
-#include <string.h>
 
 #include <vector>
 
 #include "common.cuh"
+#include "net_builder.cuh"
 #include "simt_ops.cuh"
 #include "umma_ops.cuh"
 
@@ -20,11 +20,9 @@ struct ConvW {       // one convolution (+ folded BatchNorm) on the device
   float* scale = nullptr;  // [N]
   float* shift = nullptr;  // [N]
   int cin = 0, n = 0, n_pad = 0, kh = 1, kw = 1, stride = 1;
-  // tensor-core path (precision 1): weights split into bf16 hi/lo planes, pre-blocked for umma_conv_run
+  // tensor-core path (precision 1): weights split into bf16 hi/lo planes, pre-blocked for the pair kernels
   bool umma = false;
-  void* wb_hi = nullptr;
-  void* wb_lo = nullptr;
-  int kc = 0, n_tile = 0;  // n_tile = output channels per CTA (n_c)
+  PairWeights wb;
 };
 struct LinW {        // TDF linear (+ folded BatchNorm over the channel axis)
   float* w = nullptr;  // [N][K]
@@ -32,8 +30,7 @@ struct LinW {        // TDF linear (+ folded BatchNorm over the channel axis)
   float* shift = nullptr;
   int n = 0, k = 0, channels = 0;
   bool umma = false;
-  void* w_hi = nullptr;  // bf16 [N][K]
-  void* w_lo = nullptr;
+  PairWeights wb;  // bf16 [N][K]
   UmmaGemmPlan plan;
 };
 struct BlockW {
@@ -60,8 +57,7 @@ struct b200sep_mdxnet {
   std::vector<UmmaConvPlan> planA, planB;  // per scale: TMA maps over bufA[i] / bufB[i] as conv inputs
   std::vector<char> plan_ok;
   bool pair = false;               // precision 1: activations are bf16 hi/lo pairs
-  std::vector<void*> allocs;
-  int64_t device_bytes = 0;
+  DeviceAllocs mem;
   // optional per-category device timing (bench.py roofline): CUDA events recorded around every launch
   bool profiling = false;
   struct ProfRec { int cat; cudaEvent_t a, b; double flops, bytes; };
@@ -69,35 +65,6 @@ struct b200sep_mdxnet {
 };
 
 namespace b200sep {
-
-struct ParamReader {
-  const float* p;
-  int64_t n, pos = 0;
-  bool ok = true;
-  const float* take(int64_t count) {
-    if (pos + count > n) {
-      ok = false;
-      return p;  // caller checks ok
-    }
-    const float* r = p + pos;
-    pos += count;
-    return r;
-  }
-};
-
-static int dev_alloc(b200sep_mdxnet* net, void** ptr, int64_t bytes) {
-  B2_CUDA(cudaMalloc(ptr, (size_t)bytes));
-  net->allocs.push_back(*ptr);
-  net->device_bytes += bytes;
-  return B200SEP_OK;
-}
-
-static int upload(b200sep_mdxnet* net, float** dst, const std::vector<float>& src) {
-  int rc = dev_alloc(net, (void**)dst, (int64_t)src.size() * sizeof(float));
-  if (rc) return rc;
-  B2_CUDA(cudaMemcpy(*dst, src.data(), src.size() * sizeof(float), cudaMemcpyHostToDevice));
-  return B200SEP_OK;
-}
 
 // BatchNorm(eval) after y = conv(x) + bias:  gamma*(y - mean)/sqrt(var+eps) + beta = y_nobias*s + (bias - mean)*s + beta
 static void fold_bn(int c, const float* bias, const float* gamma, const float* beta, const float* mean, const float* var, std::vector<float>& scale,
@@ -111,37 +78,6 @@ static void fold_bn(int c, const float* bias, const float* gamma, const float* b
     scale[i] = (float)s;
     shift[i] = (float)sh;
   }
-}
-
-static inline uint16_t f2bf(float f) {  // round-to-nearest-even float -> bf16 bits
-  uint32_t u;
-  memcpy(&u, &f, 4);
-  if ((u & 0x7fffffffu) > 0x7f800000u) return (uint16_t)((u >> 16) | 0x40);
-  u += 0x7fffu + ((u >> 16) & 1u);
-  return (uint16_t)(u >> 16);
-}
-static inline float bf2f(uint16_t h) {
-  uint32_t u = (uint32_t)h << 16;
-  float f;
-  memcpy(&f, &u, 4);
-  return f;
-}
-static int upload_u16(b200sep_mdxnet* net, void** dst, const std::vector<uint16_t>& src) {
-  int rc = dev_alloc(net, dst, (int64_t)src.size() * 2);
-  if (rc) return rc;
-  B2_CUDA(cudaMemcpy(*dst, src.data(), src.size() * 2, cudaMemcpyHostToDevice));
-  return B200SEP_OK;
-}
-
-// wgmma B operand of a 3x3 conv (see umma_conv_block_weights)
-static int make_conv_umma(b200sep_mdxnet* net, ConvW& cw, const float* w /*(Cout,Cin,3,3)*/) {
-  umma_conv_choose(cw.cin, cw.n, &cw.kc, &cw.n_tile);
-  std::vector<uint16_t> hi, lo;
-  umma_conv_block_weights(w, cw.n, cw.cin, cw.kc, cw.n_tile, hi, lo);
-  int rc = upload_u16(net, &cw.wb_hi, hi);
-  if (!rc) rc = upload_u16(net, &cw.wb_lo, lo);
-  cw.umma = rc == 0;
-  return rc;
 }
 
 // Conv2d weight (Cout, Cin, kh, kw) -> [Cin][kh*kw][CoutPad]
@@ -161,16 +97,13 @@ static int make_conv(b200sep_mdxnet* net, ParamReader& rd, ConvW& cw, int cin, i
       for (int t = 0; t < taps; ++t) wr[((size_t)ci * taps + t) * cw.n_pad + co] = w[((size_t)co * cin + ci) * taps + t];
   std::vector<float> sc, sh;
   fold_bn(cout, bias, g, be, mu, va, sc, sh);
-  int rc = upload(net, &cw.w, wr);
-  if (!rc) rc = upload(net, &cw.scale, sc);
-  if (!rc) rc = upload(net, &cw.shift, sh);
-  if (!rc && net->pair && stride == 1 && k == 3 && umma_conv_supported(cin, cout, 8, k, k)) rc = make_conv_umma(net, cw, w);
-  if (!rc && net->pair && stride == 2 && k == 2 && umma_updown_supported(cin, cout, 8, 0)) {
-    umma_updown_choose(cin, cout, 0, &cw.kc, &cw.n_tile);
-    std::vector<uint16_t> hi, lo;
-    umma_down_block_weights(w, cout, cin, cw.kc, cw.n_tile, hi, lo);
-    rc = upload_u16(net, &cw.wb_hi, hi);
-    if (!rc) rc = upload_u16(net, &cw.wb_lo, lo);
+  int rc = net->mem.upload_f32(&cw.w, wr.data(), (int64_t)wr.size());
+  if (!rc) rc = net->mem.upload_f32(&cw.scale, sc.data(), cout);
+  if (!rc) rc = net->mem.upload_f32(&cw.shift, sh.data(), cout);
+  const bool conv3 = stride == 1 && k == 3 && umma_conv_supported(cin, cout, 8, k, k);
+  const bool down = stride == 2 && k == 2 && umma_updown_supported(cin, cout, 8, 0);
+  if (!rc && net->pair && (conv3 || down)) {
+    rc = upload_pair_conv(net->mem, conv3 ? UMMA_CONV3 : UMMA_DOWN, w, cin, cout, cw.wb);
     cw.umma = rc == 0;
   }
   return rc;
@@ -191,15 +124,11 @@ static int make_convt(b200sep_mdxnet* net, ParamReader& rd, ConvW& cw, int cin, 
   fold_bn(cout, bias, g, be, mu, va, sc1, sh1);
   for (int q = 0; q < 4; ++q)
     for (int co = 0; co < cout; ++co) { sc[q * cout + co] = sc1[co]; sh[q * cout + co] = sh1[co]; }
-  int rc = upload(net, &cw.w, wr);
-  if (!rc) rc = upload(net, &cw.scale, sc);
-  if (!rc) rc = upload(net, &cw.shift, sh);
+  int rc = net->mem.upload_f32(&cw.w, wr.data(), (int64_t)wr.size());
+  if (!rc) rc = net->mem.upload_f32(&cw.scale, sc.data(), 4 * cout);
+  if (!rc) rc = net->mem.upload_f32(&cw.shift, sh.data(), 4 * cout);
   if (!rc && net->pair && umma_updown_supported(cin, cout, 8, 1)) {
-    umma_updown_choose(cin, cout, 1, &cw.kc, &cw.n_tile);
-    std::vector<uint16_t> hi, lo;
-    umma_up_block_weights(w, cin, cout, cw.kc, cw.n_tile, hi, lo);
-    rc = upload_u16(net, &cw.wb_hi, hi);
-    if (!rc) rc = upload_u16(net, &cw.wb_lo, lo);
+    rc = upload_pair_conv(net->mem, UMMA_UP, w, cin, cout, cw.wb);
     cw.umma = rc == 0;
   }
   return rc;
@@ -210,19 +139,13 @@ static int make_lin(b200sep_mdxnet* net, ParamReader& rd, LinW& lw, int n, int k
   const float* g = rd.take(channels); const float* be = rd.take(channels); const float* mu = rd.take(channels); const float* va = rd.take(channels);
   if (!rd.ok) return B200SEP_ERR_ARG;
   lw.n = n; lw.k = k; lw.channels = channels;
-  std::vector<float> wv(w, w + (size_t)n * k), sc, sh;
+  std::vector<float> sc, sh;
   fold_bn(channels, nullptr, g, be, mu, va, sc, sh);
-  int rc = upload(net, &lw.w, wv);
-  if (!rc) rc = upload(net, &lw.scale, sc);
-  if (!rc) rc = upload(net, &lw.shift, sh);
+  int rc = net->mem.upload_f32(&lw.w, w, (int64_t)n * k);
+  if (!rc) rc = net->mem.upload_f32(&lw.scale, sc.data(), channels);
+  if (!rc) rc = net->mem.upload_f32(&lw.shift, sh.data(), channels);
   if (!rc && net->pair && umma_gemm_supported(1, n, k)) {
-    std::vector<uint16_t> hi((size_t)n * k), lo(hi.size());
-    for (size_t i = 0; i < hi.size(); ++i) {
-      hi[i] = f2bf(w[i]);
-      lo[i] = f2bf(w[i] - bf2f(hi[i]));
-    }
-    rc = upload_u16(net, &lw.w_hi, hi);
-    if (!rc) rc = upload_u16(net, &lw.w_lo, lo);
+    rc = upload_pair_linear(net->mem, w, n, k, lw.wb);
     lw.umma = rc == 0;  // the TMA plan is bound once the activation arena exists
   }
   return rc;
@@ -282,6 +205,13 @@ static inline void* lo_of(const b200sep_mdxnet* net, const float* buf, int scale
   return net->pair ? (void*)((uint16_t*)buf + net->buf_elems[scale]) : nullptr;
 }
 
+// folded BatchNorm + ReLU (+ res) into a pair tensor: the epilogue of every pair launch of this network
+static UmmaEpilogue bn_relu(const float* scale, const float* shift, void* out_hi, void* out_lo, const void* res_hi = nullptr, const void* res_lo = nullptr) {
+  UmmaEpilogue e;
+  e.scale = scale; e.shift = shift; e.act = 1; e.out_hi = out_hi; e.out_lo = out_lo; e.res_hi = res_hi; e.res_lo = res_lo;
+  return e;
+}
+
 // TFC (l x conv3x3+BN+ReLU) then x + TDF(x) (modules.py:20-23, :63-74).  in: bufA, result left in bufB.
 static int run_block(b200sep_mdxnet* net, BlockW& bw, int scale, int B, int c, int T, int F, cudaStream_t st) {
   float* A = net->bufA[scale];
@@ -295,7 +225,7 @@ static int run_block(b200sep_mdxnet* net, BlockW& bw, int scale, int B, int c, i
       const UmmaConvPlan& pl = (src == A) ? net->planA[scale] : net->planB[scale];
       const double pix = (double)B * T * F;
       ProfScope ps(net, st, scale == 0 ? CAT_CONV3X3_S0 : CAT_CONV3X3, 2.0 * pix * cw.n * cw.cin * 9, 4.0 * (pix * cw.cin + pix * cw.n + 9.0 * cw.cin * cw.n));
-      rc = umma_conv_run(pl, cw.wb_hi, cw.wb_lo, B, cw.n, cw.n_tile, cw.kh, cw.scale, cw.shift, 1, dst, lo_of(net, dst, scale), st);
+      rc = umma_conv_run(pl, cw.wb.hi, cw.wb.lo, B, cw.n, cw.wb.n_c, bn_relu(cw.scale, cw.shift, dst, lo_of(net, dst, scale)), st);
     } else {
       rc = run_conv(net, scale == 0 ? CAT_CONV3X3_S0 : CAT_CONV3X3, cw, src, dst, nullptr, B, T, F, 1, EPI_NORMAL, st, lo_of(net, src, scale), lo_of(net, dst, scale));
     }
@@ -308,7 +238,7 @@ static int run_block(b200sep_mdxnet* net, BlockW& bw, int scale, int B, int c, i
   // t1 = relu(bn(x @ W1^T))
   if (net->pair && bw.tdf1.umma) {
     ProfScope ps(net, st, CAT_TDF, 2.0 * M * bw.tdf1.n * (double)F, 4.0 * ((double)M * F + (double)M * bw.tdf1.n + (double)bw.tdf1.n * F));
-    rc = umma_gemm_run(x == Bf ? bw.tdf1.plan : bw.tdf1.plan, bw.tdf1.scale, bw.tdf1.shift, T, c, 1, net->tdf_tmp, tmp_lo, nullptr, nullptr, M, st);
+    rc = umma_gemm_run(bw.tdf1.plan, T, c, M, bn_relu(bw.tdf1.scale, bw.tdf1.shift, net->tdf_tmp, tmp_lo), st);
   } else {
     GemmParams g;
     g.A = x; g.A_lo = lo_of(net, x, scale); g.Bw = bw.tdf1.w; g.scale = bw.tdf1.scale; g.shift = bw.tdf1.shift; g.res = nullptr;
@@ -321,7 +251,7 @@ static int run_block(b200sep_mdxnet* net, BlockW& bw, int scale, int B, int c, i
   // Bf = x + relu(bn(t1 @ W2^T))   (x == Bf when l is odd: in-place residual, each element read then written by one thread)
   if (net->pair && bw.tdf2.umma) {
     ProfScope ps(net, st, CAT_TDF, 2.0 * M * (double)F * bw.tdf2.k, 4.0 * ((double)M * bw.tdf2.k + 2.0 * M * F + (double)F * bw.tdf2.k));
-    rc = umma_gemm_run(bw.tdf2.plan, bw.tdf2.scale, bw.tdf2.shift, T, c, 1, Bf, lo_of(net, Bf, scale), x, lo_of(net, x, scale), M, st);
+    rc = umma_gemm_run(bw.tdf2.plan, T, c, M, bn_relu(bw.tdf2.scale, bw.tdf2.shift, Bf, lo_of(net, Bf, scale), x, lo_of(net, x, scale)), st);
   } else {
     GemmParams g;
     g.A = net->tdf_tmp; g.A_lo = tmp_lo; g.Bw = bw.tdf2.w; g.scale = bw.tdf2.scale; g.shift = bw.tdf2.shift;
@@ -339,9 +269,9 @@ static int bind_block_plans(b200sep_mdxnet* net, BlockW& bw, int scale, int c, i
   const int M = net->cfg.max_batch * c * T;
   float* x = (bw.tfc.size() & 1) ? net->bufB[scale] : net->bufA[scale];
   int rc = B200SEP_OK;
-  if (bw.tdf1.umma) rc = umma_gemm_plan_create(&bw.tdf1.plan, x, lo_of(net, x, scale), bw.tdf1.w_hi, bw.tdf1.w_lo, M, bw.tdf1.n, F);
+  if (bw.tdf1.umma) rc = umma_gemm_plan_create(&bw.tdf1.plan, x, lo_of(net, x, scale), bw.tdf1.wb.hi, bw.tdf1.wb.lo, M, bw.tdf1.n, F);
   if (!rc && bw.tdf2.umma)
-    rc = umma_gemm_plan_create(&bw.tdf2.plan, net->tdf_tmp, (uint16_t*)net->tdf_tmp + net->tdf_tmp_elems, bw.tdf2.w_hi, bw.tdf2.w_lo, M, F, bw.tdf2.k);
+    rc = umma_gemm_plan_create(&bw.tdf2.plan, net->tdf_tmp, (uint16_t*)net->tdf_tmp + net->tdf_tmp_elems, bw.tdf2.wb.hi, bw.tdf2.wb.lo, M, F, bw.tdf2.k);
   return rc;
 }
 
@@ -419,19 +349,18 @@ extern "C" int b200sep_mdxnet_create(b200sep_mdxnet** out, const b200sep_mdxnet_
     const int64_t ci = (int64_t)cfg->g * (i + 1), ti = cfg->dim_t >> i, fi = cfg->dim_f >> i;
     net->buf_elems[i] = (int64_t)cfg->max_batch * ci * ti * fi;
     const int64_t bytes = net->buf_elems[i] * sizeof(float);
-    rc = dev_alloc(net, (void**)&net->bufA[i], bytes);
-    if (!rc) rc = dev_alloc(net, (void**)&net->bufB[i], bytes);
+    rc = net->mem.alloc((void**)&net->bufA[i], bytes);
+    if (!rc) rc = net->mem.alloc((void**)&net->bufB[i], bytes);
     tmp_max = std::max<int64_t>(tmp_max, (int64_t)cfg->max_batch * ci * ti * (fi / cfg->bn));
+    // the 3x3 plans of a scale also serve the 2x2 down / up layers that read bufB[i] (their weights do not depend on the plan's kc)
     if (!rc && net->pair && umma_conv_supported((int)ci, (int)ci, (int)fi, 3, 3)) {
-      int kc, nt;
-      umma_conv_choose((int)ci, (int)ci, &kc, &nt);
-      rc = umma_conv_plan_create(&net->planA[i], net->bufA[i], lo_of(net, net->bufA[i], i), cfg->max_batch, (int)ci, (int)ti, (int)fi, kc);
-      if (!rc) rc = umma_conv_plan_create(&net->planB[i], net->bufB[i], lo_of(net, net->bufB[i], i), cfg->max_batch, (int)ci, (int)ti, (int)fi, kc);
+      rc = umma_conv_plan_create(&net->planA[i], UMMA_CONV3, net->bufA[i], lo_of(net, net->bufA[i], i), cfg->max_batch, (int)ci, (int)ci, (int)ti, (int)fi);
+      if (!rc) rc = umma_conv_plan_create(&net->planB[i], UMMA_CONV3, net->bufB[i], lo_of(net, net->bufB[i], i), cfg->max_batch, (int)ci, (int)ci, (int)ti, (int)fi);
       net->plan_ok[i] = rc == 0;
     }
   }
   net->tdf_tmp_elems = tmp_max;
-  if (!rc) rc = dev_alloc(net, (void**)&net->tdf_tmp, tmp_max * sizeof(float));
+  if (!rc) rc = net->mem.alloc((void**)&net->tdf_tmp, tmp_max * sizeof(float));
   for (int i = 0; i <= n && !rc; ++i) {
     const int ci = cfg->g * (i + 1), ti = cfg->dim_t >> i, fi = cfg->dim_f >> i;
     if (i < n) {
@@ -441,7 +370,7 @@ extern "C" int b200sep_mdxnet_create(b200sep_mdxnet** out, const b200sep_mdxnet_
       rc = bind_block_plans(net, net->bottleneck, i, ci, ti, fi);
     }
   }
-  if (!rc) rc = dev_alloc(net, (void**)&net->io_tmp, (int64_t)cfg->max_batch * cfg->dim_c * cfg->dim_t * cfg->dim_f * sizeof(float));
+  if (!rc) rc = net->mem.alloc((void**)&net->io_tmp, (int64_t)cfg->max_batch * cfg->dim_c * cfg->dim_t * cfg->dim_f * sizeof(float));
   if (rc) {
     b200sep_mdxnet_destroy(net);
     return rc;
@@ -453,11 +382,11 @@ extern "C" int b200sep_mdxnet_create(b200sep_mdxnet** out, const b200sep_mdxnet_
 extern "C" void b200sep_mdxnet_destroy(b200sep_mdxnet* net) {
   if (!net) return;
   for (auto& r : net->prof) { cudaEventDestroy(r.a); cudaEventDestroy(r.b); }
-  for (void* p : net->allocs) cudaFree(p);
+  net->mem.free_all();
   delete net;
 }
 
-extern "C" int64_t b200sep_mdxnet_device_bytes(const b200sep_mdxnet* net) { return net ? net->device_bytes : 0; }
+extern "C" int64_t b200sep_mdxnet_device_bytes(const b200sep_mdxnet* net) { return net ? net->mem.bytes : 0; }
 
 extern "C" int b200sep_mdxnet_forward(b200sep_mdxnet* net, const float* spec_in, float* spec_out, int batch, int layout, void* stream) {
   B2_CHECK_ARG(net && spec_in && spec_out, "mdxnet_forward: NULL argument");
@@ -492,7 +421,7 @@ extern "C" int b200sep_mdxnet_forward(b200sep_mdxnet* net, const float* spec_in,
       const ConvW& cw = net->ds[i];
       const double pix = (double)B * (T / 2) * (F / 2);
       ProfScope ps(net, st, CAT_DOWN, 2.0 * pix * cw.n * cw.cin * 4, 4.0 * ((double)B * cw.cin * T * F + pix * cw.n + 4.0 * cw.cin * cw.n));
-      rc = umma_down_run(net->planB[i], cw.wb_hi, cw.wb_lo, B, cw.n, cw.n_tile, cw.scale, cw.shift, 1, net->bufA[i + 1], lo_of(net, net->bufA[i + 1], i + 1), st);
+      rc = umma_down_run(net->planB[i], cw.wb.hi, cw.wb.lo, B, cw.n, cw.wb.n_c, bn_relu(cw.scale, cw.shift, net->bufA[i + 1], lo_of(net, net->bufA[i + 1], i + 1)), st);
     } else {
       rc = run_conv(net, CAT_DOWN, net->ds[i], net->bufB[i], net->bufA[i + 1], nullptr, B, T, F, 1, EPI_NORMAL, st, lo_of(net, net->bufB[i], i),
                     lo_of(net, net->bufA[i + 1], i + 1));
@@ -509,8 +438,9 @@ extern "C" int b200sep_mdxnet_forward(b200sep_mdxnet* net, const float* spec_in,
       const int cr = cw.n / 4;
       const double pix = (double)B * T * F;
       ProfScope ps(net, st, CAT_UP, 2.0 * pix * cw.n * cw.cin, 4.0 * (pix * cw.cin + 2.0 * pix * cw.n + (double)cw.cin * cw.n));
-      rc = umma_up_run(net->planB[s + 1], cw.wb_hi, cw.wb_lo, B, cr, cw.n_tile, cw.scale, cw.shift, 1, net->bufB[s], lo_of(net, net->bufB[s], s), net->bufA[s],
-                       lo_of(net, net->bufA[s], s), st);
+      // the skip tensor bufB[s] multiplies (UmmaEpilogue::res of the up mode)
+      rc = umma_up_run(net->planB[s + 1], cw.wb.hi, cw.wb.lo, B, cr, cw.wb.n_c,
+                       bn_relu(cw.scale, cw.shift, net->bufA[s], lo_of(net, net->bufA[s], s), net->bufB[s], lo_of(net, net->bufB[s], s)), st);
     } else {
       rc = run_conv(net, CAT_UP, net->us[i], net->bufB[s + 1], net->bufA[s], net->bufB[s], B, T, F, 1, EPI_CONVT2X2, st, lo_of(net, net->bufB[s + 1], s + 1),
                     lo_of(net, net->bufA[s], s), lo_of(net, net->bufB[s], s));

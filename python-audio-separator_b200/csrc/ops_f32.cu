@@ -621,7 +621,7 @@ extern "C" int b200sep_gemm_f32(const float* A, const float* Bw, float* C, int M
                                 int64_t strideB, int64_t strideC, float alpha, const float* bias_n, const float* bias_m, int act, const float* res,
                                 const float* res_scale, const void* w_packed, void* stream) {
   B2_CHECK_ARG(A && Bw && C && M >= 1 && N >= 1 && K >= 1 && batch >= 1 && batch <= 65535, "gemm_f32: bad argument");
-  if (tc_enabled() && tc_gemm_usable(M, N, K, batch))
+  if (tc_gemm_usable(M, N, K, batch))
     return tc_gemm_f32(A, Bw, C, M, N, K, lda, ldb, ldc, batch, strideA, strideB, strideC, alpha, bias_n, bias_m, act, res, res_scale,
                        (batch == 1 || strideB == 0) ? w_packed : nullptr, 0, (cudaStream_t)stream);
   GemmF32 p{A, Bw, C, bias_n, bias_m, res, res_scale, M, N, K, lda, ldb, ldc, strideA, strideB, strideC, alpha, act, 0};
@@ -714,7 +714,7 @@ extern "C" int b200sep_triangle_overlap_add(const float* segs, int n_segs, int c
 extern "C" int b200sep_gemm_kn_f32(const float* A, const float* B_kn, float* C, int M, int N, int K, int lda, int ldb, int ldc, int batch, int64_t strideA, int64_t strideB,
                                    int64_t strideC, float alpha, void* stream) {
   B2_CHECK_ARG(A && B_kn && C && M >= 1 && N >= 1 && K >= 1 && batch >= 1 && lda >= K && ldb >= N && ldc >= N, "gemm_kn_f32: bad argument");
-  if (!(tc_enabled() && tc_gemm_usable(M, N, K, batch))) {  // small shapes: the SIMT kernel reads B transposed
+  if (!tc_gemm_usable(M, N, K, batch)) {  // small shapes: the SIMT kernel reads B transposed
     B2_CHECK_ARG(batch <= 65535, "gemm_kn_f32: batch too large for the SIMT path");
     GemmF32 p{A, B_kn, C, nullptr, nullptr, nullptr, nullptr, M, N, K, lda, ldb, ldc, strideA, strideB, strideC, alpha, 0, 1};
     dim3 grid(cdiv(N, FBN), cdiv(M, FBM), batch);

@@ -16,7 +16,6 @@
 // DConv / rewrite convolutions, the VR CascadedASPPNet convolutions) when the shape is large enough; the SIMT kernels in ops_f32.cu /
 // conv_gen.cu remain for tiny or oddly aligned shapes and for the transposed (scatter) convolution.
 #include <cuda_bf16.h>
-#include <stdlib.h>
 
 #include <algorithm>
 
@@ -65,7 +64,6 @@ struct TcParams {
   // B operand pre-split into the kernel's shared-memory image (tc_pack_*): per (n-tile, k-block) one [hi plane | lo plane] block that a
   // single cp.async.bulk drops into the stage -- static weights cost the producer warps nothing
   const uint8_t* b_packed;
-  int sleep_ns;  // > 0: waiting producer / epilogue warps sleep between polls (B200SEP_WAIT_SLEEP_NS)
 };
 
 __device__ __forceinline__ float tc_act(float v, int act) {
@@ -263,7 +261,7 @@ __global__ void __launch_bounds__(kThreads, 1) tc_f32_kernel(const TcParams p) {
         wi0 = wo * p.SW - p.PW;
       }
       for (int i = 0; i < p.num_iters; ++i) {
-        ptx::mbar_wait_opt(&empty_bar[s], phase ^ 1, p.sleep_ns, 100 + i);
+        ptx::mbar_wait(&empty_bar[s], phase ^ 1);
         uint8_t* st = smem + (size_t)s * p.stage_bytes;
         uint8_t* a_hi = st;
         uint8_t* a_lo = st + p.a_bytes;
@@ -334,7 +332,7 @@ __global__ void __launch_bounds__(kThreads, 1) tc_f32_kernel(const TcParams p) {
     const int m0 = (rem / p.n_tiles) * kTM, n0 = (rem % p.n_tiles) * kTN;
     int prev = -1;
     for (int i = 0; i < p.num_iters; ++i) {
-      ptx::mbar_wait(&full_bar[s], phase, 200 + i);
+      ptx::mbar_wait(&full_bar[s], phase);
       const uint32_t st = ptx::smem_u32(smem + (size_t)s * p.stage_bytes);
       const uint32_t a_hi = st + (uint32_t)wg * 8192u, a_lo = a_hi + p.a_bytes, b_hi = st + 2 * p.a_bytes, b_lo = b_hi + p.b_bytes;
       ptx::wgmma_fence();
@@ -374,8 +372,6 @@ __global__ void __launch_bounds__(kThreads, 1) tc_f32_kernel(const TcParams p) {
   }
 }
 
-static int pick_n_tile(int) { return kTN; }
-
 // one thread per 16-byte chunk of the packed image: (n-tile, k-block, row, chunk)
 __global__ void tc_pack_kernel(const float* __restrict__ src, int conv, int64_t rs, int64_t ks, int N, int K, int Cin, int Cin8, int taps, int n_tile, int num_iters,
                                uint8_t* __restrict__ packed, int64_t total) {
@@ -403,17 +399,8 @@ __global__ void tc_pack_kernel(const float* __restrict__ src, int conv, int64_t 
   }
 }
 
-int wait_sleep_ns() {
-  static const int ns = [] {
-    const char* e = getenv("B200SEP_WAIT_SLEEP_NS");
-    return e ? atoi(e) : 0;
-  }();
-  return ns;
-}
-
 int tc_launch(TcParams& p, cudaStream_t st) {
-  p.sleep_ns = wait_sleep_ns();
-  p.n_tile = pick_n_tile(p.N);
+  p.n_tile = kTN;
   p.stages = 3;
   p.a_bytes = kTM * 128;
   p.b_bytes = (uint32_t)p.n_tile * 128;
@@ -597,12 +584,12 @@ __global__ void __launch_bounds__(kAttThreads, 1) tc_attention_kernel(const AttP
 #pragma unroll
   for (int e = 0; e < kAttD / 2; ++e) O[e] = 0.f;
   const uint32_t qh = ptx::smem_u32(smem) + (uint32_t)wg * 8192u, ql = qh + kAttQBytes;
-  ptx::mbar_wait(q_full, 0, 500);
+  ptx::mbar_wait(q_full, 0);
   for (int j = 0; j < nk; ++j) {
     const int st = j & 1;
     const uint32_t ph = (uint32_t)(j >> 1) & 1u;
     const uint32_t kh = ptx::smem_u32(smem + kAttOffStage + (size_t)st * kAttStage), kl = kh + kAttKBytes;
-    ptx::mbar_wait(&k_full[st], ph, 560 + st);
+    ptx::mbar_wait(&k_full[st], ph);
     float S[kAttKeys / 2];
     ptx::wgmma_fence();
 #pragma unroll
@@ -661,7 +648,7 @@ __global__ void __launch_bounds__(kAttThreads, 1) tc_attention_kernel(const AttP
       O[4 * i + 2] *= corr[1];
       O[4 * i + 3] *= corr[1];
     }
-    ptx::mbar_wait(&v_full[st], ph, 580 + st);
+    ptx::mbar_wait(&v_full[st], ph);
     const uint32_t vh = kh + 2 * kAttKBytes, vl = vh + 2 * kAttVBlk;
     ptx::wgmma_fence();
 #pragma unroll
@@ -704,8 +691,6 @@ __global__ void __launch_bounds__(kAttThreads, 1) tc_attention_kernel(const AttP
 }
 
 }  // namespace
-
-bool tc_attention_usable(int hd, int Lq, int Lk) { return tc_enabled() && hd == kAttD && Lq >= 1 && Lk >= 1; }
 
 // bytes of scratch for the pre-split Q / K / V^T tile images (one 32 KB image per 128-row tile and (batch, head))
 int64_t tc_attention_work_bytes(int B, int H, int Lq, int Lk) {
@@ -751,22 +736,10 @@ int tc_attention_f32(const float* q, const float* k, const float* vt, float* out
   return B200SEP_OK;
 }
 
-
-bool tc_enabled() {
-  static const bool on = [] {
-    const char* e = getenv("B200SEP_TC");
-    return !(e && e[0] == '0');
-  }();
-  return on;
-}
-
-int64_t tc_packed_bytes(int N, int K) {
-  const int nt = pick_n_tile(N);
-  return (int64_t)cdiv(N, nt) * cdiv(K, kTK) * 2 * nt * 128;
-}
+int64_t tc_packed_bytes(int N, int K) { return (int64_t)cdiv(N, kTN) * cdiv(K, kTK) * 2 * kTN * 128; }
 
 int tc_pack_linear(const float* W, int N, int K, int ldw, void* packed, cudaStream_t st) {
-  const int nt = pick_n_tile(N), iters = cdiv(K, kTK);
+  const int nt = kTN, iters = cdiv(K, kTK);
   const int64_t total = (int64_t)cdiv(N, nt) * iters * nt * 8;
   tc_pack_kernel<<<(int)std::min<int64_t>(cdiv(total, 256), kNumSMs * 16), 256, 0, st>>>(W, 0, ldw, 1, N, K, 0, 8, 1, nt, iters, (uint8_t*)packed, total);
   B2_LAUNCHED();
@@ -775,7 +748,7 @@ int tc_pack_linear(const float* W, int N, int K, int ldw, void* packed, cudaStre
 
 int tc_pack_conv(const float* w_blocked, int Cin, int taps, int Cout, int CoutPad, void* packed, cudaStream_t st) {
   const int cin8 = (Cin + 7) / 8 * 8, K = cin8 * taps;
-  const int nt = pick_n_tile(Cout), iters = cdiv(K, kTK);
+  const int nt = kTN, iters = cdiv(K, kTK);
   const int64_t total = (int64_t)cdiv(Cout, nt) * iters * nt * 8;
   tc_pack_kernel<<<(int)std::min<int64_t>(cdiv(total, 256), kNumSMs * 16), 256, 0, st>>>(w_blocked, 1, 0, CoutPad, Cout, K, Cin, cin8, taps, nt, iters, (uint8_t*)packed,
                                                                                           total);

@@ -5,7 +5,7 @@
 
 namespace b200sep {
 
-bool tc_enabled();  // B200SEP_TC=0 in the environment routes everything to the SIMT kernels (A/B measurements)
+// the *_usable predicates pick the tensor-core kernels by shape; smaller or unsupported shapes run on the SIMT kernels
 bool tc_gemm_usable(int M, int N, int K, int batch);
 int tc_gemm_f32(const float* A, const float* Bw, float* C, int M, int N, int K, int lda, int ldb, int ldc, int batch, int64_t sA, int64_t sB, int64_t sC, float alpha,
                 const float* bias_n, const float* bias_m, int act, const float* res, const float* res_scale, const void* w_packed, int b_is_kn,
@@ -15,7 +15,6 @@ int tc_conv2d_f32(const float* x, const float* w_blocked, const float* bias, con
                   int Wo, int KH, int KW, int SH, int SW, int PH, int PW, int DH, int DW, int act, int add_before_act, int out_c_total, int out_c_off, const void* w_packed,
                   cudaStream_t st, int up_axis = 0, int up = 1, int trim = 0, int out_len = 0);
 // fused attention, head dimension 64: out = softmax(alpha q k^T) v with vt = v transposed (keys contiguous); strides in floats (see tc_f32.cu)
-bool tc_attention_usable(int hd, int Lq, int Lk);
 int tc_attention_f32(const float* q, const float* k, const float* vt, float* out, int B, int H, int Lq, int Lk, int64_t q_bs, int64_t q_rs, int64_t k_bs, int64_t k_rs,
                      int64_t vt_bs, int64_t vt_rs, int64_t o_bs, int64_t o_rs, float alpha, int v_kn, void* work, cudaStream_t st);
 int64_t tc_attention_work_bytes(int B, int H, int Lq, int Lk);

@@ -4,12 +4,12 @@
 // per-plane kernel between them (elementwise.cu); TDF layers too small for TMA fall back to the pair-aware SIMT GEMM.
 // Activation layout: (B, C, T, F) pair tensors, F innermost (the network's own layout after transpose(-1,-2), :236).
 #include <math.h>
-#include <string.h>
 
 #include <vector>
 
 #include "common.cuh"
 #include "elementwise.cuh"
+#include "net_builder.cuh"
 #include "simt_ops.cuh"
 #include "umma_ops.cuh"
 
@@ -21,15 +21,14 @@ struct TNorm {
   int c = 0;
 };
 struct TConv {  // any convolution routed through the umma pipeline
-  void* wb_hi = nullptr;
-  void* wb_lo = nullptr;
-  int cin = 0, cout = 0, kc = 0, n_c = 0;
+  PairWeights wb;
+  UmmaConvKind kind = UMMA_CONV3;
+  int cin = 0, cout = 0;
   UmmaConvPlan plan;  // bound to the tensor this layer reads
 };
 struct TLin {
-  float* w = nullptr;    // fp32 [N][K] (SIMT fallback)
-  void* w_hi = nullptr;  // bf16 [N][K]
-  void* w_lo = nullptr;
+  float* w = nullptr;  // fp32 [N][K] (SIMT fallback)
+  PairWeights wb;      // bf16 [N][K]
   int n = 0, k = 0;
   bool umma = false;
   UmmaGemmPlan plan;
@@ -65,130 +64,67 @@ struct b200sep_tfcnet {
   std::vector<PairBuf> X, S, X1, N2, CAT, T1, NT;
   PairBuf MIX, FIRST, FC, FH;  // cws input (dim_c ch), first_conv output (c), final concat (c + dim_c), final hidden (c)
   float* out_cws = nullptr;    // fp32 (B, S*dim_c, T, Fs)
-  std::vector<void*> allocs;
-  int64_t device_bytes = 0;
+  DeviceAllocs mem;
 };
 
 namespace b200sep {
 
-struct TReader {
-  const float* p;
-  int64_t n, pos = 0;
-  bool ok = true;
-  const float* take(int64_t c) {
-    if (pos + c > n) {
-      ok = false;
-      return p;
-    }
-    const float* r = p + pos;
-    pos += c;
-    return r;
-  }
-};
-
-static int t_alloc(b200sep_tfcnet* net, void** ptr, int64_t bytes) {
-  B2_CUDA(cudaMalloc(ptr, (size_t)bytes));
-  net->allocs.push_back(*ptr);
-  net->device_bytes += bytes;
-  return B200SEP_OK;
-}
-static int t_upload_f32(b200sep_tfcnet* net, float** dst, const float* src, int64_t n) {
-  int rc = t_alloc(net, (void**)dst, n * 4);
-  if (rc) return rc;
-  B2_CUDA(cudaMemcpy(*dst, src, n * 4, cudaMemcpyHostToDevice));
-  return B200SEP_OK;
-}
-static int t_upload_u16(b200sep_tfcnet* net, void** dst, const std::vector<uint16_t>& v) {
-  int rc = t_alloc(net, dst, (int64_t)v.size() * 2);
-  if (rc) return rc;
-  B2_CUDA(cudaMemcpy(*dst, v.data(), v.size() * 2, cudaMemcpyHostToDevice));
-  return B200SEP_OK;
-}
 static int t_pair(b200sep_tfcnet* net, PairBuf& b, int64_t elems) {
   b.elems = elems;
-  return t_alloc(net, (void**)&b.p, elems * 4);
+  return net->mem.alloc((void**)&b.p, elems * 4);
 }
 
-static int t_norm(b200sep_tfcnet* net, TReader& rd, TNorm& nm, int c) {
+static int t_norm(b200sep_tfcnet* net, ParamReader& rd, TNorm& nm, int c) {
   const float* g = rd.take(c);
   const float* b = rd.take(c);
   if (!rd.ok) return B200SEP_ERR_ARG;
   nm.c = c;
-  int rc = t_upload_f32(net, &nm.gamma, g, c);
-  if (!rc) rc = t_upload_f32(net, &nm.beta, b, c);
+  int rc = net->mem.upload_f32(&nm.gamma, g, c);
+  if (!rc) rc = net->mem.upload_f32(&nm.beta, b, c);
   return rc;
 }
-enum TKind { K_CONV3, K_PW, K_DOWN, K_UP };
-static int t_conv(b200sep_tfcnet* net, TReader& rd, TConv& cv, int cin, int cout, TKind kind) {
-  const int taps = kind == K_CONV3 ? 9 : (kind == K_PW ? 1 : 4);
+static int t_conv(b200sep_tfcnet* net, ParamReader& rd, TConv& cv, int cin, int cout, UmmaConvKind kind) {
+  const int taps = kind == UMMA_CONV3 ? 9 : (kind == UMMA_PW ? 1 : 4);
   const float* w = rd.take((int64_t)cin * cout * taps);
   if (!rd.ok) return B200SEP_ERR_ARG;
+  cv.kind = kind;
   cv.cin = cin;
   cv.cout = cout;
-  std::vector<uint16_t> hi, lo;
-  if (kind == K_CONV3) {
+  if (kind == UMMA_CONV3)
     B2_CHECK_ARG(umma_conv_supported(cin, cout, 8, 3, 3), "tfcnet: 3x3 conv %d->%d channels is not supported by the tensor-core path (need multiples of 16)", cin, cout);
-    umma_conv_choose(cin, cout, &cv.kc, &cv.n_c);
-    umma_conv_block_weights(w, cout, cin, cv.kc, cv.n_c, hi, lo);
-  } else if (kind == K_PW) {
+  else if (kind == UMMA_PW)
     B2_CHECK_ARG(umma_pw_supported(cin, cout, 8), "tfcnet: 1x1 conv %d->%d channels is not supported by the tensor-core path", cin, cout);
-    umma_pw_choose(cin, cout, &cv.kc, &cv.n_c);
-    umma_pw_block_weights(w, cout, cin, cv.kc, cv.n_c, hi, lo);
-  } else {
-    const int up = kind == K_UP;
-    B2_CHECK_ARG(umma_updown_supported(cin, cout, 8, up), "tfcnet: 2x2 %s conv %d->%d channels is not supported by the tensor-core path", up ? "transposed" : "strided", cin, cout);
-    umma_updown_choose(cin, cout, up, &cv.kc, &cv.n_c);
-    if (up) umma_up_block_weights(w, cin, cout, cv.kc, cv.n_c, hi, lo);
-    else umma_down_block_weights(w, cout, cin, cv.kc, cv.n_c, hi, lo);
-  }
-  int rc = t_upload_u16(net, &cv.wb_hi, hi);
-  if (!rc) rc = t_upload_u16(net, &cv.wb_lo, lo);
-  return rc;
+  else
+    B2_CHECK_ARG(umma_updown_supported(cin, cout, 8, kind == UMMA_UP), "tfcnet: 2x2 %s conv %d->%d channels is not supported by the tensor-core path",
+                 kind == UMMA_UP ? "transposed" : "strided", cin, cout);
+  return upload_pair_conv(net->mem, kind, w, cin, cout, cv.wb);
 }
-static inline uint16_t t_f2bf(float f) {
-  uint32_t u;
-  memcpy(&u, &f, 4);
-  u += 0x7fffu + ((u >> 16) & 1u);
-  return (uint16_t)(u >> 16);
-}
-static inline float t_bf2f(uint16_t h) {
-  uint32_t u = (uint32_t)h << 16;
-  float f;
-  memcpy(&f, &u, 4);
-  return f;
-}
-static int t_lin(b200sep_tfcnet* net, TReader& rd, TLin& ln, int n, int k) {
+static int t_lin(b200sep_tfcnet* net, ParamReader& rd, TLin& ln, int n, int k) {
   const float* w = rd.take((int64_t)n * k);
   if (!rd.ok) return B200SEP_ERR_ARG;
   ln.n = n;
   ln.k = k;
-  int rc = t_upload_f32(net, &ln.w, w, (int64_t)n * k);
+  int rc = net->mem.upload_f32(&ln.w, w, (int64_t)n * k);
   if (!rc && umma_gemm_supported(1, n, k)) {
-    std::vector<uint16_t> hi((size_t)n * k), lo(hi.size());
-    for (size_t i = 0; i < hi.size(); ++i) {
-      hi[i] = t_f2bf(w[i]);
-      lo[i] = t_f2bf(w[i] - t_bf2f(hi[i]));
-    }
-    rc = t_upload_u16(net, &ln.w_hi, hi);
-    if (!rc) rc = t_upload_u16(net, &ln.w_lo, lo);
+    rc = upload_pair_linear(net->mem, w, n, k, ln.wb);
     ln.umma = rc == 0;
   }
   return rc;
 }
-static int t_block(b200sep_tfcnet* net, TReader& rd, TBlock& blk, int in_c, int c, int f) {
+static int t_block(b200sep_tfcnet* net, ParamReader& rd, TBlock& blk, int in_c, int c, int f) {
   const b200sep_tfcnet_config& cfg = net->cfg;
   blk.inner.resize(cfg.l);
   for (int i = 0; i < cfg.l; ++i) {
     TInner& ib = blk.inner[i];
     int rc = t_norm(net, rd, ib.n1, in_c);
-    if (!rc) rc = t_conv(net, rd, ib.tfc1, in_c, c, K_CONV3);
+    if (!rc) rc = t_conv(net, rd, ib.tfc1, in_c, c, UMMA_CONV3);
     if (!rc) rc = t_norm(net, rd, ib.n2, c);
     if (!rc) rc = t_lin(net, rd, ib.lin1, f / cfg.bn, f);
     if (!rc) rc = t_norm(net, rd, ib.n3, c);
     if (!rc) rc = t_lin(net, rd, ib.lin2, f, f / cfg.bn);
     if (!rc) rc = t_norm(net, rd, ib.n4, c);
-    if (!rc) rc = t_conv(net, rd, ib.tfc2, c, c, K_CONV3);
-    if (!rc) rc = t_conv(net, rd, ib.shortcut, in_c, c, K_PW);
+    if (!rc) rc = t_conv(net, rd, ib.tfc2, c, c, UMMA_CONV3);
+    if (!rc) rc = t_conv(net, rd, ib.shortcut, in_c, c, UMMA_PW);
     if (rc) return rc;
     in_c = c;
   }
@@ -205,11 +141,11 @@ static int64_t t_block_params(const b200sep_tfcnet_config& c, int64_t in_c, int6
 
 // bind a conv layer's TMA plan to its input tensor (B, cin, T, F)
 static int t_bind(const b200sep_tfcnet* net, TConv& cv, const PairBuf& in, int T, int F) {
-  return umma_conv_plan_create(&cv.plan, in.hi(), in.lo(), net->cfg.max_batch, cv.cin, T, F, cv.kc);
+  return umma_conv_plan_create(&cv.plan, cv.kind, in.hi(), in.lo(), net->cfg.max_batch, cv.cin, cv.cout, T, F);
 }
 static int t_bind_lin(const b200sep_tfcnet* net, TLin& ln, const PairBuf& a, int M) {
   if (!ln.umma) return B200SEP_OK;
-  return umma_gemm_plan_create(&ln.plan, a.hi(), a.lo(), ln.w_hi, ln.w_lo, M, ln.n, ln.k);
+  return umma_gemm_plan_create(&ln.plan, a.hi(), a.lo(), ln.wb.hi, ln.wb.lo, M, ln.n, ln.k);
 }
 static int t_bind_block(b200sep_tfcnet* net, TBlock& blk, int scale, const PairBuf& xin, int c, int T, int F) {
   const PairBuf* in = &xin;
@@ -232,7 +168,7 @@ static int t_linear(const TLin& ln, const PairBuf& a, int M, const PairBuf& out,
     UmmaEpilogue e;
     e.out_hi = out.hi(); e.out_lo = out.lo();
     if (res) { e.res_hi = res->hi(); e.res_lo = res->lo(); }
-    return umma_gemm_run_ex(ln.plan, 1, 1, M, e, st);
+    return umma_gemm_run(ln.plan, 1, 1, M, e, st);
   }
   GemmParams g;
   g.A = (const float*)a.hi(); g.A_lo = a.lo(); g.Bw = ln.w; g.scale = nullptr; g.shift = nullptr;
@@ -257,14 +193,14 @@ static int t_run_block(b200sep_tfcnet* net, TBlock& blk, int scale, const PairBu
     UmmaEpilogue e;
     // s = shortcut(x)
     e.out_hi = net->S[scale].hi(); e.out_lo = net->S[scale].lo();
-    rc = umma_pw_run_ex(ib.shortcut.plan, ib.shortcut.wb_hi, ib.shortcut.wb_lo, B, c, ib.shortcut.n_c, e, st);
+    rc = umma_pw_run(ib.shortcut.plan, ib.shortcut.wb.hi, ib.shortcut.wb.lo, B, c, ib.shortcut.wb.n_c, e, st);
     if (rc) return rc;
     // x1 = tfc1(act(norm(x)))
     rc = instnorm_act_pair(in->hi(), in->lo(), in_c, 0, ib.n1.gamma, ib.n1.beta, 2, net->N2[scale].hi(), net->N2[scale].lo(), B, in_c, P, st);
     if (rc) return rc;
     e = UmmaEpilogue();
     e.out_hi = net->X1[scale].hi(); e.out_lo = net->X1[scale].lo();
-    rc = umma_conv_run_ex(ib.tfc1.plan, ib.tfc1.wb_hi, ib.tfc1.wb_lo, B, c, ib.tfc1.n_c, e, st);
+    rc = umma_conv_run(ib.tfc1.plan, ib.tfc1.wb.hi, ib.tfc1.wb.lo, B, c, ib.tfc1.wb.n_c, e, st);
     if (rc) return rc;
     // x1 += tdf(x1): lin2(act(norm(lin1(act(norm(x1))))))
     rc = instnorm_act_pair(net->X1[scale].hi(), net->X1[scale].lo(), c, 0, ib.n2.gamma, ib.n2.beta, 2, net->N2[scale].hi(), net->N2[scale].lo(), B, c, P, st);
@@ -286,7 +222,7 @@ static int t_run_block(b200sep_tfcnet* net, TBlock& blk, int scale, const PairBu
     } else {
       e.out_hi = net->X[scale].hi(); e.out_lo = net->X[scale].lo();
     }
-    rc = umma_conv_run_ex(ib.tfc2.plan, ib.tfc2.wb_hi, ib.tfc2.wb_lo, B, c, ib.tfc2.n_c, e, st);
+    rc = umma_conv_run(ib.tfc2.plan, ib.tfc2.wb.hi, ib.tfc2.wb.lo, B, c, ib.tfc2.wb.n_c, e, st);
     if (rc) return rc;
     in = &net->X[scale];
     in_c = c;
@@ -318,7 +254,7 @@ extern "C" int64_t b200sep_tfcnet_param_count(const b200sep_tfcnet_config* c) {
 
 extern "C" void b200sep_tfcnet_destroy(b200sep_tfcnet* net) {
   if (!net) return;
-  for (void* p : net->allocs) cudaFree(p);
+  net->mem.free_all();
   delete net;
 }
 
@@ -342,25 +278,25 @@ extern "C" int b200sep_tfcnet_create(b200sep_tfcnet** out, const b200sep_tfcnet_
   net->dim_c = cfg->num_subbands * cfg->audio_channels * 2;
   net->Fs = Fs;
   const int dim_c = net->dim_c, c0 = cfg->c, g = cfg->g, T0 = cfg->dim_t, Bm = cfg->max_batch;
-  TReader rd{params_host, n_params};
-  int rc = t_conv(net, rd, net->first, dim_c, c0, K_PW);
+  ParamReader rd{params_host, n_params};
+  int rc = t_conv(net, rd, net->first, dim_c, c0, UMMA_PW);
   net->enc.resize(n); net->dec.resize(n); net->down.resize(n); net->up.resize(n); net->down_norm.resize(n); net->up_norm.resize(n);
   int f = Fs, c = c0;
   for (int i = 0; i < n && !rc; ++i) {
     rc = t_block(net, rd, net->enc[i], c, c, f);
     if (!rc) rc = t_norm(net, rd, net->down_norm[i], c);
-    if (!rc) rc = t_conv(net, rd, net->down[i], c, c + g, K_DOWN);
+    if (!rc) rc = t_conv(net, rd, net->down[i], c, c + g, UMMA_DOWN);
     f /= 2; c += g;
   }
   if (!rc) rc = t_block(net, rd, net->bottleneck, c, c, f);
   for (int i = 0; i < n && !rc; ++i) {
     rc = t_norm(net, rd, net->up_norm[i], c);
-    if (!rc) rc = t_conv(net, rd, net->up[i], c, c - g, K_UP);
+    if (!rc) rc = t_conv(net, rd, net->up[i], c, c - g, UMMA_UP);
     f *= 2; c -= g;
     if (!rc) rc = t_block(net, rd, net->dec[i], 2 * c, c, f);
   }
-  if (!rc) rc = t_conv(net, rd, net->final0, c + dim_c, c, K_PW);
-  if (!rc) rc = t_conv(net, rd, net->final2, c, cfg->num_targets * dim_c, K_PW);
+  if (!rc) rc = t_conv(net, rd, net->final0, c + dim_c, c, UMMA_PW);
+  if (!rc) rc = t_conv(net, rd, net->final2, c, cfg->num_targets * dim_c, UMMA_PW);
   if (!rc && (!rd.ok || rd.pos != n_params)) {
     set_error("tfcnet_create: parameter blob size mismatch (consumed %lld of %lld)", (long long)rd.pos, (long long)n_params);
     rc = B200SEP_ERR_ARG;
@@ -383,7 +319,7 @@ extern "C" int b200sep_tfcnet_create(b200sep_tfcnet** out, const b200sep_tfcnet_
   if (!rc) rc = t_pair(net, net->FIRST, px * c0);
   if (!rc) rc = t_pair(net, net->FC, px * (c0 + dim_c));
   if (!rc) rc = t_pair(net, net->FH, px * c0);
-  if (!rc) rc = t_alloc(net, (void**)&net->out_cws, px * cfg->num_targets * dim_c * 4);
+  if (!rc) rc = net->mem.alloc((void**)&net->out_cws, px * cfg->num_targets * dim_c * 4);
   // ---- bind TMA plans to the buffers each layer reads
   if (!rc) rc = t_bind(net, net->first, net->MIX, T0, Fs);
   for (int i = 0; i < n && !rc; ++i) {
@@ -408,7 +344,7 @@ extern "C" int b200sep_tfcnet_create(b200sep_tfcnet** out, const b200sep_tfcnet_
   return B200SEP_OK;
 }
 
-extern "C" int64_t b200sep_tfcnet_device_bytes(const b200sep_tfcnet* net) { return net ? net->device_bytes : 0; }
+extern "C" int64_t b200sep_tfcnet_device_bytes(const b200sep_tfcnet* net) { return net ? net->mem.bytes : 0; }
 
 extern "C" int b200sep_tfcnet_forward(b200sep_tfcnet* net, const float* spec_in, float* spec_out, int batch, void* stream) {
   B2_CHECK_ARG(net && spec_in && spec_out, "tfcnet_forward: NULL argument");
@@ -423,7 +359,7 @@ extern "C" int b200sep_tfcnet_forward(b200sep_tfcnet* net, const float* spec_in,
   if (rc) return rc;
   UmmaEpilogue e;
   e.out_hi = net->FIRST.hi(); e.out_lo = net->FIRST.lo();
-  rc = umma_pw_run_ex(net->first.plan, net->first.wb_hi, net->first.wb_lo, B, c0, net->first.n_c, e, st);  // first_conv (:234)
+  rc = umma_pw_run(net->first.plan, net->first.wb.hi, net->first.wb.lo, B, c0, net->first.wb.n_c, e, st);  // first_conv (:234)
   if (rc) return rc;
   int c = c0, T = T0, F = Fs;
   for (int i = 0; i < n; ++i) {  // encoder (:239-242): block output goes straight into the second half of the decoder's concat buffer
@@ -433,7 +369,7 @@ extern "C" int b200sep_tfcnet_forward(b200sep_tfcnet* net, const float* spec_in,
     if (rc) return rc;
     e = UmmaEpilogue();
     e.out_hi = net->X[i + 1].hi(); e.out_lo = net->X[i + 1].lo();
-    rc = umma_down_run_ex(net->down[i].plan, net->down[i].wb_hi, net->down[i].wb_lo, B, c + g, net->down[i].n_c, e, st);
+    rc = umma_down_run(net->down[i].plan, net->down[i].wb.hi, net->down[i].wb.lo, B, c + g, net->down[i].wb.n_c, e, st);
     if (rc) return rc;
     c += g; T /= 2; F /= 2;
   }
@@ -445,7 +381,7 @@ extern "C" int b200sep_tfcnet_forward(b200sep_tfcnet* net, const float* spec_in,
     if (rc) return rc;
     e = UmmaEpilogue();
     e.out_hi = net->CAT[s].hi(); e.out_lo = net->CAT[s].lo(); e.out_c_total = 2 * (c - g); e.out_c_off = 0;
-    rc = umma_up_run_ex(net->up[i].plan, net->up[i].wb_hi, net->up[i].wb_lo, B, c - g, net->up[i].n_c, e, st);
+    rc = umma_up_run(net->up[i].plan, net->up[i].wb.hi, net->up[i].wb.lo, B, c - g, net->up[i].wb.n_c, e, st);
     if (rc) return rc;
     c -= g; T *= 2; F *= 2;
     const bool last = s == 0;  // the last decoder block writes x * first_conv_out into channels [dim_c, dim_c + c) of the final concat
@@ -454,11 +390,11 @@ extern "C" int b200sep_tfcnet_forward(b200sep_tfcnet* net, const float* spec_in,
   }
   e = UmmaEpilogue();  // final_conv: 1x1 -> GELU -> 1x1 (:257)
   e.out_hi = net->FH.hi(); e.out_lo = net->FH.lo(); e.act = 2;
-  rc = umma_pw_run_ex(net->final0.plan, net->final0.wb_hi, net->final0.wb_lo, B, c0, net->final0.n_c, e, st);
+  rc = umma_pw_run(net->final0.plan, net->final0.wb.hi, net->final0.wb.lo, B, c0, net->final0.wb.n_c, e, st);
   if (rc) return rc;
   e = UmmaEpilogue();
   e.out_f32 = net->out_cws;
-  rc = umma_pw_run_ex(net->final2.plan, net->final2.wb_hi, net->final2.wb_lo, B, cfg.num_targets * dim_c, net->final2.n_c, e, st);
+  rc = umma_pw_run(net->final2.plan, net->final2.wb.hi, net->final2.wb.lo, B, cfg.num_targets * dim_c, net->final2.wb.n_c, e, st);
   if (rc) return rc;
   return cws_merge_f32(net->out_cws, spec_out, B, cfg.num_targets, 4, T0, K, Fs, st);  // cws2cac + (B,S,4,F,T) view (:259-263)
 }

@@ -36,29 +36,11 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
 }
 // Bounded wait: a protocol bug would otherwise hang the GPU; after ~seconds of polling the kernel traps instead
 // (surfaces as a launch failure on the host).  try_wait itself suspends the thread, so the poll count stays tiny.  No diagnostic print:
-// a function call inside a kernel that issues wgmma makes ptxas serialise the whole wgmma pipeline.  `tag` names the wait site for a debug build.
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity, int tag = 0) {
-  (void)tag;
+// a function call inside a kernel that issues wgmma makes ptxas serialise the whole wgmma pipeline.
+__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   uint32_t spins = 0;
   while (!mbar_try_wait(bar, parity))
     if (++spins > (1u << 22)) __trap();
-}
-
-// The same with a sleep between polls: a warp that spins on try_wait occupies issue slots of its scheduler; roles with slack (producers waiting for a
-// free slot) should not take them from the warps on the critical path.
-__device__ __forceinline__ void mbar_wait_backoff(uint64_t* bar, uint32_t parity, unsigned ns, int tag = 0) {
-  (void)tag;
-  uint32_t spins = 0;
-  while (!mbar_try_wait(bar, parity)) {
-    __nanosleep(ns);
-    if (++spins > (1u << 22)) __trap();
-  }
-}
-
-// ns == 0: the plain bounded wait; otherwise the sleeping one
-__device__ __forceinline__ void mbar_wait_opt(uint64_t* bar, uint32_t parity, int ns, int tag = 0) {
-  if (ns > 0) mbar_wait_backoff(bar, parity, (unsigned)ns, tag);
-  else mbar_wait(bar, parity, tag);
 }
 
 // ---- TMA ----------------------------------------------------------------------------------------------

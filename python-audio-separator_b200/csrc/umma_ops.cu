@@ -18,7 +18,6 @@
 //          shuffles (+ a small smem exchange at warp edges).
 // Warp roles per CTA (288 threads): warps 0-7 = two consumer warpgroups (wgmma issue + epilogue), warp 8 = TMA producer.
 #include <cuda_bf16.h>
-#include <stdlib.h>
 #include <string.h>
 
 #include <map>
@@ -49,7 +48,6 @@ struct UmmaParams {
   uint32_t b_res_off;          //   byte offset of the resident image [num_iters][hi | lo] from the start of dynamic shared memory (after alignment)
   int n_tile, n_total;
   int num_iters, ksteps, stages;
-  int sleep_ns;  // > 0: the waiting producer sleeps between polls (B200SEP_WAIT_SLEEP_NS)
   int num_tiles, n_ftiles, t_tiles;  // persistent tile walk (n_tiles below = tiles along N / output channels)
   uint32_t a_bytes, b_bytes, stage_bytes;
   // CONV
@@ -122,7 +120,7 @@ __device__ __forceinline__ void umma_producer_loop(const CUtensorMap& tmA_hi, co
     const TileCoord tc = decode_tile(p, tile);
     const int n0 = tc.n_idx * p.n_tile;
     for (int i = 0; i < p.num_iters; ++i) {
-      ptx::mbar_wait_opt(&empty_bar[s], phase ^ 1, p.sleep_ns, 100 + i);
+      ptx::mbar_wait(&empty_bar[s], phase ^ 1);
       uint8_t* st = smem + (size_t)s * p.stage_bytes;
       uint8_t* a_hi = st;
       uint8_t* a_lo = st + p.a_bytes;
@@ -164,7 +162,7 @@ template <class Mma>
 __device__ __forceinline__ void consumer_mainloop(const UmmaParams& p, uint8_t* smem, uint64_t* full_bar, uint64_t* empty_bar, int& s, uint32_t& phase, Mma mma) {
   int prev = -1;
   for (int i = 0; i < p.num_iters; ++i) {
-    ptx::mbar_wait(&full_bar[s], phase, 200 + i);
+    ptx::mbar_wait(&full_bar[s], phase);
     const uint32_t st = ptx::smem_u32(smem + (size_t)s * p.stage_bytes);
     const uint32_t a_hi = st, a_lo = st + p.a_bytes;
     const uint32_t b_hi = p.b_resident ? ptx::smem_u32(smem + p.b_res_off + (size_t)i * 2 * p.b_bytes) : st + 2 * p.a_bytes, b_lo = b_hi + p.b_bytes;
@@ -441,7 +439,7 @@ __global__ void __launch_bounds__(kUmmaThreads, 1) umma_conv3_kernel(const __gri
   const int wg = warp >> 2, g = lane >> 2, cq = lane & 3;
   const int mrow0 = wg * 64 + (warp & 3) * 16 + g;  // tile rows mrow0 and mrow0 + 8
   const bool issuer = threadIdx.x == 0;             // owns the bulk store groups
-  if (p.b_resident) ptx::mbar_wait(wres_bar, 0, 500);  // the resident weight image has landed
+  if (p.b_resident) ptx::mbar_wait(wres_bar, 0);  // the resident weight image has landed
   int s = 0;
   uint32_t phase = 0;
   float acc[3 * NC / 2];
@@ -560,14 +558,6 @@ static int num_sms() {
   return n;
 }
 
-static int umma_wait_sleep_ns() {
-  static const int ns = [] {
-    const char* e = getenv("B200SEP_WAIT_SLEEP_NS");
-    return e ? atoi(e) : 0;
-  }();
-  return ns;
-}
-
 // Persistent launch: one CTA per SM.
 template <class Kernel, class... Args>
 static int launch_persistent(Kernel kernel, int num_tiles, size_t smem, cudaStream_t st, Args... args) {
@@ -580,7 +570,6 @@ static int launch_persistent(Kernel kernel, int num_tiles, size_t smem, cudaStre
 // `tiles` is the logical tile grid: GEMM (n tiles, m tiles, 1); conv modes (f tiles, output rows, batch * channel tiles).
 static int launch(const CUtensorMap& a_hi, const CUtensorMap& a_lo, const CUtensorMap& b_hi, const CUtensorMap& b_lo, UmmaParams& p, dim3 tiles,
                   cudaStream_t st) {
-  p.sleep_ns = umma_wait_sleep_ns();
   B2_CHECK_ARG(p.n_tile % 16 == 0 && p.n_tile >= 16 && p.n_tile <= kMaxNTile, "umma: n_tile=%d is not a multiple of 16 in [16, %d]", p.n_tile, kMaxNTile);
   p.stage_bytes = ((2 * p.a_bytes + 2 * p.b_bytes + 1023) / 1024) * 1024;
   if (p.mode == 0) p.n_tiles = (int)tiles.x;
@@ -603,6 +592,130 @@ static int launch(const CUtensorMap& a_hi, const CUtensorMap& a_lo, const CUtens
   return launch_persistent(umma_pair_kernel, p.num_tiles, smem, st, a_hi, a_lo, b_hi, b_lo, p);
 }
 
+static void fill_epilogue(UmmaParams& p, const UmmaEpilogue& e, int Cout) {
+  p.scale = e.scale; p.shift = e.shift; p.act = e.act;
+  p.out_hi = (bf16*)e.out_hi; p.out_lo = (bf16*)e.out_lo; p.out_f32 = e.out_f32;
+  p.res_hi = (const bf16*)e.res_hi; p.res_lo = (const bf16*)e.res_lo;
+  p.mul_hi = (const bf16*)e.mul_hi; p.mul_lo = (const bf16*)e.mul_lo;
+  p.out_c_total = e.out_c_total > 0 ? e.out_c_total : Cout;
+  p.out_c_off = e.out_c_off;
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// weights in the pair format: every on-device image the kernels above read is written here
+
+static uint16_t f2bf(float f) {  // round-to-nearest-even float -> bf16 bits; NaN stays NaN
+  uint32_t u;
+  memcpy(&u, &f, 4);
+  if ((u & 0x7fffffffu) > 0x7f800000u) return (uint16_t)((u >> 16) | 0x40);
+  u += 0x7fffu + ((u >> 16) & 1u);
+  return (uint16_t)(u >> 16);
+}
+static float bf2f(uint16_t h) {
+  uint32_t u = (uint32_t)h << 16;
+  float f;
+  memcpy(&f, &u, 4);
+  return f;
+}
+
+void umma_gemm_split_weights(const float* w, int N, int K, std::vector<uint16_t>& hi, std::vector<uint16_t>& lo) {
+  hi.resize((size_t)N * K);
+  lo.resize(hi.size());
+  for (size_t i = 0; i < hi.size(); ++i) {
+    hi[i] = f2bf(w[i]);
+    lo[i] = f2bf(w[i] - bf2f(hi[i]));
+  }
+}
+
+static int pick_nc(int Cout, int mult, int limit) {  // largest n_c | Cout with mult*n_c <= limit and mult*n_c % 16 == 0
+  for (int nc = Cout; nc >= 4; --nc)
+    if (Cout % nc == 0 && mult * nc <= limit && (mult * nc) % 16 == 0 && nc % 16 == 0) return nc;
+  return 0;
+}
+
+int umma_n_c(UmmaConvKind kind, int Cout) {
+  switch (kind) {
+    case UMMA_CONV3:  // 3*n_c accumulator columns <= 240
+      for (int nc : {48, 80, 64, 32, 16})
+        if (Cout % nc == 0) return nc;
+      return 16;
+    case UMMA_UP: return pick_nc(Cout, 4, kMaxNTile);
+    case UMMA_DOWN: return pick_nc(Cout, 2, kMaxNTile);
+    case UMMA_PW: return pick_nc(Cout, 1, kMaxNTile);
+  }
+  return 0;
+}
+
+int umma_kc(UmmaConvKind kind, int Cin, int Cout) {
+  int k = 64;
+  while (k > 16 && Cin % k != 0) k -= 16;
+  if (Cin % 48 == 0) k = 48;
+  if (kind != UMMA_CONV3) return k;
+  // the 3x3 ring needs at least two stages next to the output staging tile of the TMA-store epilogue: shrink the channel step of wide tiles
+  // (n_c = 80 with 64 channels per stage is a 92 KB stage: MDX23C's 640-channel scale)
+  const int nc = umma_n_c(kind, Cout);
+  auto fits = [&](int kk) {
+    const size_t stage = ((size_t)2 * kk * 256 + (size_t)2 * (kk / 16) * (3 * nc) * 32 + 1023) / 1024 * 1024;
+    const size_t staging = (size_t)2 * nc * kConvStride * 2;  // hi + lo output planes
+    return 2 * stage + staging + 16 * 1024 <= 227 * 1024;
+  };
+  while (!fits(k) && k > 16) {
+    int kk = k - 16;
+    while (kk > 16 && Cin % kk != 0) kk -= 16;
+    if (Cin % kk != 0) break;
+    k = kk;
+  }
+  return k;
+}
+
+// Blocking: [Cout/n_c][row tap r][Cin/16] blocks of [rows][16 k], each stored as 8x8 core matrices (K-major, no swizzle).  rows = the accumulator
+// columns of one CTA in the order the epilogues read them (umma_pair_kernel / umma_conv3_kernel).
+// The image depends on n_c only, not on the plan's kc: a pipeline stage of kc input channels reads kc/16 consecutive blocks, so every kc walks the
+// same stream.  A layer may therefore read its input through a plan made for another layer on the same buffer.
+int umma_block_weights(UmmaConvKind kind, const float* w, int Cin, int Cout, std::vector<uint16_t>& hi, std::vector<uint16_t>& lo) {
+  const int n_c = umma_n_c(kind, Cout);
+  int n_r = 1, cols = 1;  // row taps; accumulator columns per output channel
+  if (kind == UMMA_CONV3) n_r = cols = 3;
+  if (kind == UMMA_UP) cols = 4;
+  if (kind == UMMA_DOWN) n_r = cols = 2;
+  const int rows = cols * n_c;
+  auto value = [&](int co0, int row, int r, int ci) {
+    switch (kind) {
+      case UMMA_CONV3: {  // (Cout, Cin, 3, 3), row tap r = dy; rows (dx, co)
+        const int dx = row / n_c, co = co0 + row % n_c;
+        return w[(((size_t)co * Cin + ci) * 3 + r) * 3 + dx];
+      }
+      case UMMA_UP: {  // ConvTranspose2d (Cin, Cout, 2, 2); rows (co, q = dy*2 + dx)
+        const int q = row & 3, co = co0 + (row >> 2);
+        return w[((size_t)ci * Cout + co) * 4 + q];
+      }
+      case UMMA_DOWN: {  // Conv2d (Cout, Cin, 2, 2) stride 2, row tap r = dy; rows (co, dx)
+        const int dx = row & 1, co = co0 + (row >> 1);
+        return w[(((size_t)co * Cin + ci) * 2 + r) * 2 + dx];
+      }
+      default:  // Conv2d (Cout, Cin, 1, 1); rows co
+        return w[(size_t)(co0 + row) * Cin + ci];
+    }
+  };
+  hi.assign((size_t)(Cout / n_c) * n_r * Cin * rows, 0);
+  lo.assign(hi.size(), 0);
+  size_t pos = 0;
+  for (int nt = 0; nt < Cout / n_c; ++nt)
+    for (int r = 0; r < n_r; ++r)
+      for (int kb = 0; kb < Cin / 16; ++kb, pos += (size_t)rows * 16)
+        for (int row = 0; row < rows; ++row)
+          for (int kk = 0; kk < 16; ++kk) {
+            const float v = value(nt * n_c, row, r, kb * 16 + kk);
+            const size_t o = pos + (size_t)((row / 8) * 2 + kk / 8) * 64 + (row % 8) * 8 + (kk % 8);
+            hi[o] = f2bf(v);
+            lo[o] = f2bf(v - bf2f(hi[o]));
+          }
+  return n_c;
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// GEMM
+
 bool umma_gemm_supported(int M, int N, int K) { return M >= 1 && N % 16 == 0 && K % 8 == 0 && N >= 16 && K >= 16; }
 
 int umma_gemm_plan_create(UmmaGemmPlan* pl, const void* a_hi, const void* a_lo, const void* w_hi, const void* w_lo, int M, int N, int K) {
@@ -624,72 +737,31 @@ int umma_gemm_plan_create(UmmaGemmPlan* pl, const void* a_hi, const void* a_lo, 
   return rc;
 }
 
-static void fill_epilogue(UmmaParams& p, const UmmaEpilogue& e, int Cout) {
-  p.scale = e.scale; p.shift = e.shift; p.act = e.act;
-  p.out_hi = (bf16*)e.out_hi; p.out_lo = (bf16*)e.out_lo; p.out_f32 = e.out_f32;
-  p.res_hi = (const bf16*)e.res_hi; p.res_lo = (const bf16*)e.res_lo;
-  p.mul_hi = (const bf16*)e.mul_hi; p.mul_lo = (const bf16*)e.mul_lo;
-  p.out_c_total = e.out_c_total > 0 ? e.out_c_total : Cout;
-  p.out_c_off = e.out_c_off;
-}
-
-int umma_gemm_run(const UmmaGemmPlan& pl, const float* scale, const float* shift, int rows_per_channel, int channels, int relu, void* out_hi,
-                  void* out_lo, const void* res_hi, const void* res_lo, int M_active, cudaStream_t st) {
-  UmmaEpilogue e;
-  e.scale = scale; e.shift = shift; e.act = relu ? 1 : 0; e.out_hi = out_hi; e.out_lo = out_lo; e.res_hi = res_hi; e.res_lo = res_lo;
-  return umma_gemm_run_ex(pl, rows_per_channel, channels, M_active, e, st);
-}
-
-int umma_gemm_run_ex(const UmmaGemmPlan& pl, int rows_per_channel, int channels, int M_active, const UmmaEpilogue& e, cudaStream_t st) {
-  const float* scale = e.scale; const float* shift = e.shift; const int relu = e.act;
-  void* out_hi = e.out_hi; void* out_lo = e.out_lo; const void* res_hi = e.res_hi; const void* res_lo = e.res_lo;
+int umma_gemm_run(const UmmaGemmPlan& pl, int rows_per_channel, int channels, int M_active, const UmmaEpilogue& e, cudaStream_t st) {
   UmmaParams p{};
   p.mode = 0;
   p.n_tile = pl.n_tile; p.n_total = pl.N;
   p.num_iters = (pl.K + 63) / 64; p.ksteps = 4;
   p.a_bytes = 128 * 128; p.b_bytes = (uint32_t)pl.n_tile * 128;
   p.M = M_active; p.K = pl.K; p.rows_per_channel = rows_per_channel; p.channels = channels;
-  p.scale = scale; p.shift = shift; p.act = relu;
-  p.out_hi = (bf16*)out_hi; p.out_lo = (bf16*)out_lo; p.res_hi = (const bf16*)res_hi; p.res_lo = (const bf16*)res_lo;
+  fill_epilogue(p, e, pl.N);
   dim3 grid(pl.N / pl.n_tile, cdiv(M_active, kTileM));
   return launch(pl.a_hi, pl.a_lo, pl.b_hi, pl.b_lo, p, grid, st);
 }
 
+// ---------------------------------------------------------------------------------------------------------
+// convolutions
+
 bool umma_conv_supported(int Cin, int Cout, int F, int kh, int kw) {
   return Cin % 16 == 0 && Cout % 16 == 0 && F % 8 == 0 && kh == 3 && kw == 3;
 }
-
-// kc = input channels per pipeline stage, n_c = output channels per CTA (3*n_c accumulator columns <= 256)
-int umma_conv_choose(int Cin, int Cout, int* kc, int* n_c) {
-  int k = 64;
-  while (k > 16 && Cin % k != 0) k -= 16;
-  if (Cin % 48 == 0) k = 48;
-  int nc = 16;
-  const int cand[5] = {48, 80, 64, 32, 16};
-  for (int i = 0; i < 5; ++i)
-    if (Cout % cand[i] == 0) {
-      nc = cand[i];
-      break;
-    }
-  // the ring needs at least two stages next to the output staging tile of the TMA-store epilogue: shrink the channel step of wide tiles
-  // (n_c = 80 with 64 channels per stage is a 92 KB stage: MDX23C's 640-channel scale)
-  auto fits = [&](int kk) {
-    const size_t stage = ((size_t)2 * kk * 256 + (size_t)2 * (kk / 16) * (3 * nc) * 32 + 1023) / 1024 * 1024;
-    const size_t staging = (size_t)2 * nc * kConvStride * 2;  // hi + lo output planes
-    return 2 * stage + staging + 16 * 1024 <= 227 * 1024;
-  };
-  while (!fits(k) && k > 16) {
-    int kk = k - 16;
-    while (kk > 16 && Cin % kk != 0) kk -= 16;
-    if (Cin % kk != 0) break;
-    k = kk;
-  }
-  *kc = k;
-  *n_c = nc;
-  return 0;
+bool umma_updown_supported(int Cin, int Cout, int F_in, int up) {
+  return Cin % 16 == 0 && F_in % 8 == 0 && umma_n_c(up ? UMMA_UP : UMMA_DOWN, Cout) > 0 && (up || F_in % 2 == 0);
 }
+bool umma_pw_supported(int Cin, int Cout, int F) { return Cin % 16 == 0 && Cout % 16 == 0 && F % 8 == 0; }
 
-int umma_conv_plan_create(UmmaConvPlan* pl, const void* x_hi, const void* x_lo, int Bmax, int Cin, int T, int F, int kc) {
+int umma_conv_plan_create(UmmaConvPlan* pl, UmmaConvKind kind, const void* x_hi, const void* x_lo, int Bmax, int Cin, int Cout, int T, int F) {
+  const int kc = umma_kc(kind, Cin, Cout);
   pl->Cin = Cin; pl->T = T; pl->F = F; pl->kc = kc;
   const uint64_t d[3] = {(uint64_t)F, (uint64_t)T, (uint64_t)Bmax * Cin};
   const uint64_t s[2] = {(uint64_t)F * 2, (uint64_t)T * F * 2};
@@ -699,12 +771,18 @@ int umma_conv_plan_create(UmmaConvPlan* pl, const void* x_hi, const void* x_lo, 
   return rc;
 }
 
-int umma_conv_run(const UmmaConvPlan& pl, const void* wb_hi, const void* wb_lo, int B, int Cout, int n_c, int ksize, const float* scale,
-                  const float* shift, int relu, void* out_hi, void* out_lo, cudaStream_t st) {
-  B2_CHECK_ARG(ksize == 3, "umma_conv: only 3x3 kernels");
-  UmmaEpilogue e;
-  e.scale = scale; e.shift = shift; e.act = relu ? 1 : 0; e.out_hi = out_hi; e.out_lo = out_lo;
-  return umma_conv_run_ex(pl, wb_hi, wb_lo, B, Cout, n_c, e, st);
+// the implicit-GEMM fields of every convolution mode: cols accumulator columns per output channel, n_r input rows per output row
+static UmmaParams conv_params(int mode, const UmmaConvPlan& pl, const void* wb_hi, const void* wb_lo, int Cout, int n_c, int cols, int n_r,
+                              const UmmaEpilogue& e) {
+  UmmaParams p{};
+  p.mode = mode; p.f_stride = kTileM; p.t_mul = 1; p.t_off = 0;
+  p.n_c = n_c; p.n_tile = cols * n_c; p.n_total = Cout;
+  p.kc = pl.kc; p.n_chunks = pl.Cin / pl.kc; p.num_iters = n_r * p.n_chunks; p.ksteps = pl.kc / 16;
+  p.a_bytes = (uint32_t)pl.kc * 256; p.b_bytes = (uint32_t)p.ksteps * p.n_tile * 32;
+  p.T = pl.T; p.F = pl.F; p.Cin = pl.Cin; p.Cout = Cout; p.n_tiles = Cout / n_c;
+  p.wb_hi = (const bf16*)wb_hi; p.wb_lo = (const bf16*)wb_lo;
+  fill_epilogue(p, e, Cout);
+  return p;
 }
 
 // TMA store maps of a conv3x3 output: the (F, T, B * C_total) bf16 planes with a [112 px][1 row][NC channels] box, no swizzle.  Encoding a map costs a few
@@ -740,27 +818,18 @@ static int launch_conv3(const CUtensorMap& a_hi, const CUtensorMap& a_lo, const 
     B2_CUDA(cudaFuncSetAttribute(umma_conv3_kernel<NC>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     attr_set = true;
   }
-  p.sleep_ns = umma_wait_sleep_ns();
   return launch_persistent(umma_conv3_kernel<NC>, p.num_tiles, smem, st, a_hi, a_lo, o_hi, o_lo, p);
 }
 
-int umma_conv_run_ex(const UmmaConvPlan& pl, const void* wb_hi, const void* wb_lo, int B, int Cout, int n_c, const UmmaEpilogue& e, cudaStream_t st) {
-  UmmaParams p{};
-  p.mode = 1; p.f_stride = kConvStride; p.f_off = -8; p.t_mul = 1; p.t_off = -1;
-  p.n_c = n_c; p.n_tile = 3 * n_c; p.n_total = Cout;
-  p.kc = pl.kc; p.n_chunks = pl.Cin / pl.kc;
-  p.num_iters = 3 * p.n_chunks; p.ksteps = pl.kc / 16;
-  p.a_bytes = (uint32_t)pl.kc * 256; p.b_bytes = (uint32_t)p.ksteps * p.n_tile * 32;
-  p.T = pl.T; p.F = pl.F; p.Cin = pl.Cin; p.Cout = Cout; p.n_tiles = Cout / n_c;
-  p.wb_hi = (const bf16*)wb_hi; p.wb_lo = (const bf16*)wb_lo;
-  fill_epilogue(p, e, Cout);
+int umma_conv_run(const UmmaConvPlan& pl, const void* wb_hi, const void* wb_lo, int B, int Cout, int n_c, const UmmaEpilogue& e, cudaStream_t st) {
+  UmmaParams p = conv_params(1, pl, wb_hi, wb_lo, Cout, n_c, 3, 3, e);
+  p.f_stride = kConvStride; p.f_off = -8; p.t_off = -1;
   B2_CHECK_ARG(Cout <= kMaxChannels, "umma_conv: more than %d output channels", kMaxChannels);
   B2_CHECK_ARG(e.out_f32 == nullptr, "umma_conv: 3x3 convolutions write pair tensors only");
   // one weight tile whose whole B operand fits next to the ring (Cin = Cout = 48: 83 KB): keep it resident; the shared-memory data pipe is the kernel's
-  // limiter (TC operand fetch + TMA fill + epilogue stores, profiles/README.md round 2) and the per-tile weight refill was 30 % of the TMA fill
+  // limiter (TC operand fetch + TMA fill + epilogue stores) and the per-tile weight refill was 30 % of the TMA fill
   const size_t b_all = (size_t)2 * p.b_bytes * p.num_iters;
-  static const bool allow_res = !(getenv("B200SEP_WRES") && atoi(getenv("B200SEP_WRES")) == 0);
-  p.b_resident = (allow_res && p.n_tiles == 1 && b_all <= 96 * 1024) ? 1 : 0;
+  p.b_resident = (p.n_tiles == 1 && b_all <= 96 * 1024) ? 1 : 0;
   p.stage_bytes = ((2 * p.a_bytes + (p.b_resident ? 0 : 2 * p.b_bytes) + 1023) / 1024) * 1024;
   p.n_ftiles = cdiv(pl.F, kConvStride);
   p.t_tiles = pl.T;
@@ -791,173 +860,26 @@ int umma_conv_run_ex(const UmmaConvPlan& pl, const void* wb_hi, const void* wb_l
   return B200SEP_ERR_ARG;
 }
 
-static int pick_nc(int Cout, int mult, int limit) {  // largest n_c | Cout with mult*n_c <= limit and mult*n_c % 16 == 0
-  for (int nc = Cout; nc >= 4; --nc)
-    if (Cout % nc == 0 && mult * nc <= limit && (mult * nc) % 16 == 0 && nc % 16 == 0) return nc;
-  return 0;
-}
-bool umma_updown_supported(int Cin, int Cout, int F_in, int up) {
-  return Cin % 16 == 0 && F_in % 8 == 0 && pick_nc(Cout, up ? 4 : 2, kMaxNTile) > 0 && (up || F_in % 2 == 0);
-}
-int umma_updown_choose(int Cin, int Cout, int up, int* kc, int* n_c) {
-  int k = 64;
-  while (k > 16 && Cin % k != 0) k -= 16;
-  if (Cin % 48 == 0) k = 48;
-  *kc = k;
-  *n_c = pick_nc(Cout, up ? 4 : 2, kMaxNTile);
-  return 0;
-}
-
 // x: pair (B, Cin, T, F) -> ConvTranspose2d(k2,s2)+BN+ReLU (* skip) -> pair (B, Cout, 2T, 2F)
-int umma_up_run(const UmmaConvPlan& pl, const void* wb_hi, const void* wb_lo, int B, int Cout, int n_c, const float* scale, const float* shift, int relu,
-                const void* skip_hi, const void* skip_lo, void* out_hi, void* out_lo, cudaStream_t st) {
-  UmmaEpilogue e;
-  e.scale = scale; e.shift = shift; e.act = relu ? 1 : 0; e.out_hi = out_hi; e.out_lo = out_lo; e.res_hi = skip_hi; e.res_lo = skip_lo;
-  return umma_up_run_ex(pl, wb_hi, wb_lo, B, Cout, n_c, e, st);
-}
-
-int umma_up_run_ex(const UmmaConvPlan& pl, const void* wb_hi, const void* wb_lo, int B, int Cout, int n_c, const UmmaEpilogue& e, cudaStream_t st) {
-  UmmaParams p{};
-  p.mode = 2; p.f_stride = kTileM; p.t_mul = 1; p.t_off = 0;
-  p.n_c = n_c; p.n_tile = 4 * n_c; p.n_total = Cout;
-  p.kc = pl.kc; p.n_chunks = pl.Cin / pl.kc; p.num_iters = p.n_chunks; p.ksteps = pl.kc / 16;
-  p.a_bytes = (uint32_t)pl.kc * 256; p.b_bytes = (uint32_t)p.ksteps * p.n_tile * 32;
-  p.T = pl.T; p.F = pl.F; p.Cin = pl.Cin; p.Cout = Cout; p.n_tiles = Cout / n_c;
-  p.wb_hi = (const bf16*)wb_hi; p.wb_lo = (const bf16*)wb_lo;
-  fill_epilogue(p, e, Cout);
+int umma_up_run(const UmmaConvPlan& pl, const void* wb_hi, const void* wb_lo, int B, int Cout, int n_c, const UmmaEpilogue& e, cudaStream_t st) {
+  UmmaParams p = conv_params(2, pl, wb_hi, wb_lo, Cout, n_c, 4, 1, e);
   dim3 grid(cdiv(pl.F, kTileM), pl.T, B * p.n_tiles);
   return launch(pl.a_hi, pl.a_lo, pl.a_hi, pl.a_lo, p, grid, st);
 }
 
 // x: pair (B, Cin, T, F) -> Conv2d(k2,s2)+BN+ReLU -> pair (B, Cout, T/2, F/2)
-int umma_down_run(const UmmaConvPlan& pl, const void* wb_hi, const void* wb_lo, int B, int Cout, int n_c, const float* scale, const float* shift, int relu,
-                  void* out_hi, void* out_lo, cudaStream_t st) {
-  UmmaEpilogue e;
-  e.scale = scale; e.shift = shift; e.act = relu ? 1 : 0; e.out_hi = out_hi; e.out_lo = out_lo;
-  return umma_down_run_ex(pl, wb_hi, wb_lo, B, Cout, n_c, e, st);
-}
-
-int umma_down_run_ex(const UmmaConvPlan& pl, const void* wb_hi, const void* wb_lo, int B, int Cout, int n_c, const UmmaEpilogue& e, cudaStream_t st) {
-  UmmaParams p{};
-  p.mode = 3; p.f_stride = kTileM; p.t_mul = 2; p.t_off = 0;
-  p.n_c = n_c; p.n_tile = 2 * n_c; p.n_total = Cout;
-  p.kc = pl.kc; p.n_chunks = pl.Cin / pl.kc; p.num_iters = 2 * p.n_chunks; p.ksteps = pl.kc / 16;
-  p.a_bytes = (uint32_t)pl.kc * 256; p.b_bytes = (uint32_t)p.ksteps * p.n_tile * 32;
-  p.T = pl.T; p.F = pl.F; p.Cin = pl.Cin; p.Cout = Cout; p.n_tiles = Cout / n_c;
-  p.wb_hi = (const bf16*)wb_hi; p.wb_lo = (const bf16*)wb_lo;
-  fill_epilogue(p, e, Cout);
+int umma_down_run(const UmmaConvPlan& pl, const void* wb_hi, const void* wb_lo, int B, int Cout, int n_c, const UmmaEpilogue& e, cudaStream_t st) {
+  UmmaParams p = conv_params(3, pl, wb_hi, wb_lo, Cout, n_c, 2, 2, e);
+  p.t_mul = 2;
   dim3 grid(cdiv(pl.F, kTileM), pl.T / 2, B * p.n_tiles);
   return launch(pl.a_hi, pl.a_lo, pl.a_hi, pl.a_lo, p, grid, st);
 }
 
-// Generic blocking: value(row, r, ci) for B rows [rows], row taps [n_r], -> [Cout/n_c][r][Cin/kc][kc/16][rows x 16 core-matrix tiled]
-template <class F>
-static void block_weights(int n_tiles, int n_r, int Cin, int kc, int rows, F value, std::vector<uint16_t>& hi, std::vector<uint16_t>& lo) {
-  auto f2bf = [](float f) {
-    uint32_t u;
-    memcpy(&u, &f, 4);
-    u += 0x7fffu + ((u >> 16) & 1u);
-    return (uint16_t)(u >> 16);
-  };
-  auto bf2f = [](uint16_t h) {
-    uint32_t u = (uint32_t)h << 16;
-    float f;
-    memcpy(&f, &u, 4);
-    return f;
-  };
-  const int n_chunks = Cin / kc, ksteps = kc / 16;
-  hi.assign((size_t)n_tiles * n_r * Cin * rows, 0);
-  lo.assign(hi.size(), 0);
-  size_t pos = 0;
-  for (int nt = 0; nt < n_tiles; ++nt)
-    for (int r = 0; r < n_r; ++r)
-      for (int ch = 0; ch < n_chunks; ++ch)
-        for (int j = 0; j < ksteps; ++j) {
-          for (int row = 0; row < rows; ++row)
-            for (int kk = 0; kk < 16; ++kk) {
-              const float v = value(nt, row, r, ch * kc + j * 16 + kk);
-              const size_t o = pos + (size_t)((row / 8) * 2 + kk / 8) * 64 + (row % 8) * 8 + (kk % 8);
-              hi[o] = f2bf(v);
-              lo[o] = f2bf(v - bf2f(hi[o]));
-            }
-          pos += (size_t)rows * 16;
-        }
-}
-// ConvTranspose2d weight (Cin, Cout, 2, 2): B rows = (co_local, q = dy*2+dx)
-void umma_up_block_weights(const float* w, int Cin, int Cout, int kc, int n_c, std::vector<uint16_t>& hi, std::vector<uint16_t>& lo) {
-  block_weights(Cout / n_c, 1, Cin, kc, 4 * n_c, [&](int nt, int row, int, int ci) {
-    const int q = row & 3, co = nt * n_c + (row >> 2);
-    return w[((size_t)ci * Cout + co) * 4 + q];
-  }, hi, lo);
-}
-// Conv2d weight (Cout, Cin, 2, 2) stride 2: row taps r = dy, B rows = (co_local, dx)
-void umma_down_block_weights(const float* w, int Cout, int Cin, int kc, int n_c, std::vector<uint16_t>& hi, std::vector<uint16_t>& lo) {
-  block_weights(Cout / n_c, 2, Cin, kc, 2 * n_c, [&](int nt, int row, int dy, int ci) {
-    const int dx = row & 1, co = nt * n_c + (row >> 1);
-    return w[(((size_t)co * Cin + ci) * 2 + dy) * 2 + dx];
-  }, hi, lo);
-}
-
-// Conv2d weight (Cout, Cin, 1, 1): one tap, B rows = co_local
-void umma_pw_block_weights(const float* w, int Cout, int Cin, int kc, int n_c, std::vector<uint16_t>& hi, std::vector<uint16_t>& lo) {
-  block_weights(Cout / n_c, 1, Cin, kc, n_c, [&](int nt, int row, int, int ci) { return w[(size_t)(nt * n_c + row) * Cin + ci]; }, hi, lo);
-}
-bool umma_pw_supported(int Cin, int Cout, int F) { return Cin % 16 == 0 && Cout % 16 == 0 && F % 8 == 0; }
-int umma_pw_choose(int Cin, int Cout, int* kc, int* n_c) {
-  int k = 64;
-  while (k > 16 && Cin % k != 0) k -= 16;
-  if (Cin % 48 == 0) k = 48;
-  *kc = k;
-  *n_c = pick_nc(Cout, 1, kMaxNTile);
-  return 0;
-}
 // x: pair (B, Cin, T, F) -> Conv2d 1x1 (+affine, act, +res, *mul) -> pair or fp32 (B, Cout, T, F)
-int umma_pw_run_ex(const UmmaConvPlan& pl, const void* wb_hi, const void* wb_lo, int B, int Cout, int n_c, const UmmaEpilogue& e, cudaStream_t st) {
-  UmmaParams p{};
-  p.mode = 4; p.f_stride = kTileM; p.t_mul = 1; p.t_off = 0;
-  p.n_c = n_c; p.n_tile = n_c; p.n_total = Cout;
-  p.kc = pl.kc; p.n_chunks = pl.Cin / pl.kc; p.num_iters = p.n_chunks; p.ksteps = pl.kc / 16;
-  p.a_bytes = (uint32_t)pl.kc * 256; p.b_bytes = (uint32_t)p.ksteps * p.n_tile * 32;
-  p.T = pl.T; p.F = pl.F; p.Cin = pl.Cin; p.Cout = Cout; p.n_tiles = Cout / n_c;
-  p.wb_hi = (const bf16*)wb_hi; p.wb_lo = (const bf16*)wb_lo;
-  fill_epilogue(p, e, Cout);
+int umma_pw_run(const UmmaConvPlan& pl, const void* wb_hi, const void* wb_lo, int B, int Cout, int n_c, const UmmaEpilogue& e, cudaStream_t st) {
+  UmmaParams p = conv_params(4, pl, wb_hi, wb_lo, Cout, n_c, 1, 1, e);
   dim3 grid(cdiv(pl.F, kTileM), pl.T, B * p.n_tiles);
   return launch(pl.a_hi, pl.a_lo, pl.a_hi, pl.a_lo, p, grid, st);
-}
-
-// Host-side blocking of a (Cout, Cin, 3, 3) fp32 filter into the B operand stream of umma_conv_run:
-// [Cout/n_c][dy][Cin/kc][kc/16] blocks of [3*n_c rows = (dx, co)][16 k] stored as 8x8 core matrices (K-major, no swizzle).
-void umma_conv_block_weights(const float* w, int Cout, int Cin, int kc, int n_c, std::vector<uint16_t>& hi, std::vector<uint16_t>& lo) {
-  auto f2bf = [](float f) {
-    uint32_t u;
-    memcpy(&u, &f, 4);
-    u += 0x7fffu + ((u >> 16) & 1u);
-    return (uint16_t)(u >> 16);
-  };
-  auto bf2f = [](uint16_t h) {
-    uint32_t u = (uint32_t)h << 16;
-    float f;
-    memcpy(&f, &u, 4);
-    return f;
-  };
-  const int n_tiles = Cout / n_c, n_chunks = Cin / kc, ksteps = kc / 16, rows = 3 * n_c;
-  hi.assign((size_t)Cout * Cin * 9, 0);
-  lo.assign(hi.size(), 0);
-  size_t pos = 0;
-  for (int nt = 0; nt < n_tiles; ++nt)
-    for (int dy = 0; dy < 3; ++dy)
-      for (int ch = 0; ch < n_chunks; ++ch)
-        for (int j = 0; j < ksteps; ++j) {
-          for (int r = 0; r < rows; ++r)
-            for (int kk = 0; kk < 16; ++kk) {
-              const int dx = r / n_c, co = nt * n_c + r % n_c, ci = ch * kc + j * 16 + kk;
-              const float v = w[(((size_t)co * Cin + ci) * 3 + dy) * 3 + dx];
-              const size_t o = pos + (size_t)((r / 8) * 2 + kk / 8) * 64 + (r % 8) * 8 + (kk % 8);
-              hi[o] = f2bf(v);
-              lo[o] = f2bf(v - bf2f(hi[o]));
-            }
-          pos += (size_t)rows * 16;
-        }
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -1005,7 +927,9 @@ extern "C" int b200sep_selftest_umma_gemm(const float* a, const float* w, const 
   if (!rc && res) rc = split_pair(res, r_p, r_p + no, no, st);
   UmmaGemmPlan pl;
   if (!rc) rc = umma_gemm_plan_create(&pl, a_p, a_p + na, w_p, w_p + nw, M, N, K);
-  if (!rc) rc = umma_gemm_run(pl, scale, shift, rows_per_channel, channels, relu, o_p, o_p + no, r_p, r_p ? r_p + no : nullptr, M, st);
+  UmmaEpilogue e;
+  e.scale = scale; e.shift = shift; e.act = relu ? 1 : 0; e.out_hi = o_p; e.out_lo = o_p + no; e.res_hi = r_p; e.res_lo = r_p ? r_p + no : nullptr;
+  if (!rc) rc = umma_gemm_run(pl, rows_per_channel, channels, M, e, st);
   if (!rc) rc = join_pair(o_p, o_p + no, out, no, st);
   cudaStreamSynchronize(st);
   cudaFree(a_p); cudaFree(w_p); cudaFree(o_p);
@@ -1018,10 +942,8 @@ extern "C" int b200sep_selftest_umma_conv3x3(const float* x, const float* w_host
   B2_CHECK_ARG(x && w_host && out && scale && shift, "selftest_umma_conv3x3: NULL argument");
   B2_CHECK_ARG(umma_conv_supported(Cin, Cout, F, 3, 3), "selftest_umma_conv3x3: Cin=%d Cout=%d F=%d not supported by the tensor-core path", Cin, Cout, F);
   cudaStream_t st = (cudaStream_t)stream;
-  int kc, n_c;
-  umma_conv_choose(Cin, Cout, &kc, &n_c);
   std::vector<uint16_t> hi, lo;
-  umma_conv_block_weights(w_host, Cout, Cin, kc, n_c, hi, lo);
+  const int n_c = umma_block_weights(UMMA_CONV3, w_host, Cin, Cout, hi, lo);
   uint16_t *x_p = nullptr, *o_p = nullptr, *w_p = nullptr;
   const int64_t nx = (int64_t)B * Cin * T * F, no = (int64_t)B * Cout * T * F, nw = (int64_t)hi.size();
   B2_CUDA(cudaMalloc(&x_p, nx * 4));
@@ -1031,8 +953,10 @@ extern "C" int b200sep_selftest_umma_conv3x3(const float* x, const float* w_host
   B2_CUDA(cudaMemcpy(w_p + nw, lo.data(), nw * 2, cudaMemcpyHostToDevice));
   int rc = split_pair(x, x_p, x_p + nx, nx, st);
   UmmaConvPlan pl;
-  if (!rc) rc = umma_conv_plan_create(&pl, x_p, x_p + nx, B, Cin, T, F, kc);
-  if (!rc) rc = umma_conv_run(pl, w_p, w_p + nw, B, Cout, n_c, 3, scale, shift, relu, o_p, o_p + no, st);
+  if (!rc) rc = umma_conv_plan_create(&pl, UMMA_CONV3, x_p, x_p + nx, B, Cin, Cout, T, F);
+  UmmaEpilogue e;
+  e.scale = scale; e.shift = shift; e.act = relu ? 1 : 0; e.out_hi = o_p; e.out_lo = o_p + no;
+  if (!rc) rc = umma_conv_run(pl, w_p, w_p + nw, B, Cout, n_c, e, st);
   if (!rc) rc = join_pair(o_p, o_p + no, out, no, st);
   cudaStreamSynchronize(st);
   cudaFree(x_p); cudaFree(o_p); cudaFree(w_p);
@@ -1044,11 +968,9 @@ extern "C" int b200sep_selftest_umma_updown(const float* x, const float* w_host,
   B2_CHECK_ARG(x && w_host && out && scale && shift, "selftest_umma_updown: NULL argument");
   B2_CHECK_ARG(umma_updown_supported(Cin, Cout, F, up), "selftest_umma_updown: Cin=%d Cout=%d F=%d not supported by the tensor-core path", Cin, Cout, F);
   cudaStream_t st = (cudaStream_t)stream;
-  int kc, n_c;
-  umma_updown_choose(Cin, Cout, up, &kc, &n_c);
+  const UmmaConvKind kind = up ? UMMA_UP : UMMA_DOWN;
   std::vector<uint16_t> hi, lo;
-  if (up) umma_up_block_weights(w_host, Cin, Cout, kc, n_c, hi, lo);
-  else umma_down_block_weights(w_host, Cout, Cin, kc, n_c, hi, lo);
+  const int n_c = umma_block_weights(kind, w_host, Cin, Cout, hi, lo);
   uint16_t *x_p = nullptr, *o_p = nullptr, *w_p = nullptr, *s_p = nullptr;
   const int64_t nx = (int64_t)B * Cin * T * F, no = up ? (int64_t)B * Cout * 4 * T * F : (int64_t)B * Cout * (T / 2) * (F / 2), nw = (int64_t)hi.size();
   B2_CUDA(cudaMalloc(&x_p, nx * 4));
@@ -1060,11 +982,11 @@ extern "C" int b200sep_selftest_umma_updown(const float* x, const float* w_host,
   int rc = split_pair(x, x_p, x_p + nx, nx, st);
   if (!rc && skip) rc = split_pair(skip, s_p, s_p + no, no, st);
   UmmaConvPlan pl;
-  if (!rc) rc = umma_conv_plan_create(&pl, x_p, x_p + nx, B, Cin, T, F, kc);
-  if (!rc) {
-    if (up) rc = umma_up_run(pl, w_p, w_p + nw, B, Cout, n_c, scale, shift, relu, s_p, s_p ? s_p + no : nullptr, o_p, o_p + no, st);
-    else rc = umma_down_run(pl, w_p, w_p + nw, B, Cout, n_c, scale, shift, relu, o_p, o_p + no, st);
-  }
+  if (!rc) rc = umma_conv_plan_create(&pl, kind, x_p, x_p + nx, B, Cin, Cout, T, F);
+  UmmaEpilogue e;
+  e.scale = scale; e.shift = shift; e.act = relu ? 1 : 0; e.out_hi = o_p; e.out_lo = o_p + no;
+  if (up) { e.res_hi = s_p; e.res_lo = s_p ? s_p + no : nullptr; }
+  if (!rc) rc = up ? umma_up_run(pl, w_p, w_p + nw, B, Cout, n_c, e, st) : umma_down_run(pl, w_p, w_p + nw, B, Cout, n_c, e, st);
   if (!rc) rc = join_pair(o_p, o_p + no, out, no, st);
   cudaStreamSynchronize(st);
   cudaFree(x_p); cudaFree(o_p); cudaFree(w_p);

@@ -38,39 +38,31 @@ struct UmmaEpilogue {
 bool umma_gemm_supported(int M, int N, int K);
 // A: pair [M][K] (K contiguous), W: pair [N][K].  Tensor maps are bound to these addresses.
 int umma_gemm_plan_create(UmmaGemmPlan* pl, const void* a_hi, const void* a_lo, const void* w_hi, const void* w_lo, int M, int N, int K);
+// hi / lo planes of a GEMM weight [N][K] (the W operand of umma_gemm_plan_create)
+void umma_gemm_split_weights(const float* w, int N, int K, std::vector<uint16_t>& hi, std::vector<uint16_t>& lo);
 // out[r][n] = act(acc*scale[c]+shift[c]) (+ res[r][n]),  c = (r / rows_per_channel) % channels;  rows >= M_active are not written
-int umma_gemm_run(const UmmaGemmPlan& pl, const float* scale, const float* shift, int rows_per_channel, int channels, int relu, void* out_hi,
-                  void* out_lo, const void* res_hi, const void* res_lo, int M_active, cudaStream_t st);
+int umma_gemm_run(const UmmaGemmPlan& pl, int rows_per_channel, int channels, int M_active, const UmmaEpilogue& e, cudaStream_t st);
 
-int umma_gemm_run_ex(const UmmaGemmPlan& pl, int rows_per_channel, int channels, int M_active, const UmmaEpilogue& e, cudaStream_t st);
-
+// Convolutions on the same pipeline: 3x3 stride 1; ConvTranspose2d / Conv2d with 2x2 kernels and stride 2 (the U-Nets' up / down sampling); 1x1.
+enum UmmaConvKind { UMMA_CONV3, UMMA_UP, UMMA_DOWN, UMMA_PW };
+// input checks: shapes that fail them run on the SIMT pair kernels (or are rejected by the caller)
 bool umma_conv_supported(int Cin, int Cout, int F, int kh, int kw);
-int umma_conv_choose(int Cin, int Cout, int* kc, int* n_c);
-void umma_conv_block_weights(const float* w, int Cout, int Cin, int kc, int n_c, std::vector<uint16_t>& hi, std::vector<uint16_t>& lo);
-// x: pair (Bmax, Cin, T, F)
-int umma_conv_plan_create(UmmaConvPlan* pl, const void* x_hi, const void* x_lo, int Bmax, int Cin, int T, int F, int kc);
-// weights pre-blocked by umma_conv_block_weights (hi plane, lo plane)
-int umma_conv_run(const UmmaConvPlan& pl, const void* wb_hi, const void* wb_lo, int B, int Cout, int n_c, int ksize, const float* scale,
-                  const float* shift, int relu, void* out_hi, void* out_lo, cudaStream_t st);
-
-// ConvTranspose2d / Conv2d with 2x2 kernels and stride 2 (the U-Net's up / down sampling) on the same pipeline
 bool umma_updown_supported(int Cin, int Cout, int F_in, int up);
-int umma_updown_choose(int Cin, int Cout, int up, int* kc, int* n_c);
-void umma_up_block_weights(const float* w /*(Cin,Cout,2,2)*/, int Cin, int Cout, int kc, int n_c, std::vector<uint16_t>& hi, std::vector<uint16_t>& lo);
-void umma_down_block_weights(const float* w /*(Cout,Cin,2,2)*/, int Cout, int Cin, int kc, int n_c, std::vector<uint16_t>& hi, std::vector<uint16_t>& lo);
-int umma_up_run(const UmmaConvPlan& pl, const void* wb_hi, const void* wb_lo, int B, int Cout, int n_c, const float* scale, const float* shift, int relu,
-                const void* skip_hi, const void* skip_lo, void* out_hi, void* out_lo, cudaStream_t st);
-int umma_down_run(const UmmaConvPlan& pl, const void* wb_hi, const void* wb_lo, int B, int Cout, int n_c, const float* scale, const float* shift, int relu,
-                  void* out_hi, void* out_lo, cudaStream_t st);
-
-int umma_conv_run_ex(const UmmaConvPlan& pl, const void* wb_hi, const void* wb_lo, int B, int Cout, int n_c, const UmmaEpilogue& e, cudaStream_t st);
-int umma_up_run_ex(const UmmaConvPlan& pl, const void* wb_hi, const void* wb_lo, int B, int Cout, int n_c, const UmmaEpilogue& e, cudaStream_t st);
-int umma_down_run_ex(const UmmaConvPlan& pl, const void* wb_hi, const void* wb_lo, int B, int Cout, int n_c, const UmmaEpilogue& e, cudaStream_t st);
-// 1x1 convolution on the same pipeline
 bool umma_pw_supported(int Cin, int Cout, int F);
-int umma_pw_choose(int Cin, int Cout, int* kc, int* n_c);
-void umma_pw_block_weights(const float* w /*(Cout,Cin)*/, int Cout, int Cin, int kc, int n_c, std::vector<uint16_t>& hi, std::vector<uint16_t>& lo);
-int umma_pw_run_ex(const UmmaConvPlan& pl, const void* wb_hi, const void* wb_lo, int B, int Cout, int n_c, const UmmaEpilogue& e, cudaStream_t st);
+// output channels per CTA: a property of the blocked weights
+int umma_n_c(UmmaConvKind kind, int Cout);
+// input channels per pipeline stage: a property of the plan
+int umma_kc(UmmaConvKind kind, int Cin, int Cout);
+// Blocks fp32 weights -- (Cout, Cin, kh, kw); UP: ConvTranspose2d (Cin, Cout, 2, 2) -- into the hi / lo weight planes of the run functions.
+// Returns n_c = umma_n_c(kind, Cout).
+int umma_block_weights(UmmaConvKind kind, const float* w, int Cin, int Cout, std::vector<uint16_t>& hi, std::vector<uint16_t>& lo);
+// x: pair (Bmax, Cin, T, F); the plan's kc is umma_kc(kind, Cin, Cout)
+int umma_conv_plan_create(UmmaConvPlan* pl, UmmaConvKind kind, const void* x_hi, const void* x_lo, int Bmax, int Cin, int Cout, int T, int F);
+// x: the plan's input, B <= Bmax; wb_hi / wb_lo: the planes of umma_block_weights
+int umma_conv_run(const UmmaConvPlan& pl, const void* wb_hi, const void* wb_lo, int B, int Cout, int n_c, const UmmaEpilogue& e, cudaStream_t st);
+int umma_up_run(const UmmaConvPlan& pl, const void* wb_hi, const void* wb_lo, int B, int Cout, int n_c, const UmmaEpilogue& e, cudaStream_t st);
+int umma_down_run(const UmmaConvPlan& pl, const void* wb_hi, const void* wb_lo, int B, int Cout, int n_c, const UmmaEpilogue& e, cudaStream_t st);
+int umma_pw_run(const UmmaConvPlan& pl, const void* wb_hi, const void* wb_lo, int B, int Cout, int n_c, const UmmaEpilogue& e, cudaStream_t st);
 
 int split_pair(const float* x, void* hi, void* lo, int64_t n, cudaStream_t st);
 int join_pair(const void* hi, const void* lo, float* y, int64_t n, cudaStream_t st);
