@@ -373,6 +373,11 @@ int b200sep_mask_average_f32(const float* mask_gathered, const int* csr_offsets,
  * max(sum_i window[q - starts[i]], 1e-10); chunks (n_chunks, channels, len), starts device int64[n_chunks] */
 int b200sep_overlap_add_starts(const float* chunks, const int64_t* starts, const float* window, int n_chunks, int channels, int len, int64_t n_out, float* out,
                                void* stream);
+/* Time-sharded form: `chunks` (n_local, channels, len) holds only a rank's chunks (halo followed by its own, in global order) and `starts` their
+ * n_local start positions; the samples [q_begin, q_end) of the (channels, n_out) output are written to out[c * out_ld + q - out_base].  Every chunk
+ * that overlaps [q_begin, q_end) must be among the n_local (the starts are on the device, so this is not checked here). */
+int b200sep_overlap_add_starts_range(const float* chunks, const int64_t* starts, int n_local, const float* window, int channels, int len, int64_t n_out,
+                                     int64_t q_begin, int64_t q_end, float* out, int64_t out_ld, int64_t out_base, void* stream);
 
 /* nn.LSTM(bidirectional=True), one layer (LSTMModule of VR 5.1, layers_new.py:124-149): the recurrence only.  x_proj (2, T, N, 4*hid) = the input
  * projections x_t @ W_ih^T + b_ih + b_hh of the forward / reverse direction (gate order i, f, g, o; computed with gemm_f32), w_hh (2, 4*hid, hid);

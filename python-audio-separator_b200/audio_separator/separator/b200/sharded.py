@@ -3,12 +3,15 @@ with overlap-region halo exchange via NCCL").
 
 The reference has no multi-GPU path (SURVEY.md section 2.1); this is new.  All three chunked architectures have the same
 structure (SURVEY.md section 8e): independent units (MDX chunks, mdx_separator.py:335-348; MDX23C chunks, mdxc_separator.py:361-402;
-Demucs segments, demucs/apply.py:215-250) placed every `stride` samples, coupled only by the overlap-add.  Two planners:
+Demucs segments, demucs/apply.py:215-250) placed every `stride` samples, coupled only by the overlap-add.  The Roformer chunks
+(mdxc_separator.py:320-341) are placed every `step` samples until one would run past the end, and every later start is clamped to N - chunk.
+Two planning rules:
 
 * `plan_shards`        -- MDX: contiguous chunk ranges, rank r finalises the padded positions [c0*step, c1*step).
-* `plan_range_shards`  -- MDX23C / Demucs: rank r finalises a fixed range [q0, q1) of OUTPUT samples (the same for every pass of a
-                          Demucs bag / shift loop, so the accumulation order per sample is the single-GPU order and the result is
-                          bit-identical); a unit belongs to the rank its first output sample falls in.
+* `plan_start_shards`  -- Roformer (explicit start list), and through `plan_range_shards` MDX23C / Demucs (regular grid): rank r finalises
+                          a fixed range [q0, q1) of OUTPUT samples (the same for every pass of a Demucs bag / shift loop, so the
+                          accumulation order per sample is the single-GPU order and the result is bit-identical); a unit belongs to
+                          the rank its first output sample falls in.
 In both, a rank needs the trailing units of its LEFT neighbour that reach into its range: one `isend`/`irecv` pair between
 time-neighbours (NCCL p2p over NVLink), posted as soon as those units are computed so the transfer overlaps the remaining forwards.
 The finalised slices go to rank 0 with point-to-point receives straight into the full-size stem buffers, or -- end-to-end entry points --
@@ -20,6 +23,7 @@ need CUDA + NCCL.
 """
 from __future__ import annotations
 
+from bisect import bisect_left, bisect_right
 from dataclasses import dataclass
 
 import torch
@@ -62,16 +66,19 @@ def plan_shards(n_samples: int, total_len: int, step: int, chunk: int, trim: int
     return shards
 
 
-def plan_range_shards(n_out: int, world: int, n_units: int, stride: int, unit_len: int, base: int) -> list[Shard]:
-    """MDX23C / Demucs.  Unit i covers the output samples [i*stride - base, i*stride - base + unit_len).  Rank r finalises the output samples
-    [n_out*r/world, n_out*(r+1)/world) and owns the units whose first output sample (clamped into [0, n_out)) lies in that range."""
-    if n_units < 1 or stride < 1 or unit_len < 1:
-        raise ValueError("plan_range_shards: bad grid")
+def plan_start_shards(starts, unit_len: int, n_out: int, world: int) -> list[Shard]:
+    """Units at explicit, nondecreasing output positions: unit i covers the output samples [starts[i], starts[i] + unit_len).  Rank r finalises
+    the output samples [n_out*r/world, n_out*(r+1)/world) and owns the units whose start lies in that range (starts before 0 go to rank 0, starts
+    at or past n_out to the last rank), so repeated starts -- the Roformer grid clamps every tail chunk to n_out - unit_len -- land on one rank.
+    Its halo is the run of its left neighbour's units that reach into the range."""
+    n_units = len(starts)
+    if n_units < 1 or unit_len < 1 or any(b < a for a, b in zip(starts, starts[1:])):
+        raise ValueError("plan_start_shards: bad grid (no units, or starts not nondecreasing)")
     qs = [n_out * r // world for r in range(world + 1)]
-    u0 = [0] + [min(n_units, max(0, -(-(qs[r] + base) // stride))) for r in range(1, world)] + [n_units]
+    u0 = [0] + [bisect_left(starts, qs[r]) for r in range(1, world)] + [n_units]
     shards = []
     for r in range(world):
-        need_lo = 0 if r == 0 else max(0, (qs[r] + base - unit_len) // stride + 1)
+        need_lo = 0 if r == 0 else bisect_right(starts, qs[r] - unit_len)  # first unit that ends past q0
         c0, c1 = u0[r], u0[r + 1]
         halo = max(0, c0 - need_lo) if qs[r + 1] > qs[r] else 0
         if r > 0 and halo > 0 and c0 - halo < u0[r - 1]:
@@ -80,6 +87,13 @@ def plan_range_shards(n_out: int, world: int, n_units: int, stride: int, unit_le
     for s in shards[1:]:
         shards[s.rank - 1].send = s.halo
     return shards
+
+
+def plan_range_shards(n_out: int, world: int, n_units: int, stride: int, unit_len: int, base: int) -> list[Shard]:
+    """MDX23C / Demucs: `plan_start_shards` on the regular grid, unit i covering the output samples [i*stride - base, i*stride - base + unit_len)."""
+    if n_units < 1 or stride < 1 or unit_len < 1:
+        raise ValueError("plan_range_shards: bad grid")
+    return plan_start_shards(range(-base, n_units * stride - base, stride), unit_len, n_out, world)
 
 
 def balanced_batches(n: int, max_batch: int) -> list[int]:

@@ -91,11 +91,13 @@ __global__ void mask_apply_kernel(const float* __restrict__ st, const float* __r
 }
 
 // Roformer branch of MDXCSeparator.demix (mdxc_separator.py:310-343): result += x * window; counter += window; result / clamp(counter, 1e-10)
-// as a gather over the chunks covering each output sample.  chunks (n_chunks, channels, len); chunk i is placed at starts[i].
+// as a gather over the chunks covering each output sample.  chunks (n_chunks, channels, len); chunk i is placed at starts[i].  Only the output
+// samples [q_begin, q_end) are written, to out[c * out_ld + q - out_base]: a time-sharded rank passes just the chunks it holds (halo + own, in
+// global order), so every sample sums the same contributions in the same order as the full grid.
 __global__ void ola_starts_kernel(const float* __restrict__ chunks, const int64_t* __restrict__ starts, const float* __restrict__ window, int n_chunks, int channels,
-                                  int len, int64_t n_out, float* __restrict__ out) {
+                                  int len, int64_t q_begin, int64_t q_end, float* __restrict__ out, int64_t out_ld, int64_t out_base) {
   const int c = blockIdx.y;
-  for (int64_t q = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; q < n_out; q += (int64_t)gridDim.x * blockDim.x) {
+  for (int64_t q = q_begin + (int64_t)blockIdx.x * blockDim.x + threadIdx.x; q < q_end; q += (int64_t)gridDim.x * blockDim.x) {
     float acc = 0.f, cnt = 0.f;
     for (int i = 0; i < n_chunks; ++i) {
       const int64_t r = q - __ldg(&starts[i]);
@@ -105,7 +107,7 @@ __global__ void ola_starts_kernel(const float* __restrict__ chunks, const int64_
         cnt += w;
       }
     }
-    out[(int64_t)c * n_out + q] = acc / fmaxf(cnt, 1e-10f);
+    out[(int64_t)c * out_ld + (q - out_base)] = acc / fmaxf(cnt, 1e-10f);
   }
 }
 
@@ -205,13 +207,25 @@ extern "C" int b200sep_roformer_mask_apply(const float* stft_tf, const float* ma
   return B200SEP_OK;
 }
 
-extern "C" int b200sep_overlap_add_starts(const float* chunks, const int64_t* starts, const float* window, int n_chunks, int channels, int len, int64_t n_out, float* out,
-                                          void* stream) {
-  B2_CHECK_ARG(chunks && starts && window && out && n_chunks >= 1 && channels >= 1 && len >= 1 && n_out >= 1, "overlap_add_starts: bad argument");
-  dim3 grid((unsigned)std::min<int64_t>(cdiv(n_out, 256), kNumSMs * 8), channels);
-  ola_starts_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(chunks, starts, window, n_chunks, channels, len, n_out, out);
+// The starts live on the device, so the host cannot check that every chunk overlapping [q_begin, q_end) is among the n_local given: that is the
+// caller's precondition (RoformerEngine checks it on its host copy of the start list).
+extern "C" int b200sep_overlap_add_starts_range(const float* chunks, const int64_t* starts, int n_local, const float* window, int channels, int len, int64_t n_out,
+                                                int64_t q_begin, int64_t q_end, float* out, int64_t out_ld, int64_t out_base, void* stream) {
+  B2_CHECK_ARG(chunks && starts && window && out && n_local >= 1 && channels >= 1 && len >= 1 && n_out >= 1, "overlap_add_starts: bad argument");
+  B2_CHECK_ARG(0 <= q_begin && q_begin <= q_end && q_end <= n_out, "overlap_add_starts: bad output range [%lld, %lld) of %lld", (long long)q_begin, (long long)q_end,
+               (long long)n_out);
+  B2_CHECK_ARG(out_base >= 0 && out_base <= q_begin && q_end - out_base <= out_ld, "overlap_add_starts: output slice does not cover [%lld, %lld)", (long long)q_begin,
+               (long long)q_end);
+  if (q_end == q_begin) return B200SEP_OK;
+  dim3 grid((unsigned)std::min<int64_t>(cdiv(q_end - q_begin, 256), kNumSMs * 8), channels);
+  ola_starts_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(chunks, starts, window, n_local, channels, len, q_begin, q_end, out, out_ld, out_base);
   B2_LAUNCHED();
   return B200SEP_OK;
+}
+
+extern "C" int b200sep_overlap_add_starts(const float* chunks, const int64_t* starts, const float* window, int n_chunks, int channels, int len, int64_t n_out, float* out,
+                                          void* stream) {
+  return b200sep_overlap_add_starts_range(chunks, starts, n_chunks, window, channels, len, n_out, 0, n_out, out, n_out, 0, stream);
 }
 
 extern "C" int b200sep_gather_pairs_f32(const float* src, const int* idx, float* dst, int64_t rows, int n_src_pairs, int n_gather, void* stream) {
