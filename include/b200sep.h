@@ -425,6 +425,10 @@ int b200sep_selftest_umma_gemm(const float* a, const float* w, const float* res,
                                int channels, const float* scale, const float* shift, int relu, void* stream);
 int b200sep_selftest_umma_conv3x3(const float* x, const float* w_host, float* out, int B, int Cin, int Cout, int T, int F, const float* scale,
                                   const float* shift, int relu, void* stream);
+/*   conv3x3_ex: out = ((act(conv2d(x, w, padding=1) * scale[co] + shift[co]) + res) * mul; act 0 none, 1 ReLU, 2 GELU; res, mul (B,Cout,T,F) may be
+ *            NULL (skipped), scale / shift may be NULL (1 / 0).  An epilogue the 3x3 kernel has no instance for returns B200SEP_ERR_ARG. */
+int b200sep_selftest_umma_conv3x3_ex(const float* x, const float* w_host, const float* res, const float* mul, float* out, int B, int Cin, int Cout, int T,
+                                     int F, const float* scale, const float* shift, int act, void* stream);
 /*   updown : up != 0: out(B,Cout,2T,2F) = act(conv_transpose2d(x, w(Cin,Cout,2,2), stride=2) * scale + shift) [* skip(B,Cout,2T,2F)]
  *            up == 0: out(B,Cout,T/2,F/2) = act(conv2d(x, w(Cout,Cin,2,2), stride=2) * scale + shift);  w is a HOST pointer, skip may be NULL */
 int b200sep_selftest_umma_updown(const float* x, const float* w_host, const float* skip, float* out, int B, int Cin, int Cout, int T, int F,

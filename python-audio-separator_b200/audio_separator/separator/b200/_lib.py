@@ -118,6 +118,7 @@ _SIGS = {
     "b200sep_ensemble_spec_abs": (i32, [vp, i32, i64, i32, i32, vp, vp]),
     "b200sep_selftest_umma_gemm": (i32, [vp, vp, vp, vp, i32, i32, i32, i32, i32, vp, vp, i32, vp]),
     "b200sep_selftest_umma_conv3x3": (i32, [vp, vp, vp, i32, i32, i32, i32, i32, vp, vp, i32, vp]),
+    "b200sep_selftest_umma_conv3x3_ex": (i32, [vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, vp, vp, i32, vp]),
     "b200sep_selftest_umma_updown": (i32, [vp, vp, vp, vp, i32, i32, i32, i32, i32, vp, vp, i32, i32, vp]),
     "b200sep_capture_begin": (i32, [vp]),
     "b200sep_capture_end": (i32, [vp, vp]),

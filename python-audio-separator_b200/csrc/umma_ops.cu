@@ -75,6 +75,12 @@ __device__ __forceinline__ float act1(float x, int act) {
   if (act == 2) return 0.5f * x * (1.f + erff(x * 0.70710678118654752440f));
   return x;
 }
+template <int ACT>
+__device__ __forceinline__ float act_c(float x) {  // act1 with the activation fixed at compile time
+  if constexpr (ACT == 1) return fmaxf(x, 0.f);
+  else if constexpr (ACT == 2) return 0.5f * x * (1.f + erff(x * 0.70710678118654752440f));
+  else return x;
+}
 
 __device__ __forceinline__ void split_store2(float v, bf16& hi, bf16& lo) {
   hi = __float2bfloat16_rn(v);
@@ -394,7 +400,9 @@ __device__ __forceinline__ void conv3_mma(float (&acc)[3 * NC / 2], uint64_t da,
   else ptx::wgmma_ss_n240<1>(acc, da, db, accum);
 }
 
-template <int NC>
+// The epilogue is fixed at compile time: ACT (0 none, 1 ReLU, 2 GELU), RES (+ residual), MUL (* multiplier).  umma_conv_run instantiates the
+// combinations the networks use (conv3_instance below).
+template <int NC, int ACT, bool RES, bool MUL>
 __global__ void __launch_bounds__(kUmmaThreads, 1) umma_conv3_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
                                                                      const __grid_constant__ CUtensorMap tmO_hi, const __grid_constant__ CUtensorMap tmO_lo,
                                                                      const UmmaParams p) {
@@ -463,32 +471,48 @@ __global__ void __launch_bounds__(kUmmaThreads, 1) umma_conv3_kernel(const __gri
     if (issuer) ptx::bulk_wait_read<0>();
     asm volatile("bar.sync %0, %1;" ::"n"(kEpiBar), "n"(kConsumerThreads) : "memory");
     const int n0 = tc.n_idx * NC;
+    // Tile row m = 16 * warp + g + 8h is output pixel f0 + m - 8 for m in [8, 120): warp 0 stores only its h = 1 rows, warp 7 only its h = 0 rows.
+    const bool row_out[2] = {warp != 0, warp != 7};
+    // residual / multiplier (B, Cout, T, F): element (n0 + col, row h) is at ro[h] + col * plane; pixels f >= F are staged unread (the store clips them)
+    const size_t plane = (size_t)p.T * p.F;
+    size_t ro[2];
+    bool f_in[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int f = tc.f0 + mrow0 + 8 * h - 8;
+      f_in[h] = f < p.F;
+      ro[h] = ((size_t)tc.b * p.Cout + n0) * plane + (size_t)tc.t * p.F + f;
+    }
 #pragma unroll
     for (int i = 0; i < G; ++i) {
+      const int col0 = 8 * i + 2 * cq;
+      // the neighbouring warps' edge rows of both columns: row 16w - 1 (P_0, read by g = 0) and row 16w + 16 (P_2, read by g = 7)
+      float2 prev = make_float2(0.f, 0.f), next = make_float2(0.f, 0.f);
+      if (g == 0 && warp > 0) prev = *reinterpret_cast<const float2*>(&edge0[(warp - 1) * NC + col0]);
+      if (g == 7 && warp < 7) next = *reinterpret_cast<const float2*>(&edge2[(warp + 1) * NC + col0]);
+      const float2 sc2 = *reinterpret_cast<const float2*>(&sc_s[n0 + col0]), sh2 = *reinterpret_cast<const float2*>(&sh_s[n0 + col0]);
 #pragma unroll
       for (int e = 0; e < 2; ++e) {
-        const int col = 8 * i + 2 * cq + e;
+        const int col = col0 + e;
         const float p0a = acc[4 * i + e], p0b = acc[4 * i + 2 + e];
         const float p1a = acc[4 * (G + i) + e], p1b = acc[4 * (G + i) + 2 + e];
         const float p2a = acc[4 * (2 * G + i) + e], p2b = acc[4 * (2 * G + i) + 2 + e];
         const float up_a = __shfl_sync(0xffffffffu, p0a, (lane + 28) & 31), up_b = __shfl_sync(0xffffffffu, p0b, (lane + 28) & 31);
         const float dn_a = __shfl_sync(0xffffffffu, p2a, (lane + 4) & 31), dn_b = __shfl_sync(0xffffffffu, p2b, (lane + 4) & 31);
-        const float prev = (g == 0 && warp > 0) ? edge0[(warp - 1) * NC + col] : 0.f;
-        const float next = (g == 7 && warp < 7) ? edge2[(warp + 1) * NC + col] : 0.f;
         float x[2];
-        x[0] = p1a + ((g > 0) ? up_a : prev) + ((g < 7) ? dn_a : dn_b);
-        x[1] = p1b + ((g > 0) ? up_b : up_a) + ((g < 7) ? dn_b : next);
+        x[0] = p1a + ((g > 0) ? up_a : (e ? prev.y : prev.x)) + ((g < 7) ? dn_a : dn_b);
+        x[1] = p1b + ((g > 0) ? up_b : up_a) + ((g < 7) ? dn_b : (e ? next.y : next.x));
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
+          if (!row_out[h]) continue;
           const int m = mrow0 + 8 * h;
-          if (m < 8 || m >= 8 + kConvStride) continue;
-          float y = act1(fmaf(x[h], sc_s[n0 + col], sh_s[n0 + col]), p.act);
-          const int f = tc.f0 + m - 8;
-          if ((p.res_hi || p.mul_hi) && f < p.F) {
-            const size_t plane = (size_t)p.T * p.F;
-            const size_t ro = ((size_t)tc.b * p.Cout + n0 + col) * plane + (size_t)tc.t * p.F + f;  // residual / multiplier: (B, Cout, T, F)
-            if (p.res_hi) y += pair_at(p.res_hi, p.res_lo, ro);
-            if (p.mul_hi) y *= pair_at(p.mul_hi, p.mul_lo, ro);
+          float y = act_c<ACT>(fmaf(x[h], e ? sc2.y : sc2.x, e ? sh2.y : sh2.x));
+          if constexpr (RES || MUL) {
+            if (f_in[h]) {
+              const size_t o = ro[h] + (size_t)col * plane;
+              if constexpr (RES) y += pair_at(p.res_hi, p.res_lo, o);
+              if constexpr (MUL) y *= pair_at(p.mul_hi, p.mul_lo, o);
+            }
           }
           split_store2(y, s_hi[col * kConvStride + (m - 8)], s_lo[col * kConvStride + (m - 8)]);
         }
@@ -811,14 +835,27 @@ static int store_map(const void* base, int F, int T, int C, int box_c, CUtensorM
   return B200SEP_OK;
 }
 
-template <int NC>
+template <int NC, int ACT, bool RES, bool MUL>
 static int launch_conv3(const CUtensorMap& a_hi, const CUtensorMap& a_lo, const CUtensorMap& o_hi, const CUtensorMap& o_lo, UmmaParams& p, size_t smem, cudaStream_t st) {
   static bool attr_set = false;
   if (!attr_set) {
-    B2_CUDA(cudaFuncSetAttribute(umma_conv3_kernel<NC>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    B2_CUDA(cudaFuncSetAttribute(umma_conv3_kernel<NC, ACT, RES, MUL>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     attr_set = true;
   }
-  return launch_persistent(umma_conv3_kernel<NC>, p.num_tiles, smem, st, a_hi, a_lo, o_hi, o_lo, p);
+  return launch_persistent(umma_conv3_kernel<NC, ACT, RES, MUL>, p.num_tiles, smem, st, a_hi, a_lo, o_hi, o_lo, p);
+}
+
+// The epilogue variants with a kernel instance: MDX-Net's BN + ReLU; MDX23C's TFC convolutions (plain, + residual, + residual * multiplier).
+template <int NC>
+static int conv3_instance(const CUtensorMap& a_hi, const CUtensorMap& a_lo, const CUtensorMap& o_hi, const CUtensorMap& o_lo, UmmaParams& p, size_t smem,
+                          cudaStream_t st) {
+  const bool res = p.res_hi != nullptr, mul = p.mul_hi != nullptr;
+  if (p.act == 1 && !res && !mul) return launch_conv3<NC, 1, false, false>(a_hi, a_lo, o_hi, o_lo, p, smem, st);
+  if (p.act == 0 && !res && !mul) return launch_conv3<NC, 0, false, false>(a_hi, a_lo, o_hi, o_lo, p, smem, st);
+  if (p.act == 0 && res && !mul) return launch_conv3<NC, 0, true, false>(a_hi, a_lo, o_hi, o_lo, p, smem, st);
+  if (p.act == 0 && res && mul) return launch_conv3<NC, 0, true, true>(a_hi, a_lo, o_hi, o_lo, p, smem, st);
+  set_error("umma_conv: no 3x3 kernel instance for the epilogue act=%d residual=%d multiplier=%d", p.act, (int)res, (int)mul);
+  return B200SEP_ERR_ARG;
 }
 
 int umma_conv_run(const UmmaConvPlan& pl, const void* wb_hi, const void* wb_lo, int B, int Cout, int n_c, const UmmaEpilogue& e, cudaStream_t st) {
@@ -850,11 +887,11 @@ int umma_conv_run(const UmmaConvPlan& pl, const void* wb_hi, const void* wb_lo, 
   if (!rc) rc = store_map(p.out_lo, pl.F, pl.T, B * p.out_c_total, n_c, &o_lo);
   if (rc) return rc;
   switch (n_c) {
-    case 16: return launch_conv3<16>(pl.a_hi, pl.a_lo, o_hi, o_lo, p, smem, st);
-    case 32: return launch_conv3<32>(pl.a_hi, pl.a_lo, o_hi, o_lo, p, smem, st);
-    case 48: return launch_conv3<48>(pl.a_hi, pl.a_lo, o_hi, o_lo, p, smem, st);
-    case 64: return launch_conv3<64>(pl.a_hi, pl.a_lo, o_hi, o_lo, p, smem, st);
-    case 80: return launch_conv3<80>(pl.a_hi, pl.a_lo, o_hi, o_lo, p, smem, st);
+    case 16: return conv3_instance<16>(pl.a_hi, pl.a_lo, o_hi, o_lo, p, smem, st);
+    case 32: return conv3_instance<32>(pl.a_hi, pl.a_lo, o_hi, o_lo, p, smem, st);
+    case 48: return conv3_instance<48>(pl.a_hi, pl.a_lo, o_hi, o_lo, p, smem, st);
+    case 64: return conv3_instance<64>(pl.a_hi, pl.a_lo, o_hi, o_lo, p, smem, st);
+    case 80: return conv3_instance<80>(pl.a_hi, pl.a_lo, o_hi, o_lo, p, smem, st);
   }
   set_error("umma_conv: n_c=%d has no kernel instance", n_c);
   return B200SEP_ERR_ARG;
@@ -937,30 +974,44 @@ extern "C" int b200sep_selftest_umma_gemm(const float* a, const float* w, const 
   return rc;
 }
 
-extern "C" int b200sep_selftest_umma_conv3x3(const float* x, const float* w_host, float* out, int B, int Cin, int Cout, int T, int F, const float* scale,
-                                             const float* shift, int relu, void* stream) {
-  B2_CHECK_ARG(x && w_host && out && scale && shift, "selftest_umma_conv3x3: NULL argument");
+extern "C" int b200sep_selftest_umma_conv3x3_ex(const float* x, const float* w_host, const float* res, const float* mul, float* out, int B, int Cin, int Cout,
+                                                int T, int F, const float* scale, const float* shift, int act, void* stream) {
+  B2_CHECK_ARG(x && w_host && out, "selftest_umma_conv3x3: NULL argument");
   B2_CHECK_ARG(umma_conv_supported(Cin, Cout, F, 3, 3), "selftest_umma_conv3x3: Cin=%d Cout=%d F=%d not supported by the tensor-core path", Cin, Cout, F);
   cudaStream_t st = (cudaStream_t)stream;
   std::vector<uint16_t> hi, lo;
   const int n_c = umma_block_weights(UMMA_CONV3, w_host, Cin, Cout, hi, lo);
-  uint16_t *x_p = nullptr, *o_p = nullptr, *w_p = nullptr;
+  uint16_t *x_p = nullptr, *o_p = nullptr, *w_p = nullptr, *r_p = nullptr, *m_p = nullptr;
   const int64_t nx = (int64_t)B * Cin * T * F, no = (int64_t)B * Cout * T * F, nw = (int64_t)hi.size();
   B2_CUDA(cudaMalloc(&x_p, nx * 4));
   B2_CUDA(cudaMalloc(&o_p, no * 4));
   B2_CUDA(cudaMalloc(&w_p, nw * 4));
+  if (res) B2_CUDA(cudaMalloc(&r_p, no * 4));
+  if (mul) B2_CUDA(cudaMalloc(&m_p, no * 4));
   B2_CUDA(cudaMemcpy(w_p, hi.data(), nw * 2, cudaMemcpyHostToDevice));
   B2_CUDA(cudaMemcpy(w_p + nw, lo.data(), nw * 2, cudaMemcpyHostToDevice));
   int rc = split_pair(x, x_p, x_p + nx, nx, st);
+  if (!rc && res) rc = split_pair(res, r_p, r_p + no, no, st);
+  if (!rc && mul) rc = split_pair(mul, m_p, m_p + no, no, st);
   UmmaConvPlan pl;
   if (!rc) rc = umma_conv_plan_create(&pl, UMMA_CONV3, x_p, x_p + nx, B, Cin, Cout, T, F);
   UmmaEpilogue e;
-  e.scale = scale; e.shift = shift; e.act = relu ? 1 : 0; e.out_hi = o_p; e.out_lo = o_p + no;
+  e.scale = scale; e.shift = shift; e.act = act; e.out_hi = o_p; e.out_lo = o_p + no;
+  if (res) { e.res_hi = r_p; e.res_lo = r_p + no; }
+  if (mul) { e.mul_hi = m_p; e.mul_lo = m_p + no; }
   if (!rc) rc = umma_conv_run(pl, w_p, w_p + nw, B, Cout, n_c, e, st);
   if (!rc) rc = join_pair(o_p, o_p + no, out, no, st);
   cudaStreamSynchronize(st);
   cudaFree(x_p); cudaFree(o_p); cudaFree(w_p);
+  if (r_p) cudaFree(r_p);
+  if (m_p) cudaFree(m_p);
   return rc;
+}
+
+extern "C" int b200sep_selftest_umma_conv3x3(const float* x, const float* w_host, float* out, int B, int Cin, int Cout, int T, int F, const float* scale,
+                                             const float* shift, int relu, void* stream) {
+  B2_CHECK_ARG(scale && shift, "selftest_umma_conv3x3: NULL argument");
+  return b200sep_selftest_umma_conv3x3_ex(x, w_host, nullptr, nullptr, out, B, Cin, Cout, T, F, scale, shift, relu ? 1 : 0, stream);
 }
 
 extern "C" int b200sep_selftest_umma_updown(const float* x, const float* w_host, const float* skip, float* out, int B, int Cin, int Cout, int T, int F,
