@@ -29,6 +29,13 @@ extern "C" {
 
 #define B200SEP_ABI_VERSION 1
 
+/* math modes of the fp32-operator tensor-core kernels (the *_math entry points; every entry without the suffix uses BF16X3):
+ *   BF16X3: each fp32 operand split into bf16 hi + lo, three products (Ah*Bh + Ah*Bl + Al*Bh), fp32 accumulation (~fp32 accuracy).
+ *   FP16:   each fp32 operand rounded once to fp16 (round to nearest even; |x| > 65504 becomes +-inf, as torch.autocast's cast), one product,
+ *           fp32 accumulation: the precision of torch.autocast("cuda") on these operators.  The SIMT fallbacks stay fp32 in both modes. */
+#define B200SEP_MATH_BF16X3 0
+#define B200SEP_MATH_FP16 1
+
 /* spectrogram memory layouts */
 #define B200SEP_LAYOUT_CFT 0 /* (B, 2C, dim_f, frames): the reference's STFT.__call__ layout (uvr_lib_v5/stft.py:44-56) */
 #define B200SEP_LAYOUT_CTF 1 /* (B, 2C, frames, dim_f): what ConvTDFNet computes on after transpose(-1,-2) (uvr_lib_v5/mdxnet.py:101) */
@@ -240,6 +247,9 @@ int b200sep_stft_inverse_ex(const b200sep_stft_plan* plan, const float* spec, in
 int b200sep_conv2d_f32(const float* x, const float* w_blocked, const float* bias, const float* add, float* y, int B, int Cin, int H, int W, int Cout,
                        int Ho, int Wo, int KH, int KW, int SH, int SW, int PH, int PW, int DH, int DW, int act, int add_before_act, int up_axis, int up,
                        int trim, int out_len, int out_c_total, int out_c_off, const void* w_packed, void* stream);
+int b200sep_conv2d_f32_math(const float* x, const float* w_blocked, const float* bias, const float* add, float* y, int B, int Cin, int H, int W, int Cout,
+                            int Ho, int Wo, int KH, int KW, int SH, int SW, int PH, int PW, int DH, int DW, int act, int add_before_act, int up_axis, int up,
+                            int trim, int out_len, int out_c_total, int out_c_off, const void* w_packed, int math, void* stream);
 /* nn.GroupNorm(1, C), affine, optional activation (demucs.py:141,144).  Channel-first x (B, C, Fr, L): one sample per (b, fr) row
  * (Fr = 1: (B, C, L); Fr > 1: DConv on every frequency row without the permute of hdemucs.py:141-146); channel_last: x (B, L, C)
  * tokens (MyGroupNorm, transformer.py:184-193).
@@ -258,12 +268,21 @@ int b200sep_layernorm_f32(const float* x, const float* gamma, const float* beta,
 int b200sep_gemm_f32(const float* A, const float* Bw, float* C, int M, int N, int K, int lda, int ldb, int ldc, int batch, int64_t strideA,
                      int64_t strideB, int64_t strideC, float alpha, const float* bias_n, const float* bias_m, int act, const float* res,
                      const float* res_scale, const void* w_packed, void* stream);
+int b200sep_gemm_f32_math(const float* A, const float* Bw, float* C, int M, int N, int K, int lda, int ldb, int ldc, int batch, int64_t strideA,
+                          int64_t strideB, int64_t strideC, float alpha, const float* bias_n, const float* bias_m, int act, const float* res,
+                          const float* res_scale, const void* w_packed, int math, void* stream);
 /* Large conv2d_f32 / gemm_f32 calls run on the tensor cores (csrc/tc_f32.cu: fp32 operands split in-kernel into bf16 hi + lo, three
  * wgmma products, fp32 accumulation).  For STATIC B operands (weights) the split can be done once: w_packed (nullable) is the image
  * tc_pack_*_weights writes into a buffer of b200sep_tc_packed_floats(N, K) floats, K = the GEMM K (linear) or ceil8(Cin)*KH*KW (conv). */
 int64_t b200sep_tc_packed_floats(int N, int K);
 int b200sep_tc_pack_linear_weights(const float* W, int N, int K, int ldw, float* packed, void* stream);
 int b200sep_tc_pack_conv_weights(const float* w_blocked, int Cin, int taps, int Cout, float* packed, void* stream);
+/* the same for a math mode: the FP16 image has one fp16 plane per (n-tile, k-block) block, half the bytes.  An image passed as w_packed to a call of
+ * the other mode returns B200SEP_ERR_ARG (the library remembers the mode each image address was last packed for; nothing is read from the device).
+ * Only images packed in this process, used at the address they were packed to, are checked: a copy made elsewhere is trusted. */
+int64_t b200sep_tc_packed_floats_math(int N, int K, int math);
+int b200sep_tc_pack_linear_weights_math(const float* W, int N, int K, int ldw, float* packed, int math, void* stream);
+int b200sep_tc_pack_conv_weights_math(const float* w_blocked, int Cin, int taps, int Cout, float* packed, int math, void* stream);
 /* Fused attention, head dimension 64: out[b, m, h*64 + d] = sum_n softmax_n(alpha <q[b, m, h], k[b, n, h]>) v[b, n, h*64 + d] with the scores kept on chip
  * (one wgmma kernel: Q K^T into registers, running softmax on the fragments, P V with P as the register operand).  q (B, Lq, .) / k (B, Lk, .) / out (B, Lq, .): batch and row
  * strides in floats, head h at columns [h*64, h*64 + 64);  v_is_kn = 0: vt = V TRANSPOSED, vt[b * vt_batch_stride + (h*64 + d) * vt_row_stride + n] (keys
@@ -272,10 +291,15 @@ int b200sep_tc_pack_conv_weights(const float* w_blocked, int Cin, int taps, int 
 int b200sep_attention_f32(const float* q, const float* k, const float* vt, float* out, int B, int H, int Lq, int Lk, int head_dim, int64_t q_batch_stride,
                           int64_t q_row_stride, int64_t k_batch_stride, int64_t k_row_stride, int64_t vt_batch_stride, int64_t vt_row_stride,
                           int64_t out_batch_stride, int64_t out_row_stride, float alpha, int v_is_kn, float* work, void* stream);
+/* FP16: Q K^T and P V each one fp16 product; the online softmax stays fp32 and P is rounded to fp16 before the second product */
+int b200sep_attention_f32_math(const float* q, const float* k, const float* vt, float* out, int B, int H, int Lq, int Lk, int head_dim, int64_t q_batch_stride,
+                               int64_t q_row_stride, int64_t k_batch_stride, int64_t k_row_stride, int64_t vt_batch_stride, int64_t vt_row_stride,
+                               int64_t out_batch_stride, int64_t out_row_stride, float alpha, int v_is_kn, float* work, int math, void* stream);
 /* work (nullable): b200sep_attention_work_floats(...) floats of 16-byte aligned device scratch.  With it Q / K / V are split into bf16 hi / lo tile images ONCE
  * (a small pre-pass) and the attention kernel fetches them with bulk copies; without it every CTA converts the tiles it reads (slower: each K / V tile is read
  * by all query tiles of its (batch, head)). */
 int64_t b200sep_attention_work_floats(int B, int H, int Lq, int Lk);
+int64_t b200sep_attention_work_floats_math(int B, int H, int Lq, int Lk, int math); /* FP16: half of the BF16X3 size */
 /* in-place softmax over the first n columns of each row (row stride ld >= n; padding columns are left untouched) */
 int b200sep_softmax_rows_f32(float* x, int64_t rows, int n, int64_t ld, void* stream);
 /* batched C[z] = alpha * A[z] (M,K; lda) @ B[z] (K,N; ldb): the P @ V product of attention without a transposed copy of V */

@@ -16,7 +16,7 @@ import torch
 from ..b200.demucs import DemucsEngine, HTDemucsNet
 from ..b200.demucs_loader import load_demucs
 from ..b200.hdemucs import HDemucsConfig, HDemucsNet
-from ..common_separator import CommonSeparator
+from ..common_separator import CommonSeparator, tensor_core_math
 
 DEMUCS_2_SOURCE_MAPPER = {CommonSeparator.INST_STEM: 0, CommonSeparator.VOCAL_STEM: 1}
 DEMUCS_4_SOURCE_MAPPER = {CommonSeparator.BASS_STEM: 0, CommonSeparator.DRUM_STEM: 1, CommonSeparator.OTHER_STEM: 2, CommonSeparator.VOCAL_STEM: 3}
@@ -41,6 +41,7 @@ class DemucsSeparator(CommonSeparator):
         """get_demucs_model(name, repo) + demucs_segments(segment_size, model) (demucs_separator.py:110-114, apply.py:263-300)."""
         models, weights, bag_segment = load_demucs(self.model_path)
         nets = []
+        math = tensor_core_math("Demucs", self.use_autocast)
         for cfg, state in models:
             if bag_segment is not None:  # BagOfModels.__init__ (apply.py:58-60)
                 cfg.segment = Fraction(bag_segment)
@@ -49,7 +50,7 @@ class DemucsSeparator(CommonSeparator):
                     cfg.segment = Fraction(int(self.segment_size))  # demucs_segments: sub.segment = int(segment)
                 except (TypeError, ValueError):
                     pass
-            nets.append((HDemucsNet if isinstance(cfg, HDemucsConfig) else HTDemucsNet)(cfg, state, device=self.torch_device))
+            nets.append((HDemucsNet if isinstance(cfg, HDemucsConfig) else HTDemucsNet)(cfg, state, device=self.torch_device, math=math))
         # segments_enabled=False: apply_model(split=False), one forward over the whole track (HTDemucs raises beyond its training segment, like the reference)
         self.engine = DemucsEngine(nets, bag_weights=weights, overlap=self.overlap, batch_size=self.batch_size, split=bool(self.segments_enabled))
 

@@ -17,7 +17,7 @@ import torch
 
 from ..b200.engine import MdxcEngine, TfcNet
 from ..b200.roformer import BSRoformerConfig, BSRoformerNet, MelBandRoformerConfig, RoformerEngine
-from ..common_separator import CommonSeparator, normalize
+from ..common_separator import CommonSeparator, normalize, tensor_core_math
 
 
 class MDXCSeparator(CommonSeparator):
@@ -54,6 +54,8 @@ class MDXCSeparator(CommonSeparator):
         audio, model, training = cfg["audio"], cfg["model"], cfg["training"]
         if self.is_roformer:
             return self._load_roformer(cfg)
+        if self.use_autocast:
+            self.logger.debug("use_autocast: MDX23C (TFC_TDF_net) keeps full precision; its pair-format kernels have no fp16 mode")
         if model.get("norm") != "InstanceNorm" or model.get("act", "gelu") != "gelu" or list(model.get("scale", [2, 2])) != [2, 2]:
             raise ValueError("the H100 TFC_TDF_net supports norm=InstanceNorm, act=gelu, scale=[2,2] (the MDX23C configuration)")
         path = self.model_path
@@ -100,7 +102,7 @@ class MDXCSeparator(CommonSeparator):
         else:
             sd = torch.load(path, map_location="cpu", weights_only=True)
             state = {k: v.float().numpy() for k, v in (sd.get("state_dict", sd)).items()}
-        self.net = BSRoformerNet(rcfg, state, device=self.torch_device)
+        self.net = BSRoformerNet(rcfg, state, device=self.torch_device, math=tensor_core_math("Roformer", self.use_autocast))
         self._select_engine()
 
     def _demix_stems(self, orig):

@@ -13,7 +13,7 @@ import torch
 
 from ..b200 import vr_params
 from ..b200.vr import NN_ARCH_SIZES, VR_51_SIZES, VREngine, VRNet, VRNet51
-from ..common_separator import CommonSeparator
+from ..common_separator import CommonSeparator, tensor_core_math
 
 
 class VRSeparator(CommonSeparator):
@@ -53,10 +53,12 @@ class VRSeparator(CommonSeparator):
         else:
             sd = torch.load(self.model_path, map_location="cpu", weights_only=True)
             state = {k: v.numpy() for k, v in sd.items()}
+        tc_math = tensor_core_math("VR", self.use_autocast)
         if self.is_vr_51_model:
-            self.net = VRNet51(self.model_params["bins"] * 2, self.model_capacity[0], self.model_capacity[1], state, nn_arch_size=arch, device=self.torch_device)
+            self.net = VRNet51(self.model_params["bins"] * 2, self.model_capacity[0], self.model_capacity[1], state, nn_arch_size=arch, device=self.torch_device,
+                               math=tc_math)
         else:
-            self.net = VRNet(arch, self.model_params["bins"] * 2, state, device=self.torch_device)
+            self.net = VRNet(arch, self.model_params["bins"] * 2, state, device=self.torch_device, math=tc_math)
         self.engine = VREngine(self.net, self.model_params, self.window_size, self.aggression_setting, self.primary_stem_name, self.batch_size)
 
     def separate(self, audio_file_path, custom_output_names=None):

@@ -19,6 +19,10 @@ lib = C.CDLL(LIB_PATH)
 LAYOUT_CFT = 0
 LAYOUT_CTF = 1
 
+# math modes of the fp32-operator tensor-core kernels (the *_math entry points)
+MATH_BF16X3 = 0  # bf16 hi / lo split, three products: ~fp32 accuracy (every entry without the suffix)
+MATH_FP16 = 1  # operands rounded once to fp16, one product: the precision of torch.autocast
+
 i32, i64, f32, vp = C.c_int, C.c_int64, C.c_float, C.c_void_p
 
 
@@ -64,6 +68,7 @@ _SIGS = {
     "b200sep_stft_forward_ex": (i32, [vp, vp, i64, i64, i64, i32, i32, i32, i32, f32, i32, i32, i32, i32, vp, vp]),
     "b200sep_stft_inverse_ex": (i32, [vp, vp, i32, i32, i32, i32, i32, i32, i32, f32, vp, vp, vp]),
     "b200sep_conv2d_f32": (i32, [vp, vp, vp, vp, vp] + [i32] * 23 + [vp, vp]),
+    "b200sep_conv2d_f32_math": (i32, [vp, vp, vp, vp, vp] + [i32] * 23 + [vp, i32, vp]),
     "b200sep_lstm_bidir_f32": (i32, [vp, vp, vp, i32, i32, i32, vp]),
     "b200sep_add_rowvec_f32": (i32, [vp, vp, i32, i32, i64, vp]),
     "b200sep_groupnorm_work_floats": (i64, [i32, i32, i32, i64]),
@@ -75,15 +80,21 @@ _SIGS = {
     "b200sep_tc_packed_floats": (i64, [i32, i32]),
     "b200sep_tc_pack_linear_weights": (i32, [vp, i32, i32, i32, vp, vp]),
     "b200sep_tc_pack_conv_weights": (i32, [vp, i32, i32, i32, vp, vp]),
+    "b200sep_tc_packed_floats_math": (i64, [i32, i32, i32]),
+    "b200sep_tc_pack_linear_weights_math": (i32, [vp, i32, i32, i32, vp, i32, vp]),
+    "b200sep_tc_pack_conv_weights_math": (i32, [vp, i32, i32, i32, vp, i32, vp]),
     "b200sep_groupnorm1_work_floats": (i64, [i32, i32, i32, i64]),
     "b200sep_groupnorm1_f32": (i32, [vp, vp, vp, vp, i32, i32, i32, i64, i32, i32, vp, vp]),
     "b200sep_permute4_f32": (i32, [vp, vp, i32, i32, i32, i32, i32, i32, i32, i32, vp]),
     "b200sep_glu_f32": (i32, [vp, vp, vp, vp, i32, i32, i64, vp]),
     "b200sep_layernorm_f32": (i32, [vp, vp, vp, vp, i64, i32, vp]),
     "b200sep_gemm_f32": (i32, [vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, i64, i64, i64, f32, vp, vp, i32, vp, vp, vp, vp]),
+    "b200sep_gemm_f32_math": (i32, [vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, i64, i64, i64, f32, vp, vp, i32, vp, vp, vp, i32, vp]),
     "b200sep_softmax_rows_f32": (i32, [vp, i64, i32, i64, vp]),
     "b200sep_attention_f32": (i32, [vp, vp, vp, vp, i32, i32, i32, i32, i32, i64, i64, i64, i64, i64, i64, i64, i64, f32, i32, vp, vp]),
     "b200sep_attention_work_floats": (i64, [i32, i32, i32, i32]),
+    "b200sep_attention_f32_math": (i32, [vp, vp, vp, vp, i32, i32, i32, i32, i32, i64, i64, i64, i64, i64, i64, i64, i64, f32, i32, vp, i32, vp]),
+    "b200sep_attention_work_floats_math": (i64, [i32, i32, i32, i32, i32]),
     "b200sep_ew_f32": (i32, [vp, vp, vp, i64, f32, f32, i32, vp]),
     "b200sep_meanstd_f32": (i32, [vp, i64, vp, vp]),
     "b200sep_meanstd_work_floats": (i64, [i32]),

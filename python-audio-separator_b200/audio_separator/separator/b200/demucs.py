@@ -17,7 +17,7 @@ from fractions import Fraction
 import numpy as np
 import torch
 
-from ._lib import LAYOUT_CFT, check, lib
+from ._lib import LAYOUT_CFT, MATH_BF16X3, check, lib
 from .engine import StftPlan, _ptr, _require_cuda, _stream
 
 ACT_NONE, ACT_RELU, ACT_GELU = 0, 1, 2
@@ -122,29 +122,41 @@ def _new(shape, like=None, device=None):
     return torch.empty(shape, dtype=torch.float32, device=like.device if like is not None else device)
 
 
-def _packed_conv(wb, cin, taps, cout):
-    """The tensor-core image of a blocked convolution weight (bf16 hi/lo planes in the kernel's shared-memory layout), built once per tensor."""
-    pk = getattr(wb, "_b200_packed", None)
+def _packed_cache(w):
+    """{math mode: packed image} of one weight tensor"""
+    cache = getattr(w, "_b200_packed", None)
+    if cache is None:
+        cache = w._b200_packed = {}
+    return cache
+
+
+def _packed_conv(wb, cin, taps, cout, math=MATH_BF16X3):
+    """The tensor-core image of a blocked convolution weight (bf16 hi/lo planes, or one fp16 plane, in the kernel's shared-memory layout), built once
+    per tensor and math mode."""
+    cache = _packed_cache(wb)
+    pk = cache.get(math)
     if pk is None and cin * taps >= 32 and cout >= 16:
         cin8 = -(-cin // 8) * 8
-        pk = _new((lib.b200sep_tc_packed_floats(cout, cin8 * taps),), wb)
-        check(lib.b200sep_tc_pack_conv_weights(_ptr(wb), cin, taps, cout, _ptr(pk), _stream()), "tc_pack_conv_weights")
-        wb._b200_packed = pk
+        pk = _new((lib.b200sep_tc_packed_floats_math(cout, cin8 * taps, math),), wb)
+        check(lib.b200sep_tc_pack_conv_weights_math(_ptr(wb), cin, taps, cout, _ptr(pk), math, _stream()), "tc_pack_conv_weights")
+        cache[math] = pk
     return pk
 
 
-def _packed_linear(w):
-    pk = getattr(w, "_b200_packed", None)
+def _packed_linear(w, math=MATH_BF16X3):
+    cache = _packed_cache(w)
+    pk = cache.get(math)
     if pk is None and w.shape[0] >= 32 and w.shape[1] >= 32:
-        pk = _new((lib.b200sep_tc_packed_floats(w.shape[0], w.shape[1]),), w)
-        check(lib.b200sep_tc_pack_linear_weights(_ptr(w), w.shape[0], w.shape[1], w.shape[1], _ptr(pk), _stream()), "tc_pack_linear_weights")
-        w._b200_packed = pk
+        pk = _new((lib.b200sep_tc_packed_floats_math(w.shape[0], w.shape[1], math),), w)
+        check(lib.b200sep_tc_pack_linear_weights_math(_ptr(w), w.shape[0], w.shape[1], w.shape[1], _ptr(pk), math, _stream()), "tc_pack_linear_weights")
+        cache[math] = pk
     return pk
 
 
-def conv2d(x, wb, bias, cout, k, s=(1, 1), p=(0, 0), dw=1, act=ACT_NONE, add=None, add_before_act=False, out_hw=None, out=None, out_c_off=0, dh=1):
+def conv2d(x, wb, bias, cout, k, s=(1, 1), p=(0, 0), dw=1, act=ACT_NONE, add=None, add_before_act=False, out_hw=None, out=None, out_c_off=0, dh=1, math=MATH_BF16X3):
     """x (B,Cin,H,W) -> (B,cout,Ho,Wo);  out_hw overrides the implied output size (right/bottom zero padding is implicit);
-    out/out_c_off: write into channels [out_c_off, out_c_off + cout) of an existing (B, C_total, Ho, Wo) tensor (a fused torch.cat)."""
+    out/out_c_off: write into channels [out_c_off, out_c_off + cout) of an existing (B, C_total, Ho, Wo) tensor (a fused torch.cat).
+    math: MATH_BF16X3 or MATH_FP16 (tensor-core arithmetic; the SIMT fallback for small shapes is fp32 either way)."""
     B, cin, H, W = x.shape
     if out_hw is None:
         Ho = (H + 2 * p[0] - dh * (k[0] - 1) - 1) // s[0] + 1
@@ -156,14 +168,14 @@ def conv2d(x, wb, bias, cout, k, s=(1, 1), p=(0, 0), dw=1, act=ACT_NONE, add=Non
     else:
         assert out.shape[0] == B and tuple(out.shape[2:]) == (Ho, Wo), (out.shape, (B, cout, Ho, Wo))
         y, ct = out, out.shape[1]
-    pk = _packed_conv(wb, cin, k[0] * k[1], cout)
-    check(lib.b200sep_conv2d_f32(_ptr(x), _ptr(wb), _ptr(bias) if bias is not None else None, _ptr(add) if add is not None else None, _ptr(y), B, cin, H, W, cout,
-                                 Ho, Wo, k[0], k[1], s[0], s[1], p[0], p[1], dh, dw, act, int(add_before_act), 0, 1, 0, 0, ct, out_c_off,
-                                 _ptr(pk) if pk is not None else None, _stream()), "conv2d_f32")
+    pk = _packed_conv(wb, cin, k[0] * k[1], cout, math)
+    check(lib.b200sep_conv2d_f32_math(_ptr(x), _ptr(wb), _ptr(bias) if bias is not None else None, _ptr(add) if add is not None else None, _ptr(y), B, cin, H, W, cout,
+                                      Ho, Wo, k[0], k[1], s[0], s[1], p[0], p[1], dh, dw, act, int(add_before_act), 0, 1, 0, 0, ct, out_c_off,
+                                      _ptr(pk) if pk is not None else None, math, _stream()), "conv2d_f32")
     return y
 
 
-def conv_transpose(x, wb, bias, cout, axis, stride, trim, out_len, act=ACT_NONE):
+def conv_transpose(x, wb, bias, cout, axis, stride, trim, out_len, act=ACT_NONE, math=MATH_BF16X3):
     """nn.ConvTranspose1d/2d with kernel 2*stride along `axis` (1 = H, 2 = W), output cropped to [trim, trim + out_len)."""
     B, cin, H, W = x.shape
     if axis == 1:
@@ -172,9 +184,9 @@ def conv_transpose(x, wb, bias, cout, axis, stride, trim, out_len, act=ACT_NONE)
     else:
         y = _new((B, cout, H, out_len), x)
         k, p, hw = (1, 2), (0, 1), (H, W + 1)
-    pk = _packed_conv(wb, cin, 2, stride * cout)
-    check(lib.b200sep_conv2d_f32(_ptr(x), _ptr(wb), _ptr(bias), None, _ptr(y), B, cin, H, W, stride * cout, hw[0], hw[1], k[0], k[1], 1, 1, p[0], p[1], 1, 1, act, 0,
-                                 axis, stride, trim, out_len, 0, 0, _ptr(pk) if pk is not None else None, _stream()), "conv2d_f32(transposed)")
+    pk = _packed_conv(wb, cin, 2, stride * cout, math)
+    check(lib.b200sep_conv2d_f32_math(_ptr(x), _ptr(wb), _ptr(bias), None, _ptr(y), B, cin, H, W, stride * cout, hw[0], hw[1], k[0], k[1], 1, 1, p[0], p[1], 1, 1, act,
+                                      0, axis, stride, trim, out_len, 0, 0, _ptr(pk) if pk is not None else None, math, _stream()), "conv2d_f32(transposed)")
     return y
 
 
@@ -208,30 +220,34 @@ def ew(a, b, out, alpha=1.0, beta=1.0, op=0):
     return out
 
 
-def linear(x2d, w, bias, act=ACT_NONE, res=None, res_scale=None):
+def linear(x2d, w, bias, act=ACT_NONE, res=None, res_scale=None, math=MATH_BF16X3):
     """(M,K) @ w(N,K)^T + bias -> (M,N); optional res + res_scale[n] * (.)"""
     M, K = x2d.shape
     N = w.shape[0]
     y = _new((M, N), x2d)
-    pk = _packed_linear(w)
-    check(lib.b200sep_gemm_f32(_ptr(x2d), _ptr(w), _ptr(y), M, N, K, K, K, N, 1, 0, 0, 0, 1.0, _ptr(bias) if bias is not None else None, None, act,
-                               _ptr(res) if res is not None else None, _ptr(res_scale) if res_scale is not None else None, _ptr(pk) if pk is not None else None,
-                               _stream()), "gemm_f32")
+    pk = _packed_linear(w, math)
+    check(lib.b200sep_gemm_f32_math(_ptr(x2d), _ptr(w), _ptr(y), M, N, K, K, K, N, 1, 0, 0, 0, 1.0, _ptr(bias) if bias is not None else None, None, act,
+                                    _ptr(res) if res is not None else None, _ptr(res_scale) if res_scale is not None else None, _ptr(pk) if pk is not None else None,
+                                    math, _stream()), "gemm_f32")
     return y
 
 
-def _gemm_raw(a_ptr, b_ptr, c_ptr, M, N, K, lda, ldb, ldc, batch, sA, sB, sC, alpha=1.0, bias_n=None, bias_m=None):
-    check(lib.b200sep_gemm_f32(a_ptr, b_ptr, c_ptr, M, N, K, lda, ldb, ldc, batch, sA, sB, sC, alpha, bias_n, bias_m, 0, None, None, None, _stream()), "gemm_f32")
+def _gemm_raw(a_ptr, b_ptr, c_ptr, M, N, K, lda, ldb, ldc, batch, sA, sB, sC, alpha=1.0, bias_n=None, bias_m=None, math=MATH_BF16X3):
+    check(lib.b200sep_gemm_f32_math(a_ptr, b_ptr, c_ptr, M, N, K, lda, ldb, ldc, batch, sA, sB, sC, alpha, bias_n, bias_m, 0, None, None, None, math, _stream()),
+          "gemm_f32")
 
 
 # --------------------------------------------------------------------------------------------------------- the network
 class HTDemucsNet:
     """Device-resident HTDemucs weights (re-blocked for the conv kernel) + the launch sequence of one forward."""
 
-    def __init__(self, cfg: HTDemucsConfig, state: dict, device=None):
+    def __init__(self, cfg: HTDemucsConfig, state: dict, device=None, math=MATH_BF16X3):
+        """math: MATH_BF16X3 (default, ~fp32) or MATH_FP16 (torch.autocast precision) for every tensor-core GEMM, convolution and attention of
+        this net, fixed for its lifetime (the graphs GraphedForward captures record the mode of each launch)."""
         _require_cuda()
         cfg.validate()
         self.cfg = cfg
+        self.math = int(math)
         self.device = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())  # one process per GPU: the rank's own device
         self.S = len(cfg.sources)
         self.stft = StftPlan(cfg.nfft, cfg.hop)
@@ -304,15 +320,15 @@ class HTDemucsNet:
                 # one fused residual layer (csrc/dconv_fused.cu); the C -> hid convolution of the widest layers stays on the tensor cores
                 u_in = None
                 if 3 * C_ * (-(-hid // 4) * 4) * 4 > 200 * 1024:
-                    u_in = conv2d(x, W[f"{p}.0.weight"], W[f"{p}.0.bias"], hid, (1, 3), p=(0, dil), dw=dil)
+                    u_in = conv2d(x, W[f"{p}.0.weight"], W[f"{p}.0.bias"], hid, (1, 3), p=(0, dil), dw=dil, math=self.math)
                 work = _new((lib.b200sep_dconv_work_floats(B, C_, Fr, L, hid),), x)
                 check(lib.b200sep_dconv_f32(_ptr(x), _ptr(x), _ptr(W[f"{p}.0.weight:raw"]), _ptr(W[f"{p}.0.bias"]), _ptr(W[f"{p}.1.weight"]), _ptr(W[f"{p}.1.bias"]),
                                             _ptr(W[f"{p}.3.weight:raw"]), _ptr(W[f"{p}.3.bias"]), _ptr(W[f"{p}.4.weight"]), _ptr(W[f"{p}.4.bias"]), _ptr(W[f"{p}.6.scale"]),
                                             B, C_, Fr, L, hid, dil, _ptr(u_in) if u_in is not None else None, _ptr(work), _stream()), "dconv_f32")
                 continue
-            h = conv2d(x, W[f"{p}.0.weight"], W[f"{p}.0.bias"], hid, (1, 3), p=(0, dil), dw=dil)
+            h = conv2d(x, W[f"{p}.0.weight"], W[f"{p}.0.bias"], hid, (1, 3), p=(0, dil), dw=dil, math=self.math)
             groupnorm1(h, W[f"{p}.1.weight"], W[f"{p}.1.bias"], ACT_GELU)
-            h = conv2d(h, W[f"{p}.3.weight"], W[f"{p}.3.bias"], 2 * C_, (1, 1))
+            h = conv2d(h, W[f"{p}.3.weight"], W[f"{p}.3.bias"], 2 * C_, (1, 1), math=self.math)
             groupnorm1(h, W[f"{p}.4.weight"], W[f"{p}.4.bias"])
             x = glu(h, res=x, scale=W[f"{p}.6.scale"])
         return x
@@ -322,13 +338,13 @@ class HTDemucsNet:
         W, cfg = self.W, self.cfg
         co = W[f"{prefix}.conv.bias"].numel()
         if freq:
-            y = conv2d(x, W[f"{prefix}.conv.weight"], W[f"{prefix}.conv.bias"], co, (cfg.kernel_size, 1), s=(cfg.stride, 1), p=(cfg.kernel_size // 4, 0), act=ACT_GELU)
+            y = conv2d(x, W[f"{prefix}.conv.weight"], W[f"{prefix}.conv.bias"], co, (cfg.kernel_size, 1), s=(cfg.stride, 1), p=(cfg.kernel_size // 4, 0), act=ACT_GELU, math=self.math)
         else:
             le = x.shape[-1]
             y = conv2d(x, W[f"{prefix}.conv.weight"], W[f"{prefix}.conv.bias"], co, (1, cfg.kernel_size), s=(1, cfg.stride), p=(0, cfg.kernel_size // 4), act=ACT_GELU,
-                       out_hw=(1, -(-le // cfg.stride)))  # F.pad to a multiple of the stride == implicit zero columns on the right
+                       out_hw=(1, -(-le // cfg.stride)), math=self.math)  # F.pad to a multiple of the stride == implicit zero columns on the right
         y = self._dconv(y, prefix)
-        z = conv2d(y, W[f"{prefix}.rewrite.weight"], W[f"{prefix}.rewrite.bias"], 2 * co, (1, 1))
+        z = conv2d(y, W[f"{prefix}.rewrite.weight"], W[f"{prefix}.rewrite.bias"], 2 * co, (1, 1), math=self.math)
         return glu(z)
 
     def _dec(self, x, skip, length, prefix, freq, last):
@@ -337,15 +353,15 @@ class HTDemucsNet:
         ci = x.shape[1]
         x = ew(x, skip, _new(x.shape, x))
         if freq:
-            y = glu(conv2d(x, W[f"{prefix}.rewrite.weight"], W[f"{prefix}.rewrite.bias"], 2 * ci, (3, 3), p=(1, 1)))
+            y = glu(conv2d(x, W[f"{prefix}.rewrite.weight"], W[f"{prefix}.rewrite.bias"], 2 * ci, (3, 3), p=(1, 1), math=self.math))
         else:
-            y = glu(conv2d(x, W[f"{prefix}.rewrite.weight"], W[f"{prefix}.rewrite.bias"], 2 * ci, (1, 3), p=(0, 1)))
+            y = glu(conv2d(x, W[f"{prefix}.rewrite.weight"], W[f"{prefix}.rewrite.bias"], 2 * ci, (1, 3), p=(0, 1), math=self.math))
         y = self._dconv(y, prefix)
         co = W[f"{prefix}.conv_tr.bias"].numel()
         act = ACT_NONE if last else ACT_GELU
         if freq:
-            return conv_transpose(y, W[f"{prefix}.conv_tr.weight"], W[f"{prefix}.conv_tr.bias"], co, 1, cfg.stride, cfg.kernel_size // 4, y.shape[2] * cfg.stride, act)
-        return conv_transpose(y, W[f"{prefix}.conv_tr.weight"], W[f"{prefix}.conv_tr.bias"], co, 2, cfg.stride, cfg.kernel_size // 4, length, act)
+            return conv_transpose(y, W[f"{prefix}.conv_tr.weight"], W[f"{prefix}.conv_tr.bias"], co, 1, cfg.stride, cfg.kernel_size // 4, y.shape[2] * cfg.stride, act, math=self.math)
+        return conv_transpose(y, W[f"{prefix}.conv_tr.weight"], W[f"{prefix}.conv_tr.bias"], co, 2, cfg.stride, cfg.kernel_size // 4, length, act, math=self.math)
 
     def _mha(self, q_in, kv_in, p, res, res_scale):
         """nn.MultiheadAttention(batch_first) + the layer-scaled residual: res + gamma * out_proj(softmax(QK^T/sqrt(hd)) V).  q_in (B,Lq,D), kv_in (B,Lk,D)."""
@@ -354,33 +370,33 @@ class HTDemucsNet:
         Lk = kv_in.shape[1]
         H = self.cfg.t_heads
         hd = D // H
-        q = linear(q_in.view(B * Lq, D), W[f"{p}.q_weight"], W[f"{p}.q_bias"])
-        k = linear(kv_in.view(B * Lk, D), W[f"{p}.k_weight"], W[f"{p}.k_bias"])
+        q = linear(q_in.view(B * Lq, D), W[f"{p}.q_weight"], W[f"{p}.q_bias"], math=self.math)
+        k = linear(kv_in.view(B * Lk, D), W[f"{p}.k_weight"], W[f"{p}.k_bias"], math=self.math)
         # V^T per batch: (D, Lk) = Wv (D,D) @ kv^T, bias per row
         vt = _new((B, D, Lk), q_in)
         wv, bv = W[f"{p}.v_weight"], W[f"{p}.v_bias"]
-        _gemm_raw(_ptr(wv), _ptr(kv_in), _ptr(vt), D, Lk, D, D, D, Lk, B, 0, Lk * D, D * Lk, bias_m=_ptr(bv))
+        _gemm_raw(_ptr(wv), _ptr(kv_in), _ptr(vt), D, Lk, D, D, D, Lk, B, 0, Lk * D, D * Lk, bias_m=_ptr(bv), math=self.math)
         o = _new((B, Lq, D), q_in)
         if hd == 64:  # one kernel, the (H, Lq, Lk) scores stay on chip
-            work = _new((lib.b200sep_attention_work_floats(B, H, Lq, Lk),), q_in)  # bf16 hi / lo tile images of Q, K, V^T (split once, not once per consumer)
-            check(lib.b200sep_attention_f32(_ptr(q), _ptr(k), _ptr(vt), _ptr(o), B, H, Lq, Lk, hd, Lq * D, D, Lk * D, D, D * Lk, Lk, Lq * D, D, 1.0 / math.sqrt(hd),
-                                            0, _ptr(work), _stream()), "attention_f32")
-            y = linear(o.view(B * Lq, D), W[f"{p}.out_proj.weight"], W[f"{p}.out_proj.bias"], res=res.view(B * Lq, D), res_scale=res_scale)
+            work = _new((lib.b200sep_attention_work_floats_math(B, H, Lq, Lk, self.math),), q_in)  # tile images of Q, K, V^T (split once, not once per consumer)
+            check(lib.b200sep_attention_f32_math(_ptr(q), _ptr(k), _ptr(vt), _ptr(o), B, H, Lq, Lk, hd, Lq * D, D, Lk * D, D, D * Lk, Lk, Lq * D, D, 1.0 / math.sqrt(hd),
+                                                 0, _ptr(work), self.math, _stream()), "attention_f32")
+            y = linear(o.view(B * Lq, D), W[f"{p}.out_proj.weight"], W[f"{p}.out_proj.bias"], res=res.view(B * Lq, D), res_scale=res_scale, math=self.math)
             return y.view(B, Lq, D)
         sc = _new((H, Lq, Lk), q_in)
         fs = 4  # bytes per float
         for b in range(B):
-            _gemm_raw(q.data_ptr() + b * Lq * D * fs, k.data_ptr() + b * Lk * D * fs, _ptr(sc), Lq, Lk, hd, D, D, Lk, H, hd, hd, Lq * Lk, alpha=1.0 / math.sqrt(hd))
+            _gemm_raw(q.data_ptr() + b * Lq * D * fs, k.data_ptr() + b * Lk * D * fs, _ptr(sc), Lq, Lk, hd, D, D, Lk, H, hd, hd, Lq * Lk, alpha=1.0 / math.sqrt(hd), math=self.math)
             check(lib.b200sep_softmax_rows_f32(_ptr(sc), H * Lq, Lk, Lk, _stream()), "softmax_rows_f32")
-            _gemm_raw(_ptr(sc), vt.data_ptr() + b * D * Lk * fs, o.data_ptr() + b * Lq * D * fs, Lq, hd, Lk, Lk, Lk, D, H, Lq * Lk, hd * Lk, hd)
-        y = linear(o.view(B * Lq, D), W[f"{p}.out_proj.weight"], W[f"{p}.out_proj.bias"], res=res.view(B * Lq, D), res_scale=res_scale)
+            _gemm_raw(_ptr(sc), vt.data_ptr() + b * D * Lk * fs, o.data_ptr() + b * Lq * D * fs, Lq, hd, Lk, Lk, Lk, D, H, Lq * Lk, hd * Lk, hd, math=self.math)
+        y = linear(o.view(B * Lq, D), W[f"{p}.out_proj.weight"], W[f"{p}.out_proj.bias"], res=res.view(B * Lq, D), res_scale=res_scale, math=self.math)
         return y.view(B, Lq, D)
 
     def _ffn(self, x_norm, x, p):
         W = self.W
         B, L, D = x.shape
-        h = linear(x_norm.view(B * L, D), W[f"{p}.linear1.weight"], W[f"{p}.linear1.bias"], act=ACT_GELU)
-        return linear(h, W[f"{p}.linear2.weight"], W[f"{p}.linear2.bias"], res=x.view(B * L, D), res_scale=W[f"{p}.gamma_2.scale"]).view(B, L, D)
+        h = linear(x_norm.view(B * L, D), W[f"{p}.linear1.weight"], W[f"{p}.linear1.bias"], act=ACT_GELU, math=self.math)
+        return linear(h, W[f"{p}.linear2.weight"], W[f"{p}.linear2.bias"], res=x.view(B * L, D), res_scale=W[f"{p}.gamma_2.scale"], math=self.math).view(B, L, D)
 
     def _self_layer(self, x, p):  # MyTransformerEncoderLayer.forward, norm_first (transformer.py:268-274)
         W = self.W
@@ -409,8 +425,8 @@ class HTDemucsNet:
         B, c0, Fr, T1 = x.shape
         if cfg.bottom_channels:
             D = cfg.bottom_channels
-            x = conv2d(x.view(B, c0, 1, Fr * T1), W["channel_upsampler.weight"], W["channel_upsampler.bias"], D, (1, 1)).view(B, D, Fr, T1)
-            xt = conv2d(xt, W["channel_upsampler_t.weight"], W["channel_upsampler_t.bias"], D, (1, 1))
+            x = conv2d(x.view(B, c0, 1, Fr * T1), W["channel_upsampler.weight"], W["channel_upsampler.bias"], D, (1, 1), math=self.math).view(B, D, Fr, T1)
+            xt = conv2d(xt, W["channel_upsampler_t.weight"], W["channel_upsampler_t.bias"], D, (1, 1), math=self.math)
         D = x.shape[1]
         T2 = xt.shape[-1]
         xs = _new((B, T1, Fr, D), x)  # "b c fr t1 -> b (t1 fr) c"
@@ -439,8 +455,8 @@ class HTDemucsNet:
         xt = _new((B, D, 1, T2), xs)
         check(lib.b200sep_permute4_f32(_ptr(xts), _ptr(xt), B, T2, 1, D, 0, 3, 2, 1, _stream()), "permute4_f32")
         if cfg.bottom_channels:
-            x = conv2d(x.view(B, D, 1, Fr * T1), W["channel_downsampler.weight"], W["channel_downsampler.bias"], c0, (1, 1)).view(B, c0, Fr, T1)
-            xt = conv2d(xt, W["channel_downsampler_t.weight"], W["channel_downsampler_t.bias"], c0, (1, 1))
+            x = conv2d(x.view(B, D, 1, Fr * T1), W["channel_downsampler.weight"], W["channel_downsampler.bias"], c0, (1, 1), math=self.math).view(B, c0, Fr, T1)
+            xt = conv2d(xt, W["channel_downsampler_t.weight"], W["channel_downsampler_t.bias"], c0, (1, 1), math=self.math)
         return x, xt
 
     # ---- forward ---------------------------------------------------------------------------------------------------

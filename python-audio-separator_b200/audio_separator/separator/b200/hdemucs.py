@@ -16,7 +16,7 @@ from dataclasses import dataclass
 import numpy as np
 import torch
 
-from ._lib import LAYOUT_CFT, check, lib
+from ._lib import LAYOUT_CFT, MATH_BF16X3, check, lib
 from .demucs import (ACT_GELU, ACT_NONE, HTDemucsNet, _gemm_raw, _new, block_conv_weight, block_convtr_weight, conv2d, conv_transpose, ew, glu, groupnorm1, linear)
 from .engine import StftPlan, _ptr, _require_cuda, _stream
 
@@ -119,10 +119,11 @@ def groupnorm(x, groups, gamma, beta, act=ACT_NONE):
 class HDemucsNet(HTDemucsNet):
     """Device-resident HDemucs weights + the launch sequence of one forward.  (Sub-classes HTDemucsNet for its plain DConv branch.)"""
 
-    def __init__(self, cfg: HDemucsConfig, state: dict, device=None):  # noqa: super().__init__ builds the HTDemucs graph; this class has its own
+    def __init__(self, cfg: HDemucsConfig, state: dict, device=None, math=MATH_BF16X3):  # noqa: super().__init__ builds the HTDemucs graph; this class has its own
         _require_cuda()
         cfg.validate()
         self.cfg = cfg
+        self.math = int(math)  # as HTDemucsNet
         self.device = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
         self.S = len(cfg.sources)
         self.stft = StftPlan(cfg.nfft, cfg.hop)
@@ -216,14 +217,14 @@ class HDemucsNet(HTDemucsNet):
             xp = _new((2, width * N, 4 * C), h)
             for d in range(2):
                 wih = W[f"{p}.lstm.wih{layer}{d}"]
-                _gemm_raw(_ptr(x2), _ptr(wih), xp[d].data_ptr(), width * N, 4 * C, K, K, K, 4 * C, 1, 0, 0, 0, bias_n=_ptr(W[f"{p}.lstm.b{layer}{d}"]))
+                _gemm_raw(_ptr(x2), _ptr(wih), xp[d].data_ptr(), width * N, 4 * C, K, K, K, 4 * C, 1, 0, 0, 0, bias_n=_ptr(W[f"{p}.lstm.b{layer}{d}"]), math=self.math)
             out = _new((width, N, 2 * C), h)
             if C <= 96:
                 check(lib.b200sep_lstm_bidir_f32(_ptr(xp), _ptr(W[f"{p}.lstm.whh{layer}"]), _ptr(out), width, N, C, _stream()), "lstm_bidir_f32")
             else:
                 check(lib.b200sep_lstm_bidir_wide_f32(_ptr(xp), _ptr(W[f"{p}.lstm.whh_t{layer}"]), _ptr(out), width, N, C, _stream()), "lstm_bidir_wide_f32")
             x2 = out.view(width * N, 2 * C)
-        lin = linear(x2, W[f"{p}.linear.weight"], W[f"{p}.linear.bias"])
+        lin = linear(x2, W[f"{p}.linear.weight"], W[f"{p}.linear.bias"], math=self.math)
         y = _new(h.shape, h)
         check(lib.b200sep_lstm_frames_scatter_f32(_ptr(lin), _ptr(h), _ptr(y), B, C, T, nf, width, stride if nf > 1 else 2, _stream()), "lstm_frames_scatter_f32")
         return y
@@ -232,14 +233,14 @@ class HDemucsNet(HTDemucsNet):
         """LocalState(hidden, heads=4, ndecay=4).forward (demucs.py:197-231) on h (B, C, 1, T)."""
         W, cfg = self.W, self.cfg
         B, C, _, T = h.shape
-        q = conv2d(h, W[f"{p}.query.weight"], W[f"{p}.query.bias"], C, (1, 1))
-        k = conv2d(h, W[f"{p}.key.weight"], W[f"{p}.key.bias"], C, (1, 1))
-        ct = conv2d(h, W[f"{p}.content.weight"], W[f"{p}.content.bias"], C, (1, 1))
+        q = conv2d(h, W[f"{p}.query.weight"], W[f"{p}.query.bias"], C, (1, 1), math=self.math)
+        k = conv2d(h, W[f"{p}.key.weight"], W[f"{p}.key.bias"], C, (1, 1), math=self.math)
+        ct = conv2d(h, W[f"{p}.content.weight"], W[f"{p}.content.bias"], C, (1, 1), math=self.math)
         nd = cfg.attn_heads * cfg.attn_ndecay
-        dq = conv2d(h, W[f"{p}.query_decay.weight"], W[f"{p}.query_decay.bias"], nd, (1, 1))
+        dq = conv2d(h, W[f"{p}.query_decay.weight"], W[f"{p}.query_decay.bias"], nd, (1, 1), math=self.math)
         res = _new(h.shape, h)
         check(lib.b200sep_local_state_attn_f32(_ptr(q), _ptr(k), _ptr(ct), _ptr(dq), _ptr(res), B, C, T, cfg.attn_heads, cfg.attn_ndecay, _stream()), "local_state_attn_f32")
-        return conv2d(res, W[f"{p}.proj.weight"], W[f"{p}.proj.bias"], C, (1, 1), add=h)
+        return conv2d(res, W[f"{p}.proj.weight"], W[f"{p}.proj.bias"], C, (1, 1), add=h, math=self.math)
 
     def _dconv_layer(self, x, prefix, L):
         """DConv.forward (demucs.py:166-168) for the layer kinds of this model: the plain branch of HTDemucsNet, or conv -> GroupNorm+GELU ->
@@ -254,7 +255,7 @@ class HDemucsNet(HTDemucsNet):
             p = f"{prefix}.dconv.layers.{d}"
             dil = 2**d
             hid = W[f"{p}.0.bias"].numel()
-            h = conv2d(x, W[f"{p}.0.weight"], W[f"{p}.0.bias"], hid, (1, 3), p=(0, dil), dw=dil)
+            h = conv2d(x, W[f"{p}.0.weight"], W[f"{p}.0.bias"], hid, (1, 3), p=(0, dil), dw=dil, math=self.math)
             groupnorm1(h, W[f"{p}.1.weight"], W[f"{p}.1.bias"], ACT_GELU)
             i = 3
             if L["lstm"]:
@@ -263,7 +264,7 @@ class HDemucsNet(HTDemucsNet):
             if L["attn"]:
                 h = self._local_state(h, f"{p}.{i}")
                 i += 1
-            h = conv2d(h, W[f"{p}.{i}.weight"], W[f"{p}.{i}.bias"], 2 * C_, (1, 1))
+            h = conv2d(h, W[f"{p}.{i}.weight"], W[f"{p}.{i}.bias"], 2 * C_, (1, 1), math=self.math)
             groupnorm1(h, W[f"{p}.{i + 1}.weight"], W[f"{p}.{i + 1}.bias"])
             x = glu(h, res=x, scale=W[f"{p}.{i + 3}.scale"])
         return x
@@ -275,13 +276,13 @@ class HDemucsNet(HTDemucsNet):
         co, k, s, pad = L["chout"], L["k"], L["s"], L["pad"]
         fused_act = ACT_NONE if (L["empty"] or L["norm"]) else ACT_GELU
         if L["freq"]:
-            y = conv2d(x, W[f"{prefix}.conv.weight"], W[f"{prefix}.conv.bias"], co, (k, 1), s=(s, 1), p=(pad, 0), act=fused_act, add=inject, add_before_act=inject is not None)
+            y = conv2d(x, W[f"{prefix}.conv.weight"], W[f"{prefix}.conv.bias"], co, (k, 1), s=(s, 1), p=(pad, 0), act=fused_act, add=inject, add_before_act=inject is not None, math=self.math)
         else:
             if x.shape[2] != 1:
                 raise ValueError(f"{prefix}: a time layer needs one frequency row, got {tuple(x.shape)}")
             le = x.shape[-1]  # F.pad to a multiple of the stride == implicit zero columns on the right
             y = conv2d(x, W[f"{prefix}.conv.weight"], W[f"{prefix}.conv.bias"], co, (1, k), s=(1, s), p=(0, pad), act=fused_act, add=inject, add_before_act=inject is not None,
-                       out_hw=(1, -(-le // s)))
+                       out_hw=(1, -(-le // s)), math=self.math)
         if L["empty"]:
             return y
         if L["norm"]:
@@ -291,9 +292,9 @@ class HDemucsNet(HTDemucsNet):
         ctx = L["context"]
         kk = 1 + 2 * ctx
         if L["freq"]:
-            z = conv2d(y, W[f"{prefix}.rewrite.weight"], W[f"{prefix}.rewrite.bias"], 2 * co, (kk, kk), p=(ctx, ctx))
+            z = conv2d(y, W[f"{prefix}.rewrite.weight"], W[f"{prefix}.rewrite.bias"], 2 * co, (kk, kk), p=(ctx, ctx), math=self.math)
         else:
-            z = conv2d(y, W[f"{prefix}.rewrite.weight"], W[f"{prefix}.rewrite.bias"], 2 * co, (1, kk), p=(0, ctx))
+            z = conv2d(y, W[f"{prefix}.rewrite.weight"], W[f"{prefix}.rewrite.bias"], 2 * co, (1, kk), p=(0, ctx), math=self.math)
         if L["norm"]:
             groupnorm(z, G, W[f"{prefix}.norm2.weight"], W[f"{prefix}.norm2.bias"])
         return glu(z)
@@ -307,9 +308,9 @@ class HDemucsNet(HTDemucsNet):
             ctx = L["context"]
             kk = 1 + 2 * ctx
             if L["freq"]:
-                y = conv2d(x, W[f"{prefix}.rewrite.weight"], W[f"{prefix}.rewrite.bias"], 2 * ci, (kk, kk), p=(ctx, ctx))
+                y = conv2d(x, W[f"{prefix}.rewrite.weight"], W[f"{prefix}.rewrite.bias"], 2 * ci, (kk, kk), p=(ctx, ctx), math=self.math)
             else:
-                y = conv2d(x, W[f"{prefix}.rewrite.weight"], W[f"{prefix}.rewrite.bias"], 2 * ci, (1, kk), p=(0, ctx))
+                y = conv2d(x, W[f"{prefix}.rewrite.weight"], W[f"{prefix}.rewrite.bias"], 2 * ci, (1, kk), p=(0, ctx), math=self.math)
             if L["norm"]:
                 groupnorm(y, G, W[f"{prefix}.norm1.weight"], W[f"{prefix}.norm1.bias"])
             y = glu(y)
@@ -324,9 +325,9 @@ class HDemucsNet(HTDemucsNet):
         target = full - 2 * pad if L["freq"] else length
         wt, bt = W[f"{prefix}.conv_tr.weight"], W[f"{prefix}.conv_tr.bias"]
         if not L["norm"]:
-            return conv_transpose(y, wt, bt, co, axis, s, pad, target, act), y
+            return conv_transpose(y, wt, bt, co, axis, s, pad, target, act, math=self.math), y
         # GroupNorm sees the UNtrimmed transposed convolution (hdemucs.py:322-328: norm2, then the crop, then GELU)
-        z = conv_transpose(y, wt, bt, co, axis, s, 0, full, ACT_NONE)
+        z = conv_transpose(y, wt, bt, co, axis, s, 0, full, ACT_NONE, math=self.math)
         groupnorm(z, G, W[f"{prefix}.norm2.weight"], W[f"{prefix}.norm2.bias"], act)
         if target != full:
             z = (z[:, :, pad : pad + target, :] if L["freq"] else z[:, :, :, pad : pad + target]).contiguous()  # a strided device copy

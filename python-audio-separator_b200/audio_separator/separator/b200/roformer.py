@@ -16,7 +16,7 @@ from dataclasses import dataclass, field
 import numpy as np
 import torch
 
-from ._lib import LAYOUT_CFT, check, lib
+from ._lib import LAYOUT_CFT, MATH_BF16X3, check, lib
 from .demucs import ACT_GELU, ACT_NONE, _new, _packed_linear
 from .engine import StftPlan, _ptr, _require_cuda, _stream
 
@@ -149,12 +149,12 @@ def mel_band_layout(cfg: "MelBandRoformerConfig"):
     return mask, idx.astype(np.int64), mask.sum(1), mask.sum(0)
 
 
-def gemm(a_ptr, w, c_ptr, M, lda, ldc, bias=None, act=ACT_NONE, res_ptr=None):
+def gemm(a_ptr, w, c_ptr, M, lda, ldc, bias=None, act=ACT_NONE, res_ptr=None, math=MATH_BF16X3):
     """rows x K (row stride lda) @ w (N, K)^T + bias -> rows x N at row stride ldc (+ res with the same strides)."""
     N, K = w.shape
-    pk = _packed_linear(w)
-    check(lib.b200sep_gemm_f32(a_ptr, _ptr(w), c_ptr, M, N, K, lda, K, ldc, 1, 0, 0, 0, 1.0, _ptr(bias) if bias is not None else None, None, act, res_ptr, None,
-                               _ptr(pk) if pk is not None else None, _stream()), "gemm_f32")
+    pk = _packed_linear(w, math)
+    check(lib.b200sep_gemm_f32_math(a_ptr, _ptr(w), c_ptr, M, N, K, lda, K, ldc, 1, 0, 0, 0, 1.0, _ptr(bias) if bias is not None else None, None, act, res_ptr, None,
+                                    _ptr(pk) if pk is not None else None, math, _stream()), "gemm_f32")
 
 
 def rmsnorm(x, gamma, rows, C, ld_in=None, out=None):
@@ -167,9 +167,11 @@ class BSRoformerNet:
     """BS-Roformer (cfg: BSRoformerConfig) or Mel-Band Roformer (cfg: MelBandRoformerConfig): the graphs differ only in the band layout (disjoint
     slices vs gathered, overlapping mel bands whose masks are averaged), the per-transformer output norm and the mask MLP depth."""
 
-    def __init__(self, cfg, state: dict, device=None):
+    def __init__(self, cfg, state: dict, device=None, math=MATH_BF16X3):
+        """math: MATH_BF16X3 (default, ~fp32) or MATH_FP16 (torch.autocast precision) for every tensor-core GEMM and attention of this net."""
         _require_cuda()
         self.cfg = cfg
+        self.math = int(math)
         self.device = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())  # one process per GPU: the rank's own device
         if not cfg.stereo:
             raise NotImplementedError("mono BS-Roformer checkpoints are not covered (the STFT kernels process stereo pairs)")
@@ -211,32 +213,32 @@ class BSRoformerNet:
             a, f = f"{p}.layers.{l}.0", f"{p}.layers.{l}.1"
             xn = rmsnorm(x, W[f"{a}.norm.gamma"], rows, d)
             qkv = _new((rows, 3 * inner), x)
-            gemm(_ptr(xn), W[f"{a}.to_qkv.weight"], _ptr(qkv), rows, d, 3 * inner)
+            gemm(_ptr(xn), W[f"{a}.to_qkv.weight"], _ptr(qkv), rows, d, 3 * inner, math=self.math)
             q, k, v = _new((Bq, H, n, dh), x), _new((Bq, H, n, dh), x), _new((Bq, H, n, dh), x)
             check(lib.b200sep_rope_split_heads_f32(_ptr(qkv), _ptr(W[f"{a}.rotary_embed.freqs"]), _ptr(q), _ptr(k), _ptr(v), Bq, n, H, dh, _stream()), "rope_split_heads_f32")
             o = _new((Bq, H, n, dh), x)
             if dh == 64:  # scores stay on chip (b200sep_attention_f32): every (batch, head) pair is one batch entry of the kernel, V untransposed
-                work = _new((lib.b200sep_attention_work_floats(Bq * H, 1, n, n),), x)
-                check(lib.b200sep_attention_f32(_ptr(q), _ptr(k), _ptr(v), _ptr(o), Bq * H, 1, n, n, dh, n * dh, dh, n * dh, dh, n * dh, dh, n * dh, dh, dh**-0.5, 1,
-                                                _ptr(work), _stream()), "attention_f32")
+                work = _new((lib.b200sep_attention_work_floats_math(Bq * H, 1, n, n, self.math),), x)
+                check(lib.b200sep_attention_f32_math(_ptr(q), _ptr(k), _ptr(v), _ptr(o), Bq * H, 1, n, n, dh, n * dh, dh, n * dh, dh, n * dh, dh, n * dh, dh, dh**-0.5,
+                                                     1, _ptr(work), self.math, _stream()), "attention_f32")
             else:
                 sc = _new((Bq * H, n, ldv), x)  # padding columns n..ldv-1 are never read: the P@V GEMM runs K = n over rows of stride ldv
-                check(lib.b200sep_gemm_f32(_ptr(q), _ptr(k), _ptr(sc), n, n, dh, dh, dh, ldv, Bq * H, n * dh, n * dh, n * ldv, dh**-0.5, None, None, 0, None, None, None,
-                                           _stream()), "gemm_f32(scores)")
+                check(lib.b200sep_gemm_f32_math(_ptr(q), _ptr(k), _ptr(sc), n, n, dh, dh, dh, ldv, Bq * H, n * dh, n * dh, n * ldv, dh**-0.5, None, None, 0, None, None,
+                                                None, self.math, _stream()), "gemm_f32(scores)")
                 check(lib.b200sep_softmax_rows_f32(_ptr(sc), Bq * H * n, n, ldv, _stream()), "softmax_rows_f32")
                 check(lib.b200sep_gemm_kn_f32(_ptr(sc), _ptr(v), _ptr(o), n, dh, n, ldv, dh, dh, Bq * H, n * ldv, n * dh, n * dh, 1.0, _stream()), "gemm_kn_f32(PV)")
             gates = _new((rows, H), x)
-            gemm(_ptr(xn), W[f"{a}.to_gates.weight"], _ptr(gates), rows, d, H, bias=W[f"{a}.to_gates.bias"])
+            gemm(_ptr(xn), W[f"{a}.to_gates.weight"], _ptr(gates), rows, d, H, bias=W[f"{a}.to_gates.bias"], math=self.math)
             merged = _new((rows, inner), x)
             check(lib.b200sep_gate_merge_heads_f32(_ptr(o), _ptr(gates), _ptr(merged), Bq, n, H, dh, _stream()), "gate_merge_heads_f32")
             x2 = _new((rows, d), x)
-            gemm(_ptr(merged), W[f"{a}.to_out.0.weight"], _ptr(x2), rows, inner, d, res_ptr=_ptr(x))  # attn(x) + x
+            gemm(_ptr(merged), W[f"{a}.to_out.0.weight"], _ptr(x2), rows, inner, d, res_ptr=_ptr(x), math=self.math)  # attn(x) + x
             hn = rmsnorm(x2, W[f"{f}.net.0.gamma"], rows, d)
             hid = W[f"{f}.net.1.bias"].numel()
             h = _new((rows, hid), x)
-            gemm(_ptr(hn), W[f"{f}.net.1.weight"], _ptr(h), rows, d, hid, bias=W[f"{f}.net.1.bias"], act=ACT_GELU)
+            gemm(_ptr(hn), W[f"{f}.net.1.weight"], _ptr(h), rows, d, hid, bias=W[f"{f}.net.1.bias"], act=ACT_GELU, math=self.math)
             x = _new((rows, d), x)
-            gemm(_ptr(h), W[f"{f}.net.4.weight"], _ptr(x), rows, hid, d, bias=W[f"{f}.net.4.bias"], res_ptr=_ptr(x2))  # ff(x) + x
+            gemm(_ptr(h), W[f"{f}.net.4.weight"], _ptr(x), rows, hid, d, bias=W[f"{f}.net.4.bias"], res_ptr=_ptr(x2), math=self.math)  # ff(x) + x
         if f"{p}.norm.gamma" in W:  # Transformer(norm_output=True): the Mel-Band variant (mel_band_roformer.py:82-101)
             x = rmsnorm(x, W[f"{p}.norm.gamma"], rows, d)
         return x
@@ -263,7 +265,7 @@ class BSRoformerNet:
         off = 0
         for bi, d_in in enumerate(self.band_dims):  # BandSplit (bs_roformer.py:134-150)
             xn = rmsnorm(src.data_ptr() + off * 4, W[f"band_split.to_features.{bi}.0.gamma"], rows, d_in, ld_in=nfeat, out=_new((rows, d_in), spec))
-            gemm(_ptr(xn), W[f"band_split.to_features.{bi}.1.weight"], x.data_ptr() + bi * d * 4, rows, d_in, nb * d, bias=W[f"band_split.to_features.{bi}.1.bias"])
+            gemm(_ptr(xn), W[f"band_split.to_features.{bi}.1.weight"], x.data_ptr() + bi * d * 4, rows, d_in, nb * d, bias=W[f"band_split.to_features.{bi}.1.bias"], math=self.math)
             off += d_in
         for i in range(cfg.depth):
             xt = _new((b, nb, T, d), x)  # "b t f d -> (b f) t d"
@@ -283,7 +285,7 @@ class BSRoformerNet:
                     w = W[f"{p}.weight"]
                     last = li == self.n_mask_linear - 1
                     y = _new((rows, w.shape[0]), spec)
-                    gemm(h_ptr, w, _ptr(y), rows, lda, w.shape[0], bias=W[f"{p}.bias"], act=ACT_NONE if last else ACT_TANH)
+                    gemm(h_ptr, w, _ptr(y), rows, lda, w.shape[0], bias=W[f"{p}.bias"], act=ACT_NONE if last else ACT_TANH, math=self.math)
                     hold = y  # keeps the buffer alive while its raw pointer is in use
                     h_ptr, lda = _ptr(y), w.shape[0]
                 for bb in range(b):  # the mask tensor is (b, S, T, features): one row block per batch element

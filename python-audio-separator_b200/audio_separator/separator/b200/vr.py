@@ -16,7 +16,7 @@ import math
 import numpy as np
 import torch
 
-from ._lib import LAYOUT_CFT, check, lib
+from ._lib import LAYOUT_CFT, MATH_BF16X3, check, lib
 from .demucs import ACT_NONE, ACT_RELU, _new, block_conv_weight, conv2d, ew, linear
 from .engine import StftPlan, _ptr, _require_cuda, _stream
 
@@ -130,8 +130,10 @@ def capacity(nn_architecture: int):
 class VRNet:
     """CascadedASPPNet in eval mode: BatchNorm folded into the preceding (bias-free) convolution, Dropout = identity."""
 
-    def __init__(self, nn_architecture: int, n_fft_bins: int, state: dict, device=None):
+    def __init__(self, nn_architecture: int, n_fft_bins: int, state: dict, device=None, math=MATH_BF16X3):
+        """math: MATH_BF16X3 (default, ~fp32) or MATH_FP16 (torch.autocast precision) for every tensor-core convolution / GEMM of this net."""
         _require_cuda()
+        self.math = int(math)
         self.arch = int(nn_architecture)
         self.c1, self.cb, self.c2, self.c3 = capacity(self.arch)
         self.n_enc = 5 if self.arch == 129605 else 4
@@ -176,7 +178,8 @@ class VRNet:
         k = self.W[p + ".k"]
         cout = self.W[p + ".b"].numel()
         pad = (dil[0] * (k // 2), dil[1] * (k // 2))  # Conv2DBNActiv(..., pad=dilation, dilation=dilation) in the ASPP modules
-        return conv2d(x, self.W[p + ".w"], self.W[p + ".b"], cout, (k, k), s=(stride, stride), p=pad, dw=dil[1], dh=dil[0], act=act, out=out, out_c_off=out_c_off)
+        return conv2d(x, self.W[p + ".w"], self.W[p + ".b"], cout, (k, k), s=(stride, stride), p=pad, dw=dil[1], dh=dil[0], act=act, out=out, out_c_off=out_c_off,
+                      math=self.math)
 
     def _sep(self, x, p, dil, out, out_c_off):
         B, C, H, W = x.shape
@@ -239,7 +242,7 @@ class VRNet:
         self_aux2 = self._base(self._cba(h1, "stg2_bridge"), "stg2_full_band_net")
         copy_view(self_aux2, h2[:, 2 + c1 :])
         h = self._base(self._cba(h2, "stg3_bridge"), "stg3_full_band_net")
-        m = conv2d(h, self.W["out.w"], None, 2, (1, 1), act=ACT_SIGMOID)
+        m = conv2d(h, self.W["out.w"], None, 2, (1, 1), act=ACT_SIGMOID, math=self.math)
         mask = _new((B, 2, self.output_bin, Wd), x)
         copy_view(m, mask[:, :, :mb])
         copy_view(m[:, :, mb - 1 : mb].expand(B, 2, self.output_bin - mb, Wd), mask[:, :, mb:])  # F.pad(mode="replicate") on the bin axis
@@ -259,8 +262,9 @@ class VRNet51(VRNet):
     """CascadedNet of VR 5.1 (vr_network/nets_new.py:52-160, layers_new.py): five band nets with stride-2 encoders, an ASPP of dilated 3x3 convolutions
     (dilations (4,2), (8,4), (12,6)) and a bidirectional-LSTM branch over the time axis in front of the last decoder; eval mode (BatchNorm folded)."""
 
-    def __init__(self, n_fft_bins: int, nout: int, nout_lstm: int, state: dict, nn_arch_size: int = 56817, device=None):
+    def __init__(self, n_fft_bins: int, nout: int, nout_lstm: int, state: dict, nn_arch_size: int = 56817, device=None, math=MATH_BF16X3):
         _require_cuda()
+        self.math = int(math)  # as VRNet
         self.arch = int(nn_arch_size)
         self.nout = 64 if self.arch == 218409 else int(nout)
         self.max_bin, self.output_bin, self.offset = n_fft_bins // 2, n_fft_bins // 2 + 1, 64
@@ -324,11 +328,11 @@ class VRNet51(VRNet):
         hid = W[f"{p}.whh"].shape[2]
         xp = _new((2, nf * N, 4 * hid), x)
         for d in range(2):
-            check(lib.b200sep_gemm_f32(_ptr(seq), _ptr(W[f"{p}.wih{d}"]), xp.data_ptr() + d * nf * N * 4 * hid * 4, nf * N, 4 * hid, nb, nb, nb, 4 * hid, 1, 0, 0, 0, 1.0,
-                                       _ptr(W[f"{p}.bih{d}"]), None, 0, None, None, None, _stream()), "gemm_f32(lstm input projection)")
+            check(lib.b200sep_gemm_f32_math(_ptr(seq), _ptr(W[f"{p}.wih{d}"]), xp.data_ptr() + d * nf * N * 4 * hid * 4, nf * N, 4 * hid, nb, nb, nb, 4 * hid, 1, 0, 0, 0,
+                                            1.0, _ptr(W[f"{p}.bih{d}"]), None, 0, None, None, None, self.math, _stream()), "gemm_f32(lstm input projection)")
         hs = _new((nf * N, 2 * hid), x)
         check(lib.b200sep_lstm_bidir_f32(_ptr(xp), _ptr(W[f"{p}.whh"]), _ptr(hs), nf, N, hid, _stream()), "lstm_bidir_f32")
-        dn = linear(hs, W[f"{p}.dense.w"], W[f"{p}.dense.b"], act=ACT_RELU)  # Linear + BatchNorm1d (folded) + ReLU: (frames*N, bins)
+        dn = linear(hs, W[f"{p}.dense.w"], W[f"{p}.dense.b"], act=ACT_RELU, math=self.math)  # Linear + BatchNorm1d (folded) + ReLU: (frames*N, bins)
         copy_view(dn.view(nf, N, nb, 1).permute(1, 3, 2, 0), out[:, out_c_off : out_c_off + 1])
 
     def _base51(self, x, p):
@@ -372,7 +376,7 @@ class VRNet51(VRNet):
         copy_view(l1, f3_in[:, 2 : 2 + c4, :bw]); copy_view(h1, f3_in[:, 2 : 2 + c4, bw:])
         copy_view(l2, f3_in[:, 2 + c4 :, :bw]); copy_view(h2, f3_in[:, 2 + c4 :, bw:])
         f3 = self._base51(f3_in, "stg3_full_band_net")
-        m = conv2d(f3, self.W["out.w"], None, 2, (1, 1), act=ACT_SIGMOID)
+        m = conv2d(f3, self.W["out.w"], None, 2, (1, 1), act=ACT_SIGMOID, math=self.math)
         mask = _new((B, 2, self.output_bin, Wd), x)
         copy_view(m, mask[:, :, :mb])
         copy_view(m[:, :, mb - 1 : mb].expand(B, 2, self.output_bin - mb, Wd), mask[:, :, mb:])

@@ -27,6 +27,19 @@ def normalize(wave, max_peak=1.0, min_peak=None):
     return wave
 
 
+# Architectures whose PyTorch linears, convolutions and attention products torch.autocast("cuda") runs in fp16 in the reference (use_autocast=True):
+# here their tensor-core launches take the same precision (B200SEP_MATH_FP16).  MDX-Net runs in ONNX Runtime in the reference, which autocast does
+# not touch, so it keeps full precision; MDX23C does too, because its pair-format kernels have no fp16 activation storage format yet.
+AUTOCAST_FP16_ARCHS = ("Demucs", "VR", "Roformer")
+
+
+def tensor_core_math(arch: str, use_autocast) -> int:
+    """The math mode (b200._lib.MATH_*) of the tensor-core launches of architecture `arch` ("MDX", "MDX23C", "Demucs", "VR", "Roformer")."""
+    from .b200._lib import MATH_BF16X3, MATH_FP16
+
+    return MATH_FP16 if use_autocast and arch in AUTOCAST_FP16_ARCHS else MATH_BF16X3
+
+
 class DeviceStem:
     """A float stem that lives in HBM.  `primary_source` / `secondary_source` of a plugin hold these after separate(); np.asarray(stem) downloads it
     (once) for code that expects the reference's host arrays, while write_audio consumes the tensor directly."""
@@ -53,7 +66,7 @@ class CommonSeparator:
     _CONFIG_KEYS = (
         "logger", "log_level", "torch_device", "torch_device_cpu", "torch_device_mps", "onnx_execution_provider", "model_name", "model_path",
         "model_data", "output_dir", "output_format", "output_bitrate", "normalization_threshold", "amplification_threshold", "enable_denoise",
-        "output_single_stem", "invert_using_spec", "sample_rate", "use_soundfile",
+        "output_single_stem", "invert_using_spec", "sample_rate", "use_soundfile", "use_autocast",
     )
 
     def __init__(self, config):

@@ -130,7 +130,7 @@ class Separator:
             "output_format": self.output_format, "output_bitrate": self.output_bitrate, "output_dir": self.output_dir,
             "normalization_threshold": self.normalization_threshold, "amplification_threshold": self.amplification_threshold,
             "output_single_stem": self.output_single_stem, "invert_using_spec": self.invert_using_spec, "sample_rate": self.sample_rate,
-            "use_soundfile": self.use_soundfile,
+            "use_soundfile": self.use_soundfile, "use_autocast": self.use_autocast,
         }
         module_name, class_name = classes[model_type].split(".")
         module = importlib.import_module(f"{__package__}.architectures.{module_name}")

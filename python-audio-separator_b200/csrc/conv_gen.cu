@@ -225,10 +225,13 @@ static int launch_gen(const ConvGenParams& p, cudaStream_t st) {
 
 using namespace b200sep;
 
-extern "C" int b200sep_conv2d_f32(const float* x, const float* w_blocked, const float* bias, const float* add, float* y, int B, int Cin, int H, int W, int Cout,
-                                  int Ho, int Wo, int KH, int KW, int SH, int SW, int PH, int PW, int DH, int DW, int act, int add_before_act, int up_axis, int up,
-                                  int trim, int out_len, int out_c_total, int out_c_off, const void* w_packed, void* stream) {
+// math selects the tensor-core arithmetic (B200SEP_MATH_*); the SIMT kernels below are fp32 in every mode
+extern "C" int b200sep_conv2d_f32_math(const float* x, const float* w_blocked, const float* bias, const float* add, float* y, int B, int Cin, int H, int W, int Cout,
+                                       int Ho, int Wo, int KH, int KW, int SH, int SW, int PH, int PW, int DH, int DW, int act, int add_before_act, int up_axis, int up,
+                                       int trim, int out_len, int out_c_total, int out_c_off, const void* w_packed, int math, void* stream) {
   B2_CHECK_ARG(x && w_blocked && y && B >= 1 && Cin >= 1 && Cout >= 1 && Ho >= 1 && Wo >= 1, "conv2d_f32: bad argument");
+  B2_CHECK_ARG(math == B200SEP_MATH_BF16X3 || math == B200SEP_MATH_FP16, "conv2d_f32: unknown math mode %d", math);
+  B2_CHECK_ARG(w_packed == nullptr || tc_packed_matches(w_packed, math), "conv2d_f32: w_packed was packed for the other math mode (asked for %d)", math);
   B2_CHECK_ARG(out_c_total == 0 || (up_axis == 0 && out_c_off >= 0 && out_c_off + Cout <= out_c_total), "conv2d_f32: bad output channel slice [%d, %d) of %d",
                out_c_off, out_c_off + Cout, out_c_total);
   ConvGenParams p;
@@ -241,7 +244,7 @@ extern "C" int b200sep_conv2d_f32(const float* x, const float* w_blocked, const 
   cudaStream_t st = (cudaStream_t)stream;
   if (tc_conv_usable(Cin, Cout, KH, KW, Ho, Wo, B) && (up_axis == 0 || (p.CoutReal % 16 == 0 && add == nullptr)))
     return tc_conv2d_f32(x, w_blocked, bias, add, y, B, Cin, H, W, Cout, p.CoutPad, Ho, Wo, KH, KW, SH, SW, PH, PW, DH, DW, act, add_before_act, out_c_total, out_c_off, w_packed,
-                         st, up_axis, up, trim, out_len);
+                         math, st, up_axis, up, trim, out_len);
 #define B2_CONV_CASE(kh, kw, sh, sw, dw) \
   if (DH == 1 && KH == kh && KW == kw && SH == sh && SW == sw && DW == dw) return launch_gen<kh, kw, sh, sw, dw>(p, st);
   B2_CONV_CASE(1, 1, 1, 1, 1)
@@ -260,4 +263,11 @@ extern "C" int b200sep_conv2d_f32(const float* x, const float* w_blocked, const 
   conv_direct_kernel<<<(int)std::min<int64_t>(cdiv(total, 256), kNumSMs * 16), 256, 0, st>>>(p, KH, KW, SH, SW, DH, DW, total);
   B2_LAUNCHED();
   return B200SEP_OK;
+}
+
+extern "C" int b200sep_conv2d_f32(const float* x, const float* w_blocked, const float* bias, const float* add, float* y, int B, int Cin, int H, int W, int Cout,
+                                  int Ho, int Wo, int KH, int KW, int SH, int SW, int PH, int PW, int DH, int DW, int act, int add_before_act, int up_axis, int up,
+                                  int trim, int out_len, int out_c_total, int out_c_off, const void* w_packed, void* stream) {
+  return b200sep_conv2d_f32_math(x, w_blocked, bias, add, y, B, Cin, H, W, Cout, Ho, Wo, KH, KW, SH, SW, PH, PW, DH, DW, act, add_before_act, up_axis, up, trim, out_len,
+                                 out_c_total, out_c_off, w_packed, B200SEP_MATH_BF16X3, stream);
 }

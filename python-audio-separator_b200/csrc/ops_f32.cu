@@ -617,13 +617,16 @@ extern "C" int b200sep_layernorm_f32(const float* x, const float* gamma, const f
   return B200SEP_OK;
 }
 
-extern "C" int b200sep_gemm_f32(const float* A, const float* Bw, float* C, int M, int N, int K, int lda, int ldb, int ldc, int batch, int64_t strideA,
-                                int64_t strideB, int64_t strideC, float alpha, const float* bias_n, const float* bias_m, int act, const float* res,
-                                const float* res_scale, const void* w_packed, void* stream) {
+// math selects the tensor-core arithmetic (B200SEP_MATH_*); the SIMT kernels below are fp32 in every mode
+extern "C" int b200sep_gemm_f32_math(const float* A, const float* Bw, float* C, int M, int N, int K, int lda, int ldb, int ldc, int batch, int64_t strideA,
+                                     int64_t strideB, int64_t strideC, float alpha, const float* bias_n, const float* bias_m, int act, const float* res,
+                                     const float* res_scale, const void* w_packed, int math, void* stream) {
   B2_CHECK_ARG(A && Bw && C && M >= 1 && N >= 1 && K >= 1 && batch >= 1 && batch <= 65535, "gemm_f32: bad argument");
+  B2_CHECK_ARG(math == B200SEP_MATH_BF16X3 || math == B200SEP_MATH_FP16, "gemm_f32: unknown math mode %d", math);
+  B2_CHECK_ARG(w_packed == nullptr || tc_packed_matches(w_packed, math), "gemm_f32: w_packed was packed for the other math mode (asked for %d)", math);
   if (tc_gemm_usable(M, N, K, batch))
     return tc_gemm_f32(A, Bw, C, M, N, K, lda, ldb, ldc, batch, strideA, strideB, strideC, alpha, bias_n, bias_m, act, res, res_scale,
-                       (batch == 1 || strideB == 0) ? w_packed : nullptr, 0, (cudaStream_t)stream);
+                       (batch == 1 || strideB == 0) ? w_packed : nullptr, 0, math, (cudaStream_t)stream);
   GemmF32 p{A, Bw, C, bias_n, bias_m, res, res_scale, M, N, K, lda, ldb, ldc, strideA, strideB, strideC, alpha, act, 0};
   if (N <= kSmallN && M >= 1024) {
     dim3 g(cdiv(M, 8), 1, batch);
@@ -637,6 +640,13 @@ extern "C" int b200sep_gemm_f32(const float* A, const float* Bw, float* C, int M
   gemm_f32_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(p);
   B2_LAUNCHED();
   return B200SEP_OK;
+}
+
+extern "C" int b200sep_gemm_f32(const float* A, const float* Bw, float* C, int M, int N, int K, int lda, int ldb, int ldc, int batch, int64_t strideA,
+                                int64_t strideB, int64_t strideC, float alpha, const float* bias_n, const float* bias_m, int act, const float* res,
+                                const float* res_scale, const void* w_packed, void* stream) {
+  return b200sep_gemm_f32_math(A, Bw, C, M, N, K, lda, ldb, ldc, batch, strideA, strideB, strideC, alpha, bias_n, bias_m, act, res, res_scale, w_packed,
+                               B200SEP_MATH_BF16X3, stream);
 }
 
 extern "C" int b200sep_softmax_rows_f32(float* x, int64_t rows, int n, int64_t ld, void* stream) {
@@ -722,19 +732,32 @@ extern "C" int b200sep_gemm_kn_f32(const float* A, const float* B_kn, float* C, 
     B2_LAUNCHED();
     return B200SEP_OK;
   }
-  return tc_gemm_f32(A, B_kn, C, M, N, K, lda, ldb, ldc, batch, strideA, strideB, strideC, alpha, nullptr, nullptr, 0, nullptr, nullptr, nullptr, 1, (cudaStream_t)stream);
+  return tc_gemm_f32(A, B_kn, C, M, N, K, lda, ldb, ldc, batch, strideA, strideB, strideC, alpha, nullptr, nullptr, 0, nullptr, nullptr, nullptr, 1, B200SEP_MATH_BF16X3,
+                     (cudaStream_t)stream);
 }
 
-extern "C" int64_t b200sep_tc_packed_floats(int N, int K) { return (N >= 1 && K >= 1) ? tc_packed_bytes(N, K) / 4 : 0; }
+extern "C" int64_t b200sep_tc_packed_floats_math(int N, int K, int math) {
+  return (N >= 1 && K >= 1 && (math == B200SEP_MATH_BF16X3 || math == B200SEP_MATH_FP16)) ? tc_packed_bytes(N, K, math) / 4 : 0;
+}
 
-extern "C" int b200sep_tc_pack_linear_weights(const float* W, int N, int K, int ldw, float* packed, void* stream) {
+extern "C" int64_t b200sep_tc_packed_floats(int N, int K) { return b200sep_tc_packed_floats_math(N, K, B200SEP_MATH_BF16X3); }
+
+extern "C" int b200sep_tc_pack_linear_weights_math(const float* W, int N, int K, int ldw, float* packed, int math, void* stream) {
   B2_CHECK_ARG(W && packed && N >= 1 && K >= 1 && ldw >= K, "tc_pack_linear_weights: bad argument");
   B2_CHECK_ARG((reinterpret_cast<uintptr_t>(packed) & 15) == 0, "tc_pack_linear_weights: packed must be 16-byte aligned");
-  return tc_pack_linear(W, N, K, ldw, packed, (cudaStream_t)stream);
+  return tc_pack_linear(W, N, K, ldw, packed, math, (cudaStream_t)stream);
+}
+
+extern "C" int b200sep_tc_pack_linear_weights(const float* W, int N, int K, int ldw, float* packed, void* stream) {
+  return b200sep_tc_pack_linear_weights_math(W, N, K, ldw, packed, B200SEP_MATH_BF16X3, stream);
+}
+
+extern "C" int b200sep_tc_pack_conv_weights_math(const float* w_blocked, int Cin, int taps, int Cout, float* packed, int math, void* stream) {
+  B2_CHECK_ARG(w_blocked && packed && Cin >= 1 && taps >= 1 && Cout >= 1, "tc_pack_conv_weights: bad argument");
+  B2_CHECK_ARG((reinterpret_cast<uintptr_t>(packed) & 15) == 0, "tc_pack_conv_weights: packed must be 16-byte aligned");
+  return tc_pack_conv(w_blocked, Cin, taps, Cout, cdiv(Cout, 48) * 48, packed, math, (cudaStream_t)stream);
 }
 
 extern "C" int b200sep_tc_pack_conv_weights(const float* w_blocked, int Cin, int taps, int Cout, float* packed, void* stream) {
-  B2_CHECK_ARG(w_blocked && packed && Cin >= 1 && taps >= 1 && Cout >= 1, "tc_pack_conv_weights: bad argument");
-  B2_CHECK_ARG((reinterpret_cast<uintptr_t>(packed) & 15) == 0, "tc_pack_conv_weights: packed must be 16-byte aligned");
-  return tc_pack_conv(w_blocked, Cin, taps, Cout, cdiv(Cout, 48) * 48, packed, (cudaStream_t)stream);
+  return b200sep_tc_pack_conv_weights_math(w_blocked, Cin, taps, Cout, packed, B200SEP_MATH_BF16X3, stream);
 }
