@@ -5,6 +5,10 @@ ctor `(common_config, arch_config)` with arch keys segment_size / shifts / overl
 `separate(path, custom_output_names)`, `demix_demucs(mix) -> (S, 2, N)` with sources 0 and 1 swapped.
 Every forward, the shift trick, the segment overlap-add and the bag average run on the GPU (b200.demucs.DemucsEngine).
 Time-domain Demucs v1 / v2 packages are not part of this path.
+
+arch key `b200_sharded`: one process per GPU under an initialised torch.distributed group (nccl); every rank calls `separate(path)` on the same
+file, the segments of every (model, shift) pass are split by time over the ranks (b200/sharded.py), with rank 0's shift offsets used on every
+rank, and rank 0 writes the stem files and returns their names while the other ranks write nothing and return [].
 """
 import os
 import random
@@ -31,8 +35,16 @@ class DemucsSeparator(CommonSeparator):
         self.overlap = arch_config.get("overlap", 0.25)
         self.segments_enabled = arch_config.get("segments_enabled", True)
         self.batch_size = int(arch_config.get("batch_size", 4))  # segments per forward (H100 addition; results do not depend on it)
+        self.sharded = bool(arch_config.get("b200_sharded", False))  # one process per GPU (torch.distributed, nccl): time-shard every track over the ranks
         if not torch.cuda.is_available():
             raise RuntimeError("DemucsSeparator (H100 build) needs a CUDA device: there is no CPU path in this package")
+        self.dist = None
+        if self.sharded:
+            import torch.distributed as dist
+
+            if not dist.is_initialized():
+                raise RuntimeError("demucs_params['b200_sharded'] needs torch.distributed to be initialised (backend nccl, one process per GPU)")
+            self.dist = dist
         self.torch_device = torch.device("cuda", torch.cuda.current_device())
         self.demucs_source_map = DEMUCS_4_SOURCE_MAPPER
         self.load_model()
@@ -52,13 +64,19 @@ class DemucsSeparator(CommonSeparator):
                     pass
             nets.append((HDemucsNet if isinstance(cfg, HDemucsConfig) else HTDemucsNet)(cfg, state, device=self.torch_device, math=math))
         # segments_enabled=False: apply_model(split=False), one forward over the whole track (HTDemucs raises beyond its training segment, like the reference)
-        self.engine = DemucsEngine(nets, bag_weights=weights, overlap=self.overlap, batch_size=self.batch_size, split=bool(self.segments_enabled))
+        self.engine = DemucsEngine(nets, bag_weights=weights, overlap=self.overlap, batch_size=self.batch_size, split=bool(self.segments_enabled),
+                                   dist=self.dist)
 
     def demix_demucs(self, mix):
-        """(2, N) -> (S, 2, N) (demucs_separator.py:162-195).  The shift offsets are drawn exactly where apply_model draws them
-        (`random.randint(0, max_shift)` per shift, per model of the bag, apply.py:207)."""
+        """(2, N) -> (S, 2, N) (demucs_separator.py:162-195); None on the ranks other than 0 of a sharded run.  The shift offsets are drawn exactly
+        where apply_model draws them (`random.randint(0, max_shift)` per shift, per model of the bag, apply.py:207); sharded, every rank draws and then
+        takes rank 0's draws, so all ranks run the same passes."""
         max_shift = int(0.5 * self.engine.cfg.samplerate)
         offsets = [[random.randint(0, max_shift) for _ in range(self.shifts)] for _ in self.engine.nets]
+        if self.dist is not None:
+            box = [offsets]
+            self.dist.broadcast_object_list(box, src=0, device=self.torch_device)
+            offsets = box[0]
         return self.engine.demix(np.asarray(mix, dtype=np.float32), offsets)
 
     def separate(self, audio_file_path, custom_output_names=None):
@@ -66,6 +84,8 @@ class DemucsSeparator(CommonSeparator):
         self.audio_file_base = os.path.splitext(os.path.basename(audio_file_path))[0]
         mix = self.prepare_mix(self.audio_file_path)
         source = self.demix_demucs(mix)
+        if source is None:  # sharded, rank != 0: rank 0 holds the stems and writes the files
+            return []
         self.demucs_source_map = {2: DEMUCS_2_SOURCE_MAPPER, 6: DEMUCS_6_SOURCE_MAPPER}.get(len(source), DEMUCS_4_SOURCE_MAPPER)  # :134-146
         output_files = []
         for stem_name, stem_value in self.demucs_source_map.items():

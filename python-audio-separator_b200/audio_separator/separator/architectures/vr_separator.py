@@ -4,6 +4,10 @@ Plugin contract of the reference's VRSeparator (audio_separator/separator/archit
 `(common_config, arch_config)` with arch keys batch_size / window_size / aggression / enable_tta / enable_post_process /
 post_process_threshold / high_end_process, `separate(path, custom_output_names)` -> [primary, secondary] files.
 The multi-band analysis, the patch loop, the mask post-processing and the band synthesis run on the GPU (b200.vr.VREngine).
+
+arch key `b200_sharded`: one process per GPU under an initialised torch.distributed group (nccl); every rank calls `separate(path)` on the same
+file, the patches of each track are split over the ranks (b200/sharded.py), and rank 0 writes the stem files and returns their names while the
+other ranks write nothing and return [].
 """
 import math
 import os
@@ -33,8 +37,16 @@ class VRSeparator(CommonSeparator):
         self.high_end_process = arch_config.get("high_end_process", False)
         self.aggression_setting = int(arch_config.get("aggression", 5))
         self.aggression = float(self.aggression_setting / 100)
+        self.sharded = bool(arch_config.get("b200_sharded", False))  # one process per GPU (torch.distributed, nccl): split every track's patches over the ranks
         if not torch.cuda.is_available():
             raise RuntimeError("VRSeparator (H100 build) needs a CUDA device: there is no CPU path in this package")
+        self.dist = None
+        if self.sharded:
+            import torch.distributed as dist
+
+            if not dist.is_initialized():
+                raise RuntimeError("vr_params['b200_sharded'] needs torch.distributed to be initialised (backend nccl, one process per GPU)")
+            self.dist = dist
         self.torch_device = torch.device("cuda", torch.cuda.current_device())
         self.model_samplerate = self.model_params["sr"]
         if self.model_samplerate != 44100:
@@ -59,17 +71,21 @@ class VRSeparator(CommonSeparator):
                                math=tc_math)
         else:
             self.net = VRNet(arch, self.model_params["bins"] * 2, state, device=self.torch_device, math=tc_math)
-        self.engine = VREngine(self.net, self.model_params, self.window_size, self.aggression_setting, self.primary_stem_name, self.batch_size)
+        self.engine = VREngine(self.net, self.model_params, self.window_size, self.aggression_setting, self.primary_stem_name, self.batch_size,
+                             dist=self.dist)
 
     def separate(self, audio_file_path, custom_output_names=None):
         self.audio_file_path = audio_file_path
         self.audio_file_base = os.path.splitext(os.path.basename(audio_file_path))[0]
         wave = self.prepare_mix(audio_file_path)  # librosa.load(mono=False, sr=44100) of a 44.1 kHz file (vr_separator.py:271)
-        primary, secondary = self.engine.separate(np.asarray(wave, dtype=np.float32), enable_tta=bool(self.enable_tta),
-                                                    post_process_threshold=self.post_process_threshold if self.enable_post_process else None,
-                                                    high_end_process=bool(self.high_end_process))
-        self.primary_source, self.secondary_source = primary.T, secondary.T
+        stems = self.engine.separate(np.asarray(wave, dtype=np.float32), enable_tta=bool(self.enable_tta),
+                                     post_process_threshold=self.post_process_threshold if self.enable_post_process else None,
+                                     high_end_process=bool(self.high_end_process))
         output_files = []
+        if stems is None:  # sharded, rank != 0: rank 0 holds the stems and writes the files
+            return output_files
+        primary, secondary = stems
+        self.primary_source, self.secondary_source = primary.T, secondary.T
         if self.output_single_stem and self.output_single_stem.lower() not in (self.primary_stem_name.lower(), self.secondary_stem_name.lower()):
             self.output_single_stem = None  # vr_separator.py:197-199
         if not self.output_single_stem or self.output_single_stem.lower() == self.primary_stem_name.lower():

@@ -12,7 +12,9 @@ Two planning rules:
                           a fixed range [q0, q1) of OUTPUT samples (the same for every pass of a Demucs bag / shift loop, so the
                           accumulation order per sample is the single-GPU order and the result is bit-identical); a unit belongs to
                           the rank its first output sample falls in.
-In both, a rank needs the trailing units of its LEFT neighbour that reach into its range: one `isend`/`irecv` pair between
+* `plan_patch_shards`  -- VR: the patches do not overlap (the 128-frame crop of every prediction), so rank r owns a contiguous run of the single-GPU
+                          loop's forwards, finalises their mask columns and needs no halo (`shard_patches`).
+In the first two, a rank needs the trailing units of its LEFT neighbour that reach into its range: one `isend`/`irecv` pair between
 time-neighbours (NCCL p2p over NVLink), posted as soon as those units are computed so the transfer overlaps the remaining forwards.
 The finalised slices go to rank 0 with point-to-point receives straight into the full-size stem buffers, or -- end-to-end entry points --
 every rank copies its own slice into a host buffer shared between the ranks (8 PCIe links in parallel, no gather at all).
@@ -94,6 +96,29 @@ def plan_range_shards(n_out: int, world: int, n_units: int, stride: int, unit_le
     if n_units < 1 or stride < 1 or unit_len < 1:
         raise ValueError("plan_range_shards: bad grid")
     return plan_start_shards(range(-base, n_units * stride - base, stride), unit_len, n_out, world)
+
+
+def plan_patch_shards(n_patches: int, world: int, roi: int = 1, batch: int = 1) -> list[Shard]:
+    """VR: patch p reads only its own input window and writes only the mask columns [p*roi, (p+1)*roi), so there is no halo and no overlap-add.
+    The patches run in forwards of `batch` (the last one holds the remainder); rank r owns the contiguous forwards [G*r/W, G*(r+1)/W) of the
+    G = ceil(n_patches / batch) of the single-GPU loop, i.e. the patches [c0, c1), and finalises the mask columns [c0*roi, c1*roi).  Every patch is then
+    predicted in the same forward, at the same batch slot, as on one GPU.  With batch 1 that is [P*r/W, P*(r+1)/W); ranks may be empty."""
+    if n_patches < 0 or world < 1 or roi < 1 or batch < 1:
+        raise ValueError("plan_patch_shards: bad arguments")
+    groups = -(-n_patches // batch)
+    shards = []
+    for r in range(world):
+        c0, c1 = (min(groups * q // world * batch, n_patches) for q in (r, r + 1))
+        shards.append(Shard(r, c0, c1, 0, c0 * roi, c1 * roi))
+    return shards
+
+
+def shard_patches(runner: "ShardRunner", n_patches: int, roi: int, batch: int, predict):
+    """The VR patch loop over the ranks: predict(p0, p1) -> this rank's mask columns (..., (p1 - p0) * roi) of the patches [p0, p1), run in
+    forwards of `batch` starting at p0.  Returns the full (..., n_patches * roi) mask on rank 0 (gather_cols), None on the other ranks."""
+    shards = plan_patch_shards(n_patches, runner.world, roi, batch)
+    sh = shards[runner.rank]
+    return runner.gather_cols(predict(sh.c0, sh.c1), [(s.q0, s.q1) for s in shards], n_patches * roi)
 
 
 def balanced_batches(n: int, max_batch: int) -> list[int]:

@@ -8,6 +8,9 @@ This file is the graph builder: device buffers + launch order.  All arithmetic i
 VR 5.1 models (nets_new.CascadedNet, LSTM branch) run through VRNet51.  enable_tta, enable_post_process and high_end_process are supported.  Not covered (raises): `reverse` model
 parameters, analysis bands resampled with anything but res_type "polyphase".  The band UP-sampling of the synthesis side uses the
 same Kaiser polyphase design (the reference calls libsamplerate "sinc_fastest" there; see DESIGN.md: parity unpinned for that step).
+
+VREngine(dist=...) splits the patches of one track over the GPUs of a box (b200/sharded.py `plan_patch_shards`): the patches do not overlap, so
+there is no halo; rank 0 gathers the mask and runs the mask post-processing and the synthesis.
 """
 from __future__ import annotations
 
@@ -386,8 +389,16 @@ class VRNet51(VRNet):
 class VREngine:
     """The VRSeparator hot path between reading the file and final_process, device resident."""
 
-    def __init__(self, net: VRNet, param: dict, window_size=512, aggression=5, primary_stem="Instrumental", batch_size=1):
+    def __init__(self, net: VRNet, param: dict, window_size=512, aggression=5, primary_stem="Instrumental", batch_size=1, dist=None, group=None):
+        """dist / group: torch.distributed (backend nccl, one process per GPU) -- every rank is given the same track, runs the front end on all of
+        it and predicts its own run of patches (b200/sharded.py `plan_patch_shards`); rank 0 gathers the mask and runs the back end, the other
+        ranks get None from `inference` and `separate`.  Without dist: the single-GPU path."""
         self.net, self.p = net, param
+        self.dist = dist
+        if dist is not None:
+            from .sharded import ShardRunner
+
+            self.runner = ShardRunner(dist, group)
         self.is_51 = isinstance(net, VRNet51)  # is_v51_model: filter masks instead of the running-gain filters, per-band convert_channels
         self.window_size, self.batch_size = int(window_size), max(1, int(batch_size))
         self.aggression, self.primary_stem = int(aggression), primary_stem
@@ -531,7 +542,8 @@ class VREngine:
         return 1 + a[0] / 3, 1 + a[0], 1 + a[1] / 3, 1 + a[1]
 
     def _execute(self, spec, pad_l, pad_r, roi):
-        """_execute of inference_vr (vr_separator.py:296-327): zero-pad the magnitudes, normalise by the maximum, run every patch -> mask (2, bins, patches*roi)."""
+        """_execute of inference_vr (vr_separator.py:296-327): zero-pad the magnitudes, normalise by the maximum, run every patch -> mask (2, bins, patches*roi).
+        Sharded: every rank pads and normalises the whole track, predicts its own patches, and rank 0 gets the gathered mask (the other ranks None)."""
         nb, n_frame = spec.shape[1], spec.shape[2]
         off = self.net.offset
         n_pad = pad_l + n_frame + pad_r
@@ -540,20 +552,40 @@ class VREngine:
         mx = _new((1,), mag)
         check(lib.b200sep_absmax(_ptr(mag), mag.numel(), _ptr(mx), _stream()), "absmax")
         peak = float(mx.cpu())
+        if self.dist is not None:  # the ranks normalise independently: a rank given a different track must fail here, not write a wrong mask
+            pk = torch.tensor([peak, -peak], dtype=torch.float32, device=self.device)
+            self.dist.all_reduce(pk, op=self.dist.ReduceOp.MAX, group=self.runner.group)
+            if float(pk[0]) != peak or float(pk[1]) != -peak:
+                raise RuntimeError(f"VREngine: the ranks disagree on the normalisation peak ({peak} here, {-float(pk[1])}..{float(pk[0])} over the group): "
+                                   "every rank must be given the same track")
         ew(mag, None, mag, 1.0 / peak if peak > 0 else float("nan"), 0.0)  # X_mag_pad /= X_mag_pad.max()
         patches = (n_pad - 2 * off) // roi
         if patches <= 0 or self.window_size - 2 * off <= 0:
             raise ValueError("Window size error: h1_shape[3] must be greater than h2_shape[3]")
-        mask = _new((2, nb, patches * roi), mag)
-        m4 = mask.view(2, nb, patches, roi)
-        for i in range(0, patches, self.batch_size):
-            b = min(self.batch_size, patches - i)
+        if self.dist is None:
+            mask = _new((2, nb, patches * roi), mag)
+            self._predict(mag, 0, patches, roi, mask)
+            return mask
+        from .sharded import shard_patches
+
+        def predict(p0, p1):
+            part = _new((2, nb, (p1 - p0) * roi), mag)
+            self._predict(mag, p0, p1, roi, part)
+            return part
+
+        return shard_patches(self.runner, patches, roi, self.batch_size, predict)
+
+    def _predict(self, mag, p0, p1, roi, out):
+        """The patches [p0, p1) of the normalised padded magnitude, in forwards of batch_size from p0 -> out (2, bins, (p1 - p0) * roi)."""
+        nb, n_pad = mag.shape[1], mag.shape[2]
+        m4 = out.view(2, nb, p1 - p0, roi)
+        for i in range(p0, p1, self.batch_size):
+            b = min(self.batch_size, p1 - i)
             batch = _new((b, 2, nb, self.window_size), mag)
             src = torch.as_strided(mag, (b, 2, nb, self.window_size), (roi, nb * n_pad, n_pad, 1), storage_offset=i * roi)
             copy_view(src, batch)
             pred = self.graphed(batch)  # (b, 2, nb, roi): CascadedASPPNet.predict_mask, its launch list replayed as one CUDA graph per batch size
-            copy_view(pred, m4[:, :, i : i + b].permute(2, 0, 1, 3))
-        return mask
+            copy_view(pred, m4[:, :, i - p0 : i - p0 + b].permute(2, 0, 1, 3))
 
     def _post_process(self, mask, n_frame, thres):
         """merge_artifacts (spec_utils.py:180-223) on the aggressiveness-adjusted mask (2, bins, stride): the min over (channel, bin) per frame is reduced
@@ -566,8 +598,9 @@ class VREngine:
             wd = torch.from_numpy(w).to(self.device)
             check(lib.b200sep_vr_mask_merge(_ptr(mask), _ptr(wd), stride, 2 * nb, n_frame, _stream()), "vr_mask_merge")
 
-    def inference(self, spec: torch.Tensor, enable_tta=False, post_process_threshold=None):
-        """VRSeparator.inference_vr (vr_separator.py:295-366): planes (4, bins+1, frames) -> (y planes, v planes)."""
+    def masks(self, spec: torch.Tensor, enable_tta=False):
+        """The network part of inference_vr (vr_separator.py:296-359): planes (4, bins+1, frames) -> mask (2, bins+1, >= frames), averaged over
+        both passes with enable_tta.  Sharded: rank 0 gets the mask, the other ranks None."""
         nb, n_frame = spec.shape[1], spec.shape[2]
         off = self.net.offset
         roi = self.window_size - 2 * off
@@ -577,11 +610,27 @@ class VREngine:
         mask = self._execute(spec, pad_l, pad_r, roi)
         if enable_tta:  # second pass shifted by half a region of interest; (mask + mask_tta[roi/2:]) / 2 on the first n_frame columns (:351-359)
             m2 = self._execute(spec, pad_l + roi // 2, pad_r + roi // 2, roi)
+            if mask is None:
+                return None
             avg = _new((2, nb, n_frame), mask)
             a_c, b_c = _new((2, nb, n_frame), mask), _new((2, nb, n_frame), mask)
             copy_view(mask[None, :, :, :n_frame], a_c[None])
             copy_view(m2[None, :, :, roi // 2 : roi // 2 + n_frame], b_c[None])
             mask = ew(a_c, b_c, avg, 0.5, 0.5)
+        return mask
+
+    def inference(self, spec: torch.Tensor, enable_tta=False, post_process_threshold=None):
+        """VRSeparator.inference_vr (vr_separator.py:295-366): planes (4, bins+1, frames) -> (y planes, v planes); None on the ranks other than 0 of a
+        sharded run."""
+        mask = self.masks(spec, enable_tta)
+        if mask is None:
+            return None
+        return self.apply_mask(spec, mask, post_process_threshold)
+
+    def apply_mask(self, spec: torch.Tensor, mask: torch.Tensor, post_process_threshold=None):
+        """The mask side of inference_vr (vr_separator.py:329-366): adjust_aggr, merge_artifacts (post_process_threshold), the products -> (y, v)
+        planes.  Updates `mask` in place when post-processing."""
+        nb, n_frame = spec.shape[1], spec.shape[2]
         y, v = _new(spec.shape, spec), _new(spec.shape, spec)
         e = self._exponents()
         if post_process_threshold is not None:  # enable_post_process: adjust_aggr first, then merge_artifacts, then the products (vr_separator.py:329-343)
@@ -654,8 +703,11 @@ class VREngine:
         return wave
 
     def separate(self, wave: np.ndarray, enable_tta=False, post_process_threshold=None, high_end_process=False):
-        """(2, N) host -> primary (2, M), secondary (2, M) host float32, M = hop_top * (frames - 1)."""
+        """(2, N) host -> primary (2, M), secondary (2, M) host float32, M = hop_top * (frames - 1); None on the ranks other than 0 of a sharded run."""
         wd = torch.from_numpy(np.ascontiguousarray(wave, dtype=np.float32)).to(self.device)
         spec = self.loading_mix(wd, keep_high_end=high_end_process)
-        y, v = self.inference(spec, enable_tta, post_process_threshold)
+        yv = self.inference(spec, enable_tta, post_process_threshold)
+        if yv is None:
+            return None
+        y, v = yv
         return self.spec_to_wav(y, high_end_process).cpu().numpy(), self.spec_to_wav(v, high_end_process).cpu().numpy()
