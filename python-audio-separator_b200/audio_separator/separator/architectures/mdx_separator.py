@@ -37,6 +37,13 @@ class MDXSeparator(CommonSeparator):
 
         if not torch.cuda.is_available():
             raise RuntimeError("MDXSeparator (H100 build) needs a CUDA device: there is no onnxruntime / CPU path in this package")
+        self.dist = None
+        if self.sharded:
+            import torch.distributed as dist
+
+            if not dist.is_initialized():
+                raise RuntimeError("mdx_params['b200_sharded'] needs torch.distributed to be initialised (backend nccl, one process per GPU)")
+            self.dist = dist
         self.torch_device = torch.device("cuda", torch.cuda.current_device())
         self.n_bins = self.trim = self.chunk_size = self.gen_size = 0
         self._host_bufs = {}
@@ -64,10 +71,8 @@ class MDXSeparator(CommonSeparator):
         flat = mdx_weights.flatten_state(state, **hp)
         max_batch = max(1, int(self.batch_size))
         self.net = MdxNet(flat, dim_t=self.segment_size, max_batch=max_batch, precision=self.precision, **hp)
-        engine_cls = MdxEngine
-        if self.sharded:
-            from ..b200.sharded import ShardedMdxEngine as engine_cls
-        self.engine = engine_cls(self.net, self.n_fft, self.hop_length, self.dim_f, self.segment_size, self.overlap, self.compensate, bool(self.enable_denoise), max_batch)
+        self.engine = MdxEngine(self.net, self.n_fft, self.hop_length, self.dim_f, self.segment_size, self.overlap, self.compensate, bool(self.enable_denoise), max_batch,
+                                dist=self.dist)
         self.model_run = lambda spek: self.net.forward(torch.as_tensor(spek, dtype=torch.float32, device=self.torch_device))
 
     def initialize_model_settings(self):

@@ -18,7 +18,8 @@ import numpy as np
 import torch
 
 from ._lib import LAYOUT_CFT, MATH_BF16X3, check, lib
-from .engine import StftPlan, _ptr, _require_cuda, _stream
+from .engine import StftPlan, _ptr, _require_cuda, _stream, _window
+from .sharded import ShardRunner, plan_range_shards
 
 ACT_NONE, ACT_RELU, ACT_GELU = 0, 1, 2
 _DCONV_FUSED_HID = (4, 6, 8, 12, 16, 24, 32, 48)  # hidden widths b200sep_dconv_f32 is instantiated for
@@ -559,8 +560,6 @@ class DemucsEngine:
 
     def __init__(self, nets, bag_weights=None, overlap=0.25, batch_size=4, dist=None, group=None, split=True):
         _require_cuda()
-        from .sharded import ShardRunner
-
         self.nets = list(nets)
         cfg = self.nets[0].cfg
         self.cfg = cfg
@@ -573,35 +572,28 @@ class DemucsEngine:
         self.batch_size = int(batch_size)
         self.device = self.nets[0].device
         self.runner = ShardRunner(dist, group)
-        self.rank, self.world = self.runner.rank, self.runner.world
         self.split = bool(split)  # apply_model(split=...): False = segments_enabled False, ONE forward over the whole (shifted) track (apply.py:251-260)
-        if not self.split and self.world > 1:
+        if not self.split and self.runner.world > 1:
             raise ValueError("split=False is one forward over the whole track: nothing to shard across ranks")
 
     def out_range(self, N):
         """Output samples [q0, q1) this rank finalises (everything on a single GPU)."""
-        return N * self.rank // self.world, N * (self.rank + 1) // self.world
+        return self.runner.out_range(N)
 
     def _apply_split(self, net, tensor, offset, length, out, q0, n_out, scale, chan_scale, accumulate):
         """apply_model's split branch on TensorChunk(tensor, offset, length) (apply.py:215-250); the weighted result's samples
         [q0, q0 + n_out) -- this rank's part [r0, r1) of them -- are scaled and written / accumulated into out (S*2, r1 - r0)."""
-        from .sharded import plan_range_shards
-
         cfg = self.cfg
         seg = cfg.seg_len
         S = len(cfg.sources)
         stride = int((1 - self.overlap) * seg)
-        total = tensor.shape[-1]
         offs = list(range(0, length, stride))
-        sh = plan_range_shards(n_out, self.world, len(offs), stride, seg, q0)[self.rank]
+        sh = plan_range_shards(n_out, self.runner.world, len(offs), stride, seg, q0)[self.runner.rank]
         assert tuple(out.shape) == (S * 2, sh.q1 - sh.q0), (out.shape, sh)
         # TensorChunk.padded zero-fills outside the tensor (apply.py:97-113): only the part this rank's segments read is materialised
         lo = offset + sh.c0 * stride - seg
         hi = offset + (sh.c1 - 1) * stride + 2 * seg if sh.n_own else lo + 1
-        ext = torch.zeros((2, hi - lo), dtype=torch.float32, device=tensor.device)
-        a, b = max(lo, 0), min(hi, total)
-        if b > a:
-            ext[:, a - lo : b - lo].copy_(tensor[:, a:b])
+        ext = _window(tensor, lo, hi)
         local = torch.empty((sh.halo + sh.n_own, S * 2, seg), dtype=torch.float32, device=tensor.device)
 
         pads = getattr(cfg, "pads_to_segment", True)  # HTDemucs: chunk.padded(valid_length = training segment); HDemucs: every chunk at its own length (apply.py:252-257)
@@ -635,10 +627,7 @@ class DemucsEngine:
             raise ValueError(f"Given length {length} is longer than training length {valid}")
         delta = valid - length
         start = offset - delta // 2
-        batch = torch.zeros((1, 2, valid), dtype=torch.float32, device=tensor.device)
-        a, b = max(start, 0), min(start + valid, tensor.shape[-1])
-        if b > a:
-            batch[0, :, a - start : b - start].copy_(tensor[:, a:b])
+        batch = _window(tensor, start, start + valid)[None]
         y = net.forward(batch).reshape(S * 2, valid)
         d = delta // 2  # center_trim (utils.py:53-70): delta // 2 off the left
         cs = chan_scale.cpu().tolist() if chan_scale is not None else [1.0] * (S * 2)
@@ -688,9 +677,7 @@ class DemucsEngine:
 
     def gather(self, part: torch.Tensor, N: int):
         """Rank 0: the full (S, 2, N) sources from every rank's demix_device slice (None elsewhere); identity on a single GPU."""
-        if self.world == 1:
-            return part
-        return self.runner.gather_cols(part, [(N * r // self.world, N * (r + 1) // self.world) for r in range(self.world)], N)
+        return self.runner.gather_cols(part, [self.runner.out_range(N, r) for r in range(self.runner.world)], N)
 
     def demix_host(self, mix_host: torch.Tensor, out_host: torch.Tensor, shift_offsets):
         """End-to-end entry point on page-locked host tensors: mix_host (2, N) -> out_host (S, 2, N).  Sharded runs map the SAME two buffers in every rank:

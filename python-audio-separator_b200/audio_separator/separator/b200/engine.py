@@ -14,6 +14,7 @@ import torch
 
 from . import _lib
 from ._lib import LAYOUT_CFT, LAYOUT_CTF, check, lib
+from .sharded import ShardRunner, plan_range_shards, plan_shards
 
 
 def _require_cuda():
@@ -24,6 +25,15 @@ def _require_cuda():
 def _ptr(t: torch.Tensor) -> int:
     assert t.is_cuda and t.is_contiguous(), "engine buffers must be contiguous CUDA tensors"
     return t.data_ptr()
+
+
+def _window(x: torch.Tensor, lo: int, hi: int) -> torch.Tensor:
+    """Samples [lo, hi) of the (2, N) signal x as a new contiguous float32 (2, hi - lo) tensor, zero where they fall outside [0, N)."""
+    out = torch.zeros((2, hi - lo), dtype=torch.float32, device=x.device)
+    a, b = max(lo, 0), min(hi, x.shape[-1])
+    if b > a:
+        out[:, a - lo : b - lo].copy_(x[:, a:b])
+    return out
 
 
 def _stream() -> int:
@@ -123,9 +133,16 @@ class MdxNet:
 
 
 class MdxEngine:
-    """Device-resident MDX separation: chunk grid, run_model batches, windowed overlap-add, stem arithmetic."""
+    """Device-resident MDX separation: chunk grid, run_model batches, windowed overlap-add, stem arithmetic.
 
-    def __init__(self, net: MdxNet | None, n_fft, hop_length, dim_f, segment_size, overlap, compensate=1.0, enable_denoise=False, batch_size=None):
+    With `dist` (torch.distributed, nccl, one process per GPU) the chunk grid is time-sharded (b200/sharded.py, plan_shards): rank r runs a
+    contiguous range of chunks, receives from its left neighbour the chunks that reach into its range and finalises the padded positions
+    [c0*step, c1*step).  Every rank is given the same (2, N) mix and the stems are gathered on rank 0 (`separate_device`), or every rank reads
+    and writes only its part of host buffers shared between the ranks (`separate_host`).  Without `dist` the same code runs as one shard holding
+    every chunk."""
+
+    def __init__(self, net: MdxNet | None, n_fft, hop_length, dim_f, segment_size, overlap, compensate=1.0, enable_denoise=False, batch_size=None,
+                 dist=None, group=None):
         _require_cuda()
         self.net = net
         self.n_fft, self.hop, self.dim_f = int(n_fft), int(hop_length), int(dim_f)
@@ -142,6 +159,7 @@ class MdxEngine:
             self.batch = min(self.batch, net.max_batch)
         self._work = None
         self.device = torch.device("cuda", torch.cuda.current_device())
+        self.runner = ShardRunner(dist, group)
 
     # ---- chunk grid (mdx_separator.py:307-348)
     def grid(self, n_samples: int, is_match_mix=False):
@@ -175,45 +193,96 @@ class MdxEngine:
             )
         return out
 
+    def _plan(self, N, is_match_mix=False):
+        """The chunk grid and this rank's shard of it: (grid, shards, sh, p0, p1), with [p0, p1) the padded positions this rank's chunks read."""
+        grid = L, step, n_chunks, _ = self.grid(N, is_match_mix)
+        shards = plan_shards(N, L, step, self.chunk_size, self.trim, n_chunks, self.runner.world)
+        sh = shards[self.runner.rank]
+        p0 = sh.c0 * step
+        p1 = min(L, (sh.c1 - 1) * step + self.chunk_size) if sh.n_own else p0
+        return grid, shards, sh, p0, p1
+
+    def _chunks_and_ola(self, N, grid, sh, p0, sl, is_match_mix, out_scale, primary, secondary, out_base, mix, mix_ld, mix_base, interleave):
+        """Own chunks from `sl` = the padded mixture's positions [p0, p0 + len), halo exchange, overlap-add of this rank's output range [q0, q1)
+        into primary / secondary rows [q - out_base] (columns when not interleave)."""
+        L, step, n_chunks, overlap = grid
+        T = self.chunk_size
+        local = torch.empty((sh.halo + sh.n_own, 2, T), dtype=torch.float32, device=self.device)  # [halo | own]
+        net = None if is_match_mix else self.net.handle
+        Ls = sl.shape[1]
+
+        def compute(buf, slot0, unit0, n):
+            work = self._workspace(n)
+            off = unit0 * step - p0
+            check(lib.b200sep_mdx_run_model(self.plan.handle, net, sl.data_ptr() + off * 4, step, Ls, Ls - off, n, T, self.dim_f, int(self.enable_denoise),
+                                            _ptr(buf[slot0 : slot0 + n]), _ptr(work), _stream()), "mdx_run_model")
+
+        self.runner.wait_all(self.runner.run_units(sh, local, compute, self.batch))
+        if sh.q1 > sh.q0:
+            check(lib.b200sep_demix_overlap_add_range_ex(_ptr(local), sh.c0 - sh.halo, sh.halo + sh.n_own, n_chunks, T, step, L, self.trim, N, sh.q0, sh.q1, int(overlap != 0),
+                                                         float(out_scale), _ptr(mix) if mix is not None else None, mix_ld, mix_base, self.compensate, int(interleave),
+                                                         _ptr(primary), _ptr(secondary) if secondary is not None else None, out_base, _stream()), "demix_overlap_add_range_ex")
+
     def demix_device(self, mix_dev: torch.Tensor, is_match_mix=False, out_scale=1.0, with_secondary=False, interleave=False):
         """MDXSeparator.demix (mdx_separator.py:293-412) with everything resident in HBM.
 
-        mix_dev: (2,N) float32 CUDA (already peak-normalised by the caller).  Returns primary (2,N) [or (N,2) when
-        interleave] and, with_secondary, secondary = mix - compensate*primary (mdx_separator.py:182).
+        mix_dev: (2,N) float32 CUDA (already peak-normalised by the caller), the same on every rank.  Returns primary (2,N) [or (N,2) when
+        interleave] and, with_secondary, secondary = mix - compensate*primary (mdx_separator.py:182); None on the ranks other than 0.
+        Planar (2,N) output needs a world of size 1.
         """
         assert mix_dev.is_cuda and mix_dev.dtype == torch.float32 and mix_dev.shape[0] == 2
+        assert interleave or self.runner.world == 1, "the time-sharded path produces (N, 2) stems"
         mix_dev = mix_dev.contiguous()
         N = mix_dev.shape[1]
-        L, step, n_chunks, overlap = self.grid(N, is_match_mix)
-        T = self.chunk_size
-        mixture = torch.zeros((2, L), dtype=torch.float32, device=self.device)  # [0]*trim + mix + [0]*pad, :329
-        mixture[:, self.trim : self.trim + N] = mix_dev
-        chunks = torch.empty((n_chunks, 2, T), dtype=torch.float32, device=self.device)
-        net = None if is_match_mix else self.net.handle
-        esz = 4
-        for b0 in range(0, n_chunks, self.batch):
-            nb = min(self.batch, n_chunks - b0)
-            work = self._workspace(nb)
-            check(
-                lib.b200sep_mdx_run_model(
-                    self.plan.handle, net, mixture.data_ptr() + b0 * step * esz, step, L, L - b0 * step, nb, T, self.dim_f, int(self.enable_denoise), _ptr(chunks[b0 : b0 + nb]), _ptr(work), _stream()
-                ),
-                "mdx_run_model",
-            )
+        grid, shards, sh, p0, p1 = self._plan(N, is_match_mix)
+        sl = _window(mix_dev, p0 - self.trim, p0 - self.trim + max(p1 - p0, 1))  # this rank's part of [0]*trim + mix + [0]*pad (:329)
         shape = (N, 2) if interleave else (2, N)
         primary = torch.empty(shape, dtype=torch.float32, device=self.device)
         secondary = torch.empty(shape, dtype=torch.float32, device=self.device) if with_secondary else None
-        check(
-            lib.b200sep_demix_overlap_add(
-                _ptr(chunks), n_chunks, T, step, L, self.trim, N, int(overlap != 0), float(out_scale), _ptr(mix_dev) if with_secondary else None, self.compensate, int(interleave), _ptr(primary), _ptr(secondary) if with_secondary else None, _stream()
-            ),
-            "demix_overlap_add",
-        )
+        self._chunks_and_ola(N, grid, sh, p0, sl, is_match_mix, out_scale, primary, secondary, 0, mix_dev if with_secondary else None, N, 0, interleave)
+        self.runner.gather_rows([primary] + ([secondary] if with_secondary else []), shards, dim=0)
+        if self.runner.rank != 0:
+            return (None, None) if with_secondary else None
         return (primary, secondary) if with_secondary else primary
+
+    def separate_host(self, mix_host: torch.Tensor, out_primary: torch.Tensor, out_secondary: torch.Tensor, normalization_threshold=0.9, amplification_threshold=0.0):
+        """End-to-end entry point over host buffers SHARED by the ranks (pinned): mix_host (2, N) float32; out_* (N, 2) float32.  Every rank uploads only
+        the samples its chunks and its output range touch, the peak (mdx_separator.py:155) is an all-reduce(MAX) of the per-rank partial peaks, and every
+        rank writes its own slice of both stems into the shared output buffers: N PCIe links in parallel, no gather.  Returns this rank's (h2d, d2h) bytes."""
+        N = mix_host.shape[1]
+        grid, _, sh, p0, p1 = self._plan(N)
+        a, b = max(p0, self.trim), min(p1, self.trim + N)  # padded positions of this rank's chunks that hold real samples
+        lo, hi = sh.q0, sh.q1
+        if b > a:
+            lo, hi = min(lo, a - self.trim), max(hi, b - self.trim)
+        n_part, n_q = max(hi - lo, 0), sh.q1 - sh.q0
+        part = torch.zeros((2, max(n_part, 1)), dtype=torch.float32, device=self.device)
+        for c in range(2 if n_part else 0):  # contiguous row slices: true async copies out of the pinned buffer
+            part[c, :n_part].copy_(mix_host[c, lo:hi], non_blocking=True)
+        peak = torch.zeros(1, dtype=torch.float32, device=self.device)
+        if n_q > 0:  # peak over the DISJOINT partition [q0, q1)
+            own = part[:, sh.q0 - lo : sh.q1 - lo].contiguous()
+            check(lib.b200sep_absmax(_ptr(own), own.numel(), _ptr(peak), _stream()), "absmax")
+        if self.runner.world > 1:
+            dist = self.runner.dist
+            dist.all_reduce(peak, op=dist.ReduceOp.MAX, group=self.runner.group)
+        min_peak = -1.0 if amplification_threshold is None else float(amplification_threshold)
+        partn = torch.empty_like(part)
+        check(lib.b200sep_normalize(_ptr(part), part.numel(), _ptr(peak), float(normalization_threshold), min_peak, _ptr(partn), _stream()), "normalize")
+        peak_h = float(peak.item())  # `source = demix(mix) * peak` (:159): out_scale is a host float in the C ABI
+        sl = _window(partn[:, :n_part], p0 - self.trim - lo, p0 - self.trim - lo + max(p1 - p0, 1))
+        prim = torch.empty((max(n_q, 1), 2), dtype=torch.float32, device=self.device)
+        sec = torch.empty((max(n_q, 1), 2), dtype=torch.float32, device=self.device)
+        self._chunks_and_ola(N, grid, sh, p0, sl, False, peak_h, prim, sec, sh.q0, partn, partn.shape[1], lo, True)
+        if n_q > 0:
+            out_primary[sh.q0 : sh.q1].copy_(prim[:n_q], non_blocking=True)
+            out_secondary[sh.q0 : sh.q1].copy_(sec[:n_q], non_blocking=True)
+        torch.cuda.current_stream().synchronize()
+        return int(2 * n_part * 4), int(2 * n_q * 2 * 4)
 
     # ---- array-level body of MDXSeparator.separate (mdx_separator.py:152-182)
     def separate_device(self, mix_dev: torch.Tensor, normalization_threshold=0.9, amplification_threshold=0.0):
-        """mix_dev (2,N) float32 CUDA as loaded -> (primary (N,2), secondary (N,2)) CUDA float32."""
+        """mix_dev (2,N) float32 CUDA as loaded -> (primary (N,2), secondary (N,2)) CUDA float32; (None, None) on the ranks other than 0."""
         n = mix_dev.numel()
         peak = torch.empty(1, dtype=torch.float32, device=self.device)
         check(lib.b200sep_absmax(_ptr(mix_dev), n, _ptr(peak), _stream()), "absmax")  # :155
@@ -346,8 +415,6 @@ class MdxcEngine:
 
     def __init__(self, net: TfcNet, n_fft, hop_length, dim_f, dim_t, overlap, dist=None, group=None):
         _require_cuda()
-        from .sharded import ShardRunner
-
         self.net, self.n_fft, self.hop, self.dim_f, self.dim_t, self.overlap = net, int(n_fft), int(hop_length), int(dim_f), int(dim_t), int(overlap)
         self.chunk_size = self.hop * (self.dim_t - 1)  # :361
         self.hop_size = self.chunk_size // self.overlap  # :364
@@ -355,7 +422,6 @@ class MdxcEngine:
         self.batch = net.max_batch
         self.device = torch.device("cuda", torch.cuda.current_device())
         self.runner = ShardRunner(dist, group)
-        self.rank, self.world = self.runner.rank, self.runner.world
 
     def grid(self, n_samples):
         chunk, hop = self.chunk_size, self.hop_size
@@ -378,24 +444,19 @@ class MdxcEngine:
         return out
 
     def out_range(self, N):
-        return N * self.rank // self.world, N * (self.rank + 1) // self.world
+        return self.runner.out_range(N)
 
     def demix_device(self, mix_dev: torch.Tensor) -> torch.Tensor:
         """mix (2,N) float32 CUDA -> (S, 2, q1 - q0): this rank's output range (the whole (S, 2, N) on a single GPU)."""
-        from .sharded import plan_range_shards
-
         mix_dev = mix_dev.contiguous()
         N = mix_dev.shape[1]
         Lp, front, pad, n_chunks = self.grid(N)
         T, hop, S = self.chunk_size, self.hop_size, self.net.num_targets
-        sh = plan_range_shards(N, self.world, n_chunks, hop, T, front)[self.rank]
+        sh = plan_range_shards(N, self.runner.world, n_chunks, hop, T, front)[self.runner.rank]
         # this rank's part of the padded mixture (:371): positions [c0*hop, (c1-1)*hop + chunk)
         p0 = sh.c0 * hop
         p1 = (sh.c1 - 1) * hop + T if sh.n_own else p0 + 1
-        padded = torch.zeros((2, p1 - p0), dtype=torch.float32, device=self.device)
-        a, b = max(p0, front), min(p1, front + N)
-        if b > a:
-            padded[:, a - p0 : b - p0] = mix_dev[:, a - front : b - front]
+        padded = _window(mix_dev, p0 - front, p1 - front)
         Ls = padded.shape[1]
         local = torch.empty((sh.halo + sh.n_own, S * 2, T), dtype=torch.float32, device=self.device)
 
@@ -418,6 +479,4 @@ class MdxcEngine:
 
     def gather(self, part: torch.Tensor, N: int):
         """Rank 0: the full (S, 2, N) stems from every rank's demix_device slice (None elsewhere); identity on a single GPU."""
-        if self.world == 1:
-            return part
-        return self.runner.gather_cols(part, [(N * r // self.world, N * (r + 1) // self.world) for r in range(self.world)], N)
+        return self.runner.gather_cols(part, [self.runner.out_range(N, r) for r in range(self.runner.world)], N)

@@ -19,6 +19,7 @@ import torch
 from ._lib import LAYOUT_CFT, MATH_BF16X3, check, lib
 from .demucs import ACT_GELU, ACT_NONE, _new, _packed_linear
 from .engine import StftPlan, _ptr, _require_cuda, _stream
+from .sharded import ShardRunner, plan_start_shards
 
 ACT_TANH = 5
 DEFAULT_FREQS_PER_BANDS = (2,) * 24 + (4,) * 12 + (12,) * 8 + (24,) * 8 + (48,) * 8 + (128, 129)
@@ -312,8 +313,6 @@ class RoformerEngine:
     range.  Without `dist` the same code runs as one shard holding every chunk."""
 
     def __init__(self, net: BSRoformerNet, dim_t: int, overlap, sample_rate=44100, n_instruments=1, batch_size=1, dist=None, group=None):
-        from .sharded import ShardRunner
-
         self.net = net
         cfg = net.cfg
         self.chunk_size = int(cfg.stft_hop_length) * (int(dim_t) - 1)  # :301
@@ -329,7 +328,6 @@ class RoformerEngine:
 
         self.graphed = GraphedForward(self.net.forward)
         self.runner = ShardRunner(dist, group)
-        self.rank, self.world = self.runner.rank, self.runner.world
 
     def chunk_starts(self, N: int) -> list[int]:
         """i*step until a chunk would run past the end of the track, then N - chunk for every remaining start (:320-341)."""
@@ -339,18 +337,16 @@ class RoformerEngine:
         return [i if i + C <= N else N - C for i in range(0, N, self.step)]
 
     def out_range(self, N):
-        return N * self.rank // self.world, N * (self.rank + 1) // self.world
+        return self.runner.out_range(N)
 
     def demix_device(self, mix: torch.Tensor) -> torch.Tensor:
         """mix (2, N) cuda -> (n_out, 2, q1 - q0): this rank's output range (the whole (n_out, 2, N) on a single GPU); n_out = num_stems rows
         for multi-stem models, 1 row for single-target models."""
-        from .sharded import plan_start_shards
-
         mix = mix.contiguous()
         N = mix.shape[1]
         C, S = self.chunk_size, self.net.cfg.num_stems
         starts = self.chunk_starts(N)
-        sh = plan_start_shards(starts, C, N, self.world)[self.rank]
+        sh = plan_start_shards(starts, C, N, self.runner.world)[self.runner.rank]
         local = _new((sh.halo + sh.n_own, S * 2, C), mix)  # [halo | own]
 
         def compute(buf, slot0, unit0, nb):
@@ -377,6 +373,4 @@ class RoformerEngine:
 
     def gather(self, part: torch.Tensor, N: int):
         """Rank 0: the full (n_out, 2, N) stems from every rank's demix_device slice (None elsewhere); identity on a single GPU."""
-        if self.world == 1:
-            return part
-        return self.runner.gather_cols(part, [(N * r // self.world, N * (r + 1) // self.world) for r in range(self.world)], N)
+        return self.runner.gather_cols(part, [self.runner.out_range(N, r) for r in range(self.runner.world)], N)

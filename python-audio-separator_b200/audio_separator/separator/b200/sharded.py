@@ -19,9 +19,10 @@ time-neighbours (NCCL p2p over NVLink), posted as soon as those units are comput
 The finalised slices go to rank 0 with point-to-point receives straight into the full-size stem buffers, or -- end-to-end entry points --
 every rank copies its own slice into a host buffer shared between the ranks (8 PCIe links in parallel, no gather at all).
 
-The planners and `ShardRunner` (the control flow: unit order, halo exchange, overlap-add, gather) are pure host logic over
-torch.distributed and run unchanged on CPU tensors with gloo (tests/test_sharding_cpu.py injects the compute); the engines below them
-need CUDA + NCCL.
+This module is pure host logic: the planners and `ShardRunner` (the control flow: unit order, halo exchange, gather) import only the
+standard library and torch, and run unchanged on CPU tensors with gloo (tests/test_sharding_cpu.py injects the compute).  The engines that
+use them (MdxEngine, MdxcEngine in engine.py; RoformerEngine, DemucsEngine, VREngine) supply the CUDA compute and overlap-add; a single GPU
+is a world of size 1 through the same code.
 """
 from __future__ import annotations
 
@@ -143,6 +144,11 @@ class ShardRunner:
     def _peer(self, r):
         return r if self.group is None else self.dist.get_global_rank(self.group, r)
 
+    def out_range(self, n: int, rank: int | None = None):
+        """The output samples [n*r/W, n*(r+1)/W) rank r (default: this rank) finalises in the even partition of n."""
+        r = self.rank if rank is None else rank
+        return n * r // self.world, n * (r + 1) // self.world
+
     def run_units(self, sh: Shard, local: torch.Tensor, compute, max_batch: int):
         """Own units into local[halo:] in balanced batches; the batches holding the trailing `send` units run FIRST and the p2p pair is posted
         right after them, so the transfer to the right neighbour overlaps the remaining forwards.  Returns the outstanding requests
@@ -206,7 +212,10 @@ class ShardRunner:
 
     def gather_cols(self, part: torch.Tensor, ranges, n_total: int):
         """part (..., q1 - q0) on every rank -> the full (..., n_total) tensor on rank 0 (None elsewhere).  Slices along the LAST axis are not
-        contiguous in the destination, so rank 0 receives into per-rank staging tensors and copies them in place."""
+        contiguous in the destination, so rank 0 receives into per-rank staging tensors and copies them in place.  In a world of 1, `part` is
+        returned as it is."""
+        if self.world == 1:
+            return part
         dist = self.dist
         part = part.contiguous()
         if self.rank != 0:
@@ -228,104 +237,3 @@ class ShardRunner:
         for q0, q1, t in stage:
             full[..., q0:q1] = t
         return full
-
-
-# =========================================================================================================== MDX
-from .engine import MdxEngine, _ptr, _stream, check, lib  # noqa: E402  (the planners above stay importable on their own)
-
-
-class ShardedMdxEngine(MdxEngine):
-    """MdxEngine whose demix runs on torch.distributed ranks (backend nccl, one process per GPU).  Every rank is given the same (2, N) mix
-    (`separate_device`), or reads only its part of a host buffer shared between the ranks (`separate_host`); stems are returned on rank 0."""
-
-    def __init__(self, *args, group=None, **kw):
-        super().__init__(*args, **kw)
-        import torch.distributed as dist
-
-        if not dist.is_initialized():
-            raise RuntimeError("ShardedMdxEngine needs torch.distributed to be initialised (backend nccl)")
-        self.runner = ShardRunner(dist, group)
-        self.dist, self.group, self.rank, self.world = dist, group, self.runner.rank, self.runner.world
-
-    def _plan(self, N, is_match_mix=False):
-        L, step, n_chunks, overlap = self.grid(N, is_match_mix)
-        shards = plan_shards(N, L, step, self.chunk_size, self.trim, n_chunks, self.world)
-        sh = shards[self.rank]
-        p0 = sh.c0 * step  # padded positions [p0, p1) = what this rank's chunks read
-        p1 = min(L, (sh.c1 - 1) * step + self.chunk_size) if sh.n_own else p0
-        return L, step, n_chunks, overlap, shards, sh, p0, p1
-
-    def _chunks_and_ola(self, sl, p0, N, is_match_mix, out_scale, primary, secondary, out_base, mix, mix_ld, mix_base):
-        """Own chunks from `sl` = the padded mixture's positions [p0, p0 + len), halo exchange, overlap-add of this rank's output range [q0, q1)
-        into primary / secondary rows [q - out_base]."""
-        L, step, n_chunks, overlap, shards, sh, _, _ = self._plan(N, is_match_mix)
-        T = self.chunk_size
-        local = torch.empty((sh.halo + sh.n_own, 2, T), dtype=torch.float32, device=self.device)  # [halo | own]
-        net = None if is_match_mix else self.net.handle
-        Ls = sl.shape[1]
-
-        def compute(buf, slot0, unit0, n):
-            work = self._workspace(n)
-            off = unit0 * step - p0
-            check(lib.b200sep_mdx_run_model(self.plan.handle, net, sl.data_ptr() + off * 4, step, Ls, Ls - off, n, T, self.dim_f, int(self.enable_denoise),
-                                            _ptr(buf[slot0 : slot0 + n]), _ptr(work), _stream()), "mdx_run_model")
-
-        self.runner.wait_all(self.runner.run_units(sh, local, compute, self.batch))
-        if sh.q1 > sh.q0:
-            check(lib.b200sep_demix_overlap_add_range_ex(_ptr(local), sh.c0 - sh.halo, sh.halo + sh.n_own, n_chunks, T, step, L, self.trim, N, sh.q0, sh.q1, int(overlap != 0),
-                                                         float(out_scale), _ptr(mix) if mix is not None else None, mix_ld, mix_base, self.compensate, 1, _ptr(primary),
-                                                         _ptr(secondary) if secondary is not None else None, out_base, _stream()), "demix_overlap_add_range_ex")
-        return shards
-
-    def demix_device(self, mix_dev, is_match_mix=False, out_scale=1.0, with_secondary=False, interleave=True):
-        assert interleave, "the sharded path produces (N, 2) stems"
-        mix_dev = mix_dev.contiguous()
-        N = mix_dev.shape[1]
-        _, _, _, _, _, sh, p0, p1 = self._plan(N, is_match_mix)
-        sl = torch.zeros((2, max(p1 - p0, 1)), dtype=torch.float32, device=self.device)  # this rank's part of [0]*trim + mix + [0]*pad (:329)
-        a, b = max(p0, self.trim), min(p1, self.trim + N)
-        if b > a:
-            sl[:, a - p0 : b - p0] = mix_dev[:, a - self.trim : b - self.trim]
-        primary = torch.empty((N, 2), dtype=torch.float32, device=self.device)
-        secondary = torch.empty((N, 2), dtype=torch.float32, device=self.device) if with_secondary else None
-        shards = self._chunks_and_ola(sl, p0, N, is_match_mix, out_scale, primary, secondary, 0, mix_dev if with_secondary else None, N, 0)
-        self.runner.gather_rows([primary] + ([secondary] if with_secondary else []), shards, dim=0)
-        if self.rank != 0:
-            return (None, None) if with_secondary else None
-        return (primary, secondary) if with_secondary else primary
-
-    def separate_host(self, mix_host: torch.Tensor, out_primary: torch.Tensor, out_secondary: torch.Tensor, normalization_threshold=0.9, amplification_threshold=0.0):
-        """End-to-end entry point over host buffers SHARED by the ranks (pinned): mix_host (2, N) float32; out_* (N, 2) float32.  Every rank uploads only
-        the samples its chunks and its output range touch, the peak (mdx_separator.py:155) is an all-reduce(MAX) of the per-rank partial peaks, and every
-        rank writes its own slice of both stems into the shared output buffers: N PCIe links in parallel, no gather.  Returns this rank's (h2d, d2h) bytes."""
-        dist = self.dist
-        N = mix_host.shape[1]
-        _, _, _, _, _, sh, p0, p1 = self._plan(N)
-        a, b = max(p0, self.trim), min(p1, self.trim + N)  # padded positions of this rank's chunks that hold real samples
-        lo, hi = sh.q0, sh.q1
-        if b > a:
-            lo, hi = min(lo, a - self.trim), max(hi, b - self.trim)
-        n_part, n_q = max(hi - lo, 0), sh.q1 - sh.q0
-        part = torch.zeros((2, max(n_part, 1)), dtype=torch.float32, device=self.device)
-        for c in range(2 if n_part else 0):  # contiguous row slices: true async copies out of the pinned buffer
-            part[c, :n_part].copy_(mix_host[c, lo:hi], non_blocking=True)
-        peak = torch.zeros(1, dtype=torch.float32, device=self.device)
-        if n_q > 0:  # peak over the DISJOINT partition [q0, q1)
-            own = part[:, sh.q0 - lo : sh.q1 - lo].contiguous()
-            check(lib.b200sep_absmax(_ptr(own), own.numel(), _ptr(peak), _stream()), "absmax")
-        dist.all_reduce(peak, op=dist.ReduceOp.MAX, group=self.group)
-        min_peak = -1.0 if amplification_threshold is None else float(amplification_threshold)
-        partn = torch.empty_like(part)
-        check(lib.b200sep_normalize(_ptr(part), part.numel(), _ptr(peak), float(normalization_threshold), min_peak, _ptr(partn), _stream()), "normalize")
-        peak_h = float(peak.item())  # `source = demix(mix) * peak` (:159): out_scale is a host float in the C ABI
-        sl = torch.zeros((2, max(p1 - p0, 1)), dtype=torch.float32, device=self.device)
-        if b > a:
-            sl[:, a - p0 : b - p0] = partn[:, a - self.trim - lo : b - self.trim - lo]
-        prim = torch.empty((max(n_q, 1), 2), dtype=torch.float32, device=self.device)
-        sec = torch.empty((max(n_q, 1), 2), dtype=torch.float32, device=self.device)
-        self._chunks_and_ola(sl, p0, N, False, peak_h, prim, sec, sh.q0, partn, partn.shape[1], lo)
-        if n_q > 0:
-            out_primary[sh.q0 : sh.q1].copy_(prim[:n_q], non_blocking=True)
-            out_secondary[sh.q0 : sh.q1].copy_(sec[:n_q], non_blocking=True)
-        torch.cuda.current_stream().synchronize()
-        return int(2 * n_part * 4), int(2 * n_q * 2 * 4)

@@ -22,6 +22,7 @@ import torch
 from ._lib import LAYOUT_CFT, MATH_BF16X3, check, lib
 from .demucs import ACT_NONE, ACT_RELU, _new, block_conv_weight, conv2d, ew, linear
 from .engine import StftPlan, _ptr, _require_cuda, _stream
+from .sharded import ShardRunner, shard_patches
 
 ACT_LEAKY, ACT_SIGMOID = 3, 4
 NON_ACCOM_STEMS = ("Vocals", "Other", "Bass", "Drums", "Guitar", "Piano", "Synthesizer", "Strings", "Woodwinds", "Brass", "Wind Inst")  # common_separator.py:55
@@ -392,13 +393,9 @@ class VREngine:
     def __init__(self, net: VRNet, param: dict, window_size=512, aggression=5, primary_stem="Instrumental", batch_size=1, dist=None, group=None):
         """dist / group: torch.distributed (backend nccl, one process per GPU) -- every rank is given the same track, runs the front end on all of
         it and predicts its own run of patches (b200/sharded.py `plan_patch_shards`); rank 0 gathers the mask and runs the back end, the other
-        ranks get None from `inference` and `separate`.  Without dist: the single-GPU path."""
+        ranks get None from `inference` and `separate`.  Without dist the same code runs as one rank predicting every patch."""
         self.net, self.p = net, param
-        self.dist = dist
-        if dist is not None:
-            from .sharded import ShardRunner
-
-            self.runner = ShardRunner(dist, group)
+        self.runner = ShardRunner(dist, group)
         self.is_51 = isinstance(net, VRNet51)  # is_v51_model: filter masks instead of the running-gain filters, per-band convert_channels
         self.window_size, self.batch_size = int(window_size), max(1, int(batch_size))
         self.aggression, self.primary_stem = int(aggression), primary_stem
@@ -552,9 +549,10 @@ class VREngine:
         mx = _new((1,), mag)
         check(lib.b200sep_absmax(_ptr(mag), mag.numel(), _ptr(mx), _stream()), "absmax")
         peak = float(mx.cpu())
-        if self.dist is not None:  # the ranks normalise independently: a rank given a different track must fail here, not write a wrong mask
+        if self.runner.world > 1:  # the ranks normalise independently: a rank given a different track must fail here, not write a wrong mask
+            dist = self.runner.dist
             pk = torch.tensor([peak, -peak], dtype=torch.float32, device=self.device)
-            self.dist.all_reduce(pk, op=self.dist.ReduceOp.MAX, group=self.runner.group)
+            dist.all_reduce(pk, op=dist.ReduceOp.MAX, group=self.runner.group)
             if float(pk[0]) != peak or float(pk[1]) != -peak:
                 raise RuntimeError(f"VREngine: the ranks disagree on the normalisation peak ({peak} here, {-float(pk[1])}..{float(pk[0])} over the group): "
                                    "every rank must be given the same track")
@@ -562,11 +560,6 @@ class VREngine:
         patches = (n_pad - 2 * off) // roi
         if patches <= 0 or self.window_size - 2 * off <= 0:
             raise ValueError("Window size error: h1_shape[3] must be greater than h2_shape[3]")
-        if self.dist is None:
-            mask = _new((2, nb, patches * roi), mag)
-            self._predict(mag, 0, patches, roi, mask)
-            return mask
-        from .sharded import shard_patches
 
         def predict(p0, p1):
             part = _new((2, nb, (p1 - p0) * roi), mag)

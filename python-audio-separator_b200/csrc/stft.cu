@@ -557,16 +557,8 @@ extern "C" int b200sep_demix_overlap_add_range(const float* chunks, int first_ch
 extern "C" int b200sep_demix_overlap_add(const float* chunks, int n_chunks, int chunk_len, int64_t step, int64_t total_len, int64_t trim,
                                          int64_t n_out, int use_window, float out_scale, const float* mix, float compensate,
                                          int interleave, float* primary, float* secondary, void* stream) {
-  B2_CHECK_ARG(chunks && primary, "demix_overlap_add: NULL argument");
-  B2_CHECK_ARG(mix == nullptr || secondary != nullptr, "demix_overlap_add: mix given without a secondary buffer");
-  B2_CHECK_ARG(n_chunks >= 1 && chunk_len >= 1 && step >= 1 && total_len >= 1 && trim >= 0 && n_out >= 0, "demix_overlap_add: bad sizes");
-  B2_CHECK_ARG(trim + n_out <= total_len, "demix_overlap_add: trim+n_out exceeds total_len");
-  if (n_out == 0) return B200SEP_OK;
-  const int blocks = (int)std::min<int64_t>(cdiv(n_out, 256), kNumSMs * 16);
-  demix_ola_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(chunks, 0, n_chunks, chunk_len, step, total_len, trim, n_out, 0, n_out, use_window, out_scale,
-                                                             mix, n_out, 0, compensate, interleave, primary, secondary, 0, n_out);
-  B2_LAUNCHED();
-  return B200SEP_OK;
+  return b200sep_demix_overlap_add_range_ex(chunks, 0, n_chunks, n_chunks, chunk_len, step, total_len, trim, n_out, 0, n_out, use_window, out_scale, mix, n_out, 0,
+                                            compensate, interleave, primary, secondary, 0, stream);
 }
 
 extern "C" int b200sep_rect_overlap_add_range(const float* chunks, int first_chunk, int n_local, int n_chunks, int channels, int chunk_len, int64_t hop, int64_t front,

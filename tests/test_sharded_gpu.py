@@ -1,8 +1,9 @@
-"""GPU: the time-sharded engines (audio_separator/separator/b200/sharded.py and the `dist=` paths of MdxcEngine / DemucsEngine) through NCCL.
+"""GPU: the time-sharded engines (the `dist=` paths of MdxEngine / MdxcEngine / DemucsEngine over audio_separator/separator/b200/sharded.py) through NCCL.
 
-World size 1 (always runs on the one-GPU box): the sharded code path -- slice of the padded mixture, ShardRunner, ranged overlap-add with slice
-outputs, the shared-host-buffer end-to-end entry -- must reproduce the plain engines bit for bit.  World size 2 (skipped unless two GPUs are
-visible, `gpurun --gpus 2`): two processes, halo exchange + gather over NVLink, compared with the single-GPU result inside rank 0."""
+World size 1 (runs on any one GPU): the sharded code path -- slice of the padded mixture, ShardRunner, ranged overlap-add with slice
+outputs, the shared-host-buffer end-to-end entry -- must reproduce the single-GPU results bit for bit (for MDX: the whole-grid path written out
+below, for MDX23C / Demucs: the engines without `dist`).  World size 2 (skipped unless two GPUs are
+visible): two processes, halo exchange + gather over NVLink, compared with the single-GPU result inside rank 0."""
 import os
 import socket
 
@@ -23,14 +24,35 @@ def _free_port():
         return s.getsockname()[1]
 
 
-def _mdx_pair(cfg, batch, sharded_cls, precision=1):
+def _mdx_engine(cfg, batch, dist, precision=1):
     from audio_separator.separator.b200 import engine, mdx_weights
 
     w = O.make_convtdfnet_weights(cfg, seed=3, out_gain=0.05)
     hp = mdx_weights.infer_hparams_from_state(w)
     net = engine.MdxNet(mdx_weights.flatten_state(w, **hp), dim_t=cfg.dim_t, max_batch=batch, precision=precision, **hp)
-    args = (net, cfg.n_fft, cfg.hop_length, cfg.dim_f, cfg.segment_size, cfg.overlap, cfg.compensate)
-    return engine.MdxEngine(*args, batch_size=batch), sharded_cls(*args, batch_size=batch)
+    return engine.MdxEngine(net, cfg.n_fft, cfg.hop_length, cfg.dim_f, cfg.segment_size, cfg.overlap, cfg.compensate, batch_size=batch, dist=dist)
+
+
+def _mdx_single_gpu(e, mix, normalization_threshold, amplification_threshold):
+    """MdxEngine.separate_device the single-GPU way: peak-normalise, pad the whole mixture, run_model on every chunk, then one whole-grid
+    b200sep_demix_overlap_add with mix and secondary, interleaved -> (primary (N, 2), secondary (N, 2))."""
+    from audio_separator.separator.b200._lib import check, lib
+    from audio_separator.separator.b200.engine import _stream
+
+    N = mix.shape[1]
+    peak = torch.empty(1, device=mix.device)
+    check(lib.b200sep_absmax(mix.data_ptr(), mix.numel(), peak.data_ptr(), _stream()), "absmax")
+    mixn = torch.empty_like(mix)
+    check(lib.b200sep_normalize(mix.data_ptr(), mix.numel(), peak.data_ptr(), normalization_threshold, amplification_threshold, mixn.data_ptr(), _stream()), "normalize")
+    L, step, n_chunks, overlap = e.grid(N)
+    T = e.chunk_size
+    mixture = torch.zeros((2, (n_chunks - 1) * step + T), device=mix.device)  # [0]*trim + mix + [0]*pad, and zeros past L for the last chunks
+    mixture[:, e.trim : e.trim + N] = mixn
+    chunks = e.run_model(mixture.unfold(1, T, step).transpose(0, 1).contiguous())
+    primary, secondary = torch.empty((N, 2), device=mix.device), torch.empty((N, 2), device=mix.device)
+    check(lib.b200sep_demix_overlap_add(chunks.data_ptr(), n_chunks, T, step, L, e.trim, N, int(overlap != 0), float(peak.item()), mixn.data_ptr(), e.compensate, 1,
+                                        primary.data_ptr(), secondary.data_ptr(), _stream()), "demix_overlap_add")
+    return primary, secondary
 
 
 def _demucs_small():
@@ -58,21 +80,20 @@ def _mdxc_small():
 def _check_all(rank, world, results):
     """Runs on every rank of an initialised nccl group; rank 0 appends (name, bit_identical, max_abs_diff)."""
     import torch.distributed as dist
-    from audio_separator.separator.b200.sharded import ShardedMdxEngine
 
     dev = torch.device("cuda", torch.cuda.current_device())
     # ---- MDX: device-resident and shared-host-buffer entries
     cfg = O.MDXConfig(**SMALL)
     n = 9 * cfg.chunk_size // 2 + 321
     mix = torch.from_numpy(O.synth_music(n, seed=2)).to(dev)
-    single, sharded = _mdx_pair(cfg, 2, ShardedMdxEngine)
+    sharded = _mdx_engine(cfg, 2, dist)
     got = sharded.separate_device(mix, 0.9, 0.0)
     if world == 1:
         mh = torch.from_numpy(O.synth_music(n, seed=2)).pin_memory()
         outs = [torch.empty((n, 2)).pin_memory() for _ in range(2)]
         sharded.separate_host(mh, outs[0], outs[1], 0.9, 0.0)
     if rank == 0:
-        ref = single.separate_device(mix, 0.9, 0.0)
+        ref = _mdx_single_gpu(sharded, mix, 0.9, 0.0)
         for name, g, r in (("mdx primary", got[0], ref[0]), ("mdx secondary", got[1], ref[1])):
             results.append((name, bool(torch.equal(g, r)), float((g - r).abs().max())))
         if world == 1:
@@ -134,14 +155,14 @@ def _run(world):
 
 
 @pytest.mark.timeout(900)
-def test_sharded_engines_world1_equal_plain_engines(lib_built):
+def test_dist_engines_world1_equal_single_gpu_path(lib_built):
     for name, same, diff in _run(1):
         assert same and diff == 0.0, (name, diff)
 
 
 @pytest.mark.timeout(900)
 @pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs two GPUs")
-def test_sharded_engines_world2_equal_single_gpu(lib_built):
+def test_dist_engines_world2_equal_single_gpu_path(lib_built):
     for name, same, diff in _run(2):
         # per-sample arithmetic is the single-GPU arithmetic (same contributions, same order).  The ranks batch their segments differently from the
         # single-GPU run; every reduction inside a forward is partitioned independently of the batch size (GroupNorm since round 2), so the Demucs

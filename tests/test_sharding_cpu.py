@@ -1,6 +1,6 @@
 """CPU (gloo, world_size 2 and 3): the time-sharding control flow of audio_separator/separator/b200/sharded.py.
 
-The sharded engines (ShardedMdxEngine, MdxcEngine, DemucsEngine) all run `ShardRunner.run_units` (unit order, balanced batches, halo
+The chunked engines (MdxEngine, MdxcEngine, DemucsEngine) all run `ShardRunner.run_units` (unit order, balanced batches, halo
 isend/irecv), an overlap-add of their own output range, and `gather_rows` / `gather_cols`.  These tests execute exactly that code over gloo
 with the per-unit compute and the range overlap-add injected as numpy restatements of the kernels (the kernels themselves are parity-tested
 on the GPU): the sharded result must equal the single-process oracle sample for sample."""
