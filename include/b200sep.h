@@ -127,6 +127,20 @@ int b200sep_to_pcm16(const float* x, int64_t n, int16_t* y, void* stream);
 int b200sep_to_pcm_bytes(const float* x, int64_t n, int bits, int via_int16, uint8_t* y, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------
+ * FLAC frames (RFC 9639) of a normalised stereo stem: the `.flac` output of write_audio (common_separator.py:302-451) without a CPU encoder.
+ * x: (n_samples, 2) interleaved float32, 8-byte aligned.  Each sample is quantised exactly as b200sep_to_pcm_bytes(x, ., bits, via_int16) does and
+ * shifted right by bits - stream_bps (stream_bps 16 or 24, <= bits), so the decoded stream holds the WAV writer's samples.  Fixed block size 4096
+ * (the last block may be shorter), frame numbers from 0; the caller writes "fLaC" + STREAMINFO in front of the frames.
+ *   work:   b200sep_flac_work_bytes(n_samples) bytes of 8-byte aligned device scratch (per-frame plans and offsets);
+ *   out:    b200sep_flac_max_bytes(n_samples, stream_bps) bytes: every frame is at most its VERBATIM coding, so this bound cannot overflow;
+ *   result: device int64[4] = {total frame bytes, min frame bytes, max frame bytes, frames whose packed size differs from the planned size (0)}.
+ * The output is deterministic byte for byte.  Both queries return -1 for bad arguments. */
+int64_t b200sep_flac_work_bytes(int64_t n_samples);
+int64_t b200sep_flac_max_bytes(int64_t n_samples, int stream_bps);
+int b200sep_flac_encode(const float* x, int64_t n_samples, int bits, int via_int16, int stream_bps, int sample_rate, void* work, uint8_t* out,
+                        int64_t* result, void* stream);
+
+/* ---------------------------------------------------------------------------------------------------
  * ConvTDFNet (the graph inside UVR-MDX-NET-*.onnx; topology: uvr_lib_v5/mdxnet.py:30-120, modules.py:1-74).
  * Replaces `self.model_run(spek)` = ort.InferenceSession.run (architectures/mdx_separator.py:122-123, :443).
  *

@@ -50,6 +50,9 @@ _SIGS = {
     "b200sep_normalize": (i32, [vp, i64, vp, f32, f32, vp, vp]),
     "b200sep_to_pcm16": (i32, [vp, i64, vp, vp]),
     "b200sep_to_pcm_bytes": (i32, [vp, i64, i32, i32, vp, vp]),
+    "b200sep_flac_work_bytes": (i64, [i64]),
+    "b200sep_flac_max_bytes": (i64, [i64, i32]),
+    "b200sep_flac_encode": (i32, [vp, i64, i32, i32, i32, i32, vp, vp, vp, vp]),
     "b200sep_mdxnet_param_count": (i64, [C.POINTER(MdxNetConfig)]),
     "b200sep_mdxnet_create": (i32, [C.POINTER(vp), C.POINTER(MdxNetConfig), vp, i64]),
     "b200sep_mdxnet_destroy": (None, [vp]),

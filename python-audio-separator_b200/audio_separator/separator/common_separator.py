@@ -2,9 +2,10 @@
 
 Mirrors what `Separator` and the plugins rely on from the reference's CommonSeparator
 (audio_separator/separator/common_separator.py:57-157 config/stem naming, :217-282 prepare_mix,
-:284-451 write_audio, :453-507 cache + output paths).  Audio decode/encode is NOT part of the accelerated
+:284-451 write_audio, :453-507 cache + output paths).  Audio decode is NOT part of the accelerated
 path (SURVEY.md section 2, row 2): WAV goes through the stdlib `wave` module, anything else through
-soundfile/librosa when those wheels are installed.
+soundfile/librosa when those wheels are installed.  Output: WAV through `wave`, FLAC encoded on the GPU
+(b200/flac.py), anything else through soundfile.
 """
 import gc
 import os
@@ -164,6 +165,25 @@ class CommonSeparator:
             return None
         return np.ascontiguousarray((s * 32767).astype(np.int16)).reshape(-1)
 
+    def _normalized_on_device(self, stem):
+        """spec_utils.normalize of a CUDA stem with the b200sep_absmax / _normalize kernels; None (with the reference's warning) for a near-silent stem."""
+        from .b200._lib import check, lib
+
+        x = stem.contiguous()
+        n = x.numel()
+        st = torch.cuda.current_stream().cuda_stream
+        peak = torch.empty(1, dtype=torch.float32, device=x.device)
+        check(lib.b200sep_absmax(x.data_ptr(), n, peak.data_ptr(), st), "absmax")
+        norm = torch.empty_like(x)
+        min_peak = -1.0 if self.amplification_threshold is None else float(self.amplification_threshold)
+        check(lib.b200sep_normalize(x.data_ptr(), n, peak.data_ptr(), float(self.normalization_threshold), min_peak, norm.data_ptr(), st), "normalize")
+        pk = float(peak.item())
+        scale = self.normalization_threshold / pk if pk > self.normalization_threshold else (min_peak / pk if (min_peak >= 0 and 0 < pk < min_peak) else 1.0)
+        if pk * scale < 1e-6:
+            self.logger.warning("Warning: stem_source array is near-silent or empty.")
+            return None
+        return norm
+
     def pcm_bytes(self, stem_source):
         """(N, 2) float stem -> (bits, interleaved little-endian PCM bytes) at the input's bit depth, or None for a near-silent stem.
         A CUDA tensor never leaves the device as floats: peak, normalisation, quantisation and byte packing are kernels (b200sep_absmax / _normalize /
@@ -173,21 +193,12 @@ class CommonSeparator:
         if isinstance(stem_source, torch.Tensor) and stem_source.is_cuda:
             from .b200._lib import check, lib
 
-            x = stem_source.contiguous()
-            n = x.numel()
-            st = torch.cuda.current_stream().cuda_stream
-            peak = torch.empty(1, dtype=torch.float32, device=x.device)
-            check(lib.b200sep_absmax(x.data_ptr(), n, peak.data_ptr(), st), "absmax")
-            norm = torch.empty_like(x)
-            min_peak = -1.0 if self.amplification_threshold is None else float(self.amplification_threshold)
-            check(lib.b200sep_normalize(x.data_ptr(), n, peak.data_ptr(), float(self.normalization_threshold), min_peak, norm.data_ptr(), st), "normalize")
-            out = torch.empty(n * bits // 8, dtype=torch.uint8, device=x.device)
-            check(lib.b200sep_to_pcm_bytes(norm.data_ptr(), n, bits, int(via16), out.data_ptr(), st), "to_pcm_bytes")
-            pk = float(peak.item())
-            scale = self.normalization_threshold / pk if pk > self.normalization_threshold else (min_peak / pk if (min_peak >= 0 and 0 < pk < min_peak) else 1.0)
-            if pk * scale < 1e-6:
-                self.logger.warning("Warning: stem_source array is near-silent or empty.")
+            norm = self._normalized_on_device(stem_source)
+            if norm is None:
                 return None
+            n = norm.numel()
+            out = torch.empty(n * bits // 8, dtype=torch.uint8, device=norm.device)
+            check(lib.b200sep_to_pcm_bytes(norm.data_ptr(), n, bits, int(via16), out.data_ptr(), torch.cuda.current_stream().cuda_stream), "to_pcm_bytes")
             return bits, out.cpu().numpy().tobytes()
         if isinstance(stem_source, np.ndarray) and stem_source.dtype == np.int16:
             q = stem_source.reshape(-1).astype(np.int64)
@@ -213,7 +224,33 @@ class CommonSeparator:
         b4 = q.astype("<i4").view(np.uint8).reshape(-1, 4)
         return bits, np.ascontiguousarray(b4[:, :3]).tobytes()
 
+    def write_flac(self, stem_path, stem_source):
+        """`.flac` output encoded on the GPU (b200/flac.py).  A CUDA stem never leaves the device as PCM; a host array is uploaded first.  The stored
+        samples are the WAV writer's at the input bit depth, at the stream sample size of the reference's writer (flac.stream_bps)."""
+        from .b200 import flac
+
+        if isinstance(stem_source, np.ndarray) and stem_source.dtype == np.int16:
+            raise TypeError("FLAC output takes float stems")
+        if not (isinstance(stem_source, torch.Tensor) and stem_source.is_cuda):
+            stem_source = torch.as_tensor(np.ascontiguousarray(stem_source, dtype=np.float32), device="cuda")
+        norm = self._normalized_on_device(stem_source.float())
+        if norm is None:
+            return
+        bits = self._output_bits()
+        bps = flac.stream_bps(bits, bool(self.use_soundfile))
+        if self.output_dir:
+            os.makedirs(self.output_dir, exist_ok=True)
+            stem_path = os.path.join(self.output_dir, stem_path)
+        if bps is None:
+            self.logger.error(f"Error exporting audio file: libsndfile has no {bits}-bit FLAC subtype, {stem_path} not written")
+            return
+        data = flac.encode(norm, bits, not self.use_soundfile, bps, int(self.sample_rate))
+        with open(stem_path, "wb") as f:
+            f.write(data)
+
     def write_audio(self, stem_path, stem_source):
+        if stem_path.lower().endswith(".flac"):
+            return self.write_flac(stem_path, stem_source)
         packed = self.pcm_bytes(stem_source)
         if packed is None:
             return

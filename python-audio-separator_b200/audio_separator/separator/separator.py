@@ -175,6 +175,9 @@ class Separator:
                     self.load_model(model_filename)
                     self.output_dir = temp_dir
                     self.model_instance.output_dir = temp_dir
+                    if self.output_format.lower() == "flac":
+                        # lossless either way: WAV intermediates hold the samples the reference's FLAC round trip holds, and need no FLAC reader
+                        self.model_instance.output_format = "WAV"
                     try:
                         model_stems = self._separate_file(path, None)  # default "base_(Stem)_model.ext" names: the stem type is parsed from them
                     finally:

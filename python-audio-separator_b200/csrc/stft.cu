@@ -9,6 +9,7 @@
 
 #include "common.cuh"
 #include "internal.h"
+#include "pcm.cuh"
 
 namespace b200sep {
 
@@ -350,22 +351,11 @@ __global__ void pcm16_kernel(const float* __restrict__ x, int64_t n, int16_t* __
   }
 }
 
-// PCM bytes (little endian) at the input file's bit depth (common_separator.py:322-383).  via_int16 = the pydub writer: samples are quantised to int16
-// first ((x * 32767).astype(int16)) and ffmpeg widens them (s16 -> s32 = << 16; pcm_s24le keeps the top three bytes).  Otherwise the libsndfile
-// writer: lrint(x * (2^(bits-1) - 1)) (PCM_32 scales by 2^31 and saturates).
+// PCM bytes (little endian) at the input file's bit depth; the quantisation rules are pcm_quantize's (pcm.cuh).
 __global__ void pcm_bytes_kernel(const float* __restrict__ x, int64_t n, int bits, int via_int16, uint8_t* __restrict__ y) {
   const int width = bits >> 3;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
-    int v;
-    if (via_int16) {
-      v = (int)(int16_t)(int)__fmul_rn(x[i], 32767.f);
-      v = (int)((unsigned)v << (bits - 16));
-    } else if (bits == 32) {
-      const double d = rint((double)x[i] * 2147483648.0);
-      v = d >= 2147483647.0 ? 2147483647 : (d <= -2147483648.0 ? (int)0x80000000 : (int)d);
-    } else {
-      v = (int)rintf(__fmul_rn(x[i], (float)((1 << (bits - 1)) - 1)));
-    }
+    const int v = pcm_quantize(x[i], bits, via_int16);
     uint8_t* o = y + i * width;
     for (int b = 0; b < width; ++b) o[b] = (uint8_t)((unsigned)v >> (8 * b));
   }
