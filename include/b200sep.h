@@ -141,6 +141,34 @@ int b200sep_flac_encode(const float* x, int64_t n_samples, int bits, int via_int
                         int64_t* result, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------
+ * FLAC decoding (RFC 9639): the frames of a stream (everything after the metadata, without a trailing ID3v1 tag) -> the planar float mix that
+ * prepare_mix returns, mix[c, n] = sample[n, c] * 2^-(bps-1), for the first min(channels, 2) channels.  Two calls with one host read between them:
+ *   b200sep_flac_locate  finds the frames: every byte position that starts a frame header agreeing with STREAMINFO and carrying a matching CRC-8 is
+ *                        a candidate; a candidate's successor is the nearest later candidate (or the end of the data) whose frame or sample number
+ *                        follows and for which the CRC-16 of the bytes in between is zero; the frames are the chain of successors from offset 0.
+ *   b200sep_flac_decode  decodes every frame (one CTA per frame) straight into out; the parsed end of each frame must be its chain boundary.
+ * frames:   device bytes, 16-byte aligned and readable up to n_bytes rounded up to a multiple of 16 (n_bytes < 2^31).
+ * stream:   STREAMINFO sample rate, sample size (4-24 bits), channel count (1-8), and the blocking-strategy bit of the first frame header (0 fixed,
+ *           1 variable).
+ * work:     b200sep_flac_decode_work_bytes(n_bytes) bytes of 8-byte aligned device scratch, passed unchanged from locate to decode.
+ * result:   device int64[8] = {frames, samples, error code, error frame index, error byte offset in frames, largest frame in bytes, first coded frame
+ *           or sample number, 0}.  locate clears it; decode only adds an error.  Pass result[0] and result[5] to decode.
+ * out:      rows min(channels, 2) of out_ld >= result[1] floats.
+ * A malformed stream is an input error reported in result[2..4], never a device fault: every read is bounded by n_bytes and no state outlives a
+ * call.  The CRC-16 of every frame is checked; the STREAMINFO MD5 is not. */
+#define B200SEP_FLAC_OK 0
+#define B200SEP_FLAC_ERR_SYNC 1      /* no valid frame header (sync, codes, CRC-8) at the offset where a frame must start */
+#define B200SEP_FLAC_ERR_CRC 2       /* no later candidate or end of data closes the frame with a zero CRC-16 residue: damaged or truncated */
+#define B200SEP_FLAC_ERR_NUMBER 3    /* the frame or sample numbers do not follow the running sample count */
+#define B200SEP_FLAC_ERR_SUBFRAME 4  /* a reserved or invalid subframe, predictor or residual code */
+#define B200SEP_FLAC_ERR_LENGTH 5    /* the subframes end somewhere else than the frame's CRC-16, or a residual runs past it */
+int64_t b200sep_flac_decode_work_bytes(int64_t n_bytes);
+int b200sep_flac_locate(const uint8_t* frames, int64_t n_bytes, int sample_rate, int bps, int channels, int variable_blocking, void* work,
+                        int64_t* result, void* stream);
+int b200sep_flac_decode(const uint8_t* frames, int64_t n_bytes, void* work, int64_t n_frames, int64_t max_frame_bytes, float* out,
+                        int64_t out_ld, int64_t* result, void* stream);
+
+/* ---------------------------------------------------------------------------------------------------
  * ConvTDFNet (the graph inside UVR-MDX-NET-*.onnx; topology: uvr_lib_v5/mdxnet.py:30-120, modules.py:1-74).
  * Replaces `self.model_run(spek)` = ort.InferenceSession.run (architectures/mdx_separator.py:122-123, :443).
  *

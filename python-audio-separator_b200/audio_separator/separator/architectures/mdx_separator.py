@@ -137,7 +137,10 @@ class MDXSeparator(CommonSeparator):
             raise NotImplementedError("invert_using_spec=True (spec_utils.invert_stem) is not part of the accelerated path yet")
         # device-resident output pipeline: the float stems stay in HBM; write_audio pulls bits/8 bytes per sample (normalise, quantise and pack are kernels)
         self.initialize_model_settings()
-        mix_dev = torch.from_numpy(np.ascontiguousarray(mix, dtype=np.float32)).to(self.torch_device)
+        if isinstance(mix, DeviceStem):  # decoded on the GPU (FLAC input): the mix never visits the host
+            mix_dev = mix.tensor.to(self.torch_device)
+        else:
+            mix_dev = torch.from_numpy(np.ascontiguousarray(mix, dtype=np.float32)).to(self.torch_device)
         primary_dev, secondary_dev = self.engine.separate_device(mix_dev, self.normalization_threshold, self.amplification_threshold)
         if not isinstance(self.primary_source, np.ndarray):
             self.primary_source = DeviceStem(primary_dev)

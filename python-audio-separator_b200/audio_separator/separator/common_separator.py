@@ -3,8 +3,8 @@
 Mirrors what `Separator` and the plugins rely on from the reference's CommonSeparator
 (audio_separator/separator/common_separator.py:57-157 config/stem naming, :217-282 prepare_mix,
 :284-451 write_audio, :453-507 cache + output paths).  Audio decode is NOT part of the accelerated
-path (SURVEY.md section 2, row 2): WAV goes through the stdlib `wave` module, anything else through
-soundfile/librosa when those wheels are installed.  Output: WAV through `wave`, FLAC encoded on the GPU
+path (SURVEY.md section 2, row 2): WAV goes through the stdlib `wave` module, FLAC (recognised by content) is
+decoded on the GPU (b200/flac.py) into a DeviceStem, anything else goes through soundfile/librosa when those wheels are installed.  Output: WAV through `wave`, FLAC encoded on the GPU
 (b200/flac.py), anything else through soundfile.
 """
 import gc
@@ -114,14 +114,50 @@ class CommonSeparator:
             data = mix.T
         else:
             data = self._read_audio(mix)
+            if isinstance(data, torch.Tensor):
+                return self._device_mix(mix, data)
             if not np.any(data):
                 raise ValueError(f"Audio file {mix} is empty or not valid")
         if data.ndim == 1:
             data = np.asfortranarray([data, data])
         return data
 
+    def _device_mix(self, path, data):
+        """A decoded (C, N) CUDA mix -> DeviceStem of (2, N): the "empty or not valid" check by the b200sep_absmax kernel, mono as two equal rows."""
+        from .b200._lib import check, lib
+
+        peak = torch.empty(1, dtype=torch.float32, device=data.device)
+        check(lib.b200sep_absmax(data.data_ptr(), data.numel(), peak.data_ptr(), torch.cuda.current_stream(data.device).cuda_stream), "absmax")
+        if data.numel() == 0 or float(peak.item()) == 0.0:
+            raise ValueError(f"Audio file {path} is empty or not valid")
+        if data.shape[0] == 1:
+            data = data.expand(2, -1).contiguous()
+        return DeviceStem(data)
+
+    def _read_flac(self, path):
+        """FLAC decoded on the GPU (b200/flac.py): (C, N) float32 CUDA tensor, C = min(channels, 2)."""
+        from .b200 import flac
+
+        with open(path, "rb") as f:
+            data = f.read()
+        info, _, _ = flac.parse(data)
+        if info["sample_rate"] != self.sample_rate:
+            return None
+        depth, subtype = flac.input_bit_depth(info["bps"]) if info["bps"] <= 24 else (None, None)
+        mix, info = flac.decode(data, self.torch_device if self.torch_device is not None and self.torch_device.type == "cuda" else "cuda")
+        if info["total_samples"] and info["total_samples"] != info["n_samples"]:
+            self.logger.warning(f"{path}: STREAMINFO gives {info['total_samples']} samples, the frames hold {info['n_samples']}")
+        self.input_bit_depth, self.input_subtype = depth, subtype
+        return mix
+
     def _read_audio(self, path):
-        if path.lower().endswith(".wav"):
+        from .b200 import flac
+
+        if flac.is_flac(path):
+            mix = self._read_flac(path)
+            if mix is not None:
+                return mix
+        elif path.lower().endswith(".wav"):
             try:
                 with _wave.open(path, "rb") as wf:
                     ch, width, sr, n = wf.getnchannels(), wf.getsampwidth(), wf.getframerate(), wf.getnframes()

@@ -14,10 +14,15 @@
 #include <math.h>
 
 #include "common.cuh"
+#include "flac_common.cuh"
 #include "pcm.cuh"
 
 namespace b200sep {
 namespace {
+
+using flac::crc8;
+using flac::gf2_mulmod16;
+using flac::x8_pow_mod16;
 
 constexpr int kBlock = 4096;
 constexpr int kThreads = 256;
@@ -120,16 +125,6 @@ __device__ __forceinline__ long long residual_at(const int* s, int i, int type, 
   long long p = 0;
   for (int j = 0; j < order; ++j) p += (long long)coef[j] * s[i - 1 - j];
   return (long long)s[i] - (p >> shift);
-}
-
-__device__ uint8_t crc8(const uint8_t* p, int n) {
-  unsigned c = 0;
-  for (int i = 0; i < n; ++i) {
-    c ^= p[i];
-    for (int b = 0; b < 8; ++b) c = (c & 0x80) ? ((c << 1) ^ 0x07) : (c << 1);
-    c &= 0xFF;
-  }
-  return (uint8_t)c;
 }
 
 // Frame header with its CRC-8 -> h (kHeaderMax bytes); returns its length.
@@ -523,23 +518,6 @@ __device__ unsigned item_bits(PackSmem& sm, int c, int i, int bs, unsigned pos) 
   return len;
 }
 
-__device__ __forceinline__ unsigned gf2_mulmod16(unsigned a, unsigned b) {  // a * b mod x^16 + x^15 + x^2 + 1
-  unsigned r = 0;
-  for (int i = 15; i >= 0; --i) {
-    r <<= 1;
-    if (r & 0x10000u) r ^= 0x18005u;
-    if ((b >> i) & 1u) r ^= a;
-  }
-  return r;
-}
-__device__ unsigned x8_pow_mod16(unsigned n) {  // x^(8n) mod the CRC-16 polynomial
-  unsigned r = 1, b = 0x100;
-  for (; n; n >>= 1) {
-    if (n & 1u) r = gf2_mulmod16(r, b);
-    b = gf2_mulmod16(b, b);
-  }
-  return r;
-}
 __device__ __forceinline__ unsigned frame_byte(const unsigned* buf, int b) { return (buf[b >> 2] >> (24 - 8 * (b & 3))) & 0xFFu; }
 
 __global__ void __launch_bounds__(kThreads) flac_pack_kernel(const float* __restrict__ x, int64_t n, int bits, int via_int16, int sbps, int sr_code,
@@ -558,11 +536,7 @@ __global__ void __launch_bounds__(kThreads) flac_pack_kernel(const float* __rest
     int* dst = reinterpret_cast<int*>(&sm.sub[c]);
     for (int i = t; i < (int)(sizeof(Sub) / 4); i += kThreads) dst[i] = src[i];
   }
-  {
-    unsigned c = (unsigned)t << 8;
-    for (int b = 0; b < 8; ++b) c = (c & 0x8000u) ? ((c << 1) ^ 0x8005u) : (c << 1);
-    sm.crc_tab[t] = (uint16_t)c;
-  }
+  sm.crc_tab[t] = flac::crc16_table_entry((unsigned)t);
   const int a = P.assign == 1 ? 0 : P.assign - 7;
   const int ch0 = sub_channel(a, 0), ch1 = sub_channel(a, 1);
   __syncthreads();
