@@ -412,6 +412,13 @@ int b200sep_vr_mirror_high_end(const float* spec_m, int bins, const float* high_
  * y[c][k] = sum_i x[c][i] * taps[(k + n_pre_remove)*down - i*up];  taps = the zero-padded FIR scaled by `up` */
 int b200sep_resample_poly_f32(const float* x, const float* taps, int n_taps, int up, int down, int64_t n_pre_remove, int channels, int64_t n_in,
                               int64_t n_out, float* y, void* stream);
+/* Band-limited resampling at any ratio (stand-in for librosa.resample's soxr / libsamplerate / resampy backends):
+ *   y[c][n] = g * sum_k x[c][k] * h(g * |n*step - k|),  step = 1.0 / ratio (double),  g = min(1, ratio),
+ * where h is the Kaiser-windowed sinc tabulated at `per_zero` points per zero crossing over [0, n_zeros] (table[n_zeros*per_zero] is the
+ * last entry), linearly interpolated; x is zero outside [0, n_in).  x (channels, n_in) -> y (channels, n_out), both contiguous.
+ * ratio must lie in [1/16, 16] (B200SEP_ERR_ARG otherwise). */
+int b200sep_resample_sinc_f32(const float* x, int channels, int64_t n_in, const float* table, int n_zeros, int per_zero, double ratio,
+                              int64_t n_out, float* y, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------
  * Operators of the BS-Roformer path (uvr_lib_v5/roformer/bs_roformer.py, attend.py; mdxc_separator.py:272-343).

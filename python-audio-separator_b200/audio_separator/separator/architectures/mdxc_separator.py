@@ -4,7 +4,12 @@ Plugin contract of the reference's MDXCSeparator (audio_separator/separator/arch
 ctor `(common_config, arch_config)` with arch keys segment_size / override_model_segment_size / batch_size / overlap /
 pitch_shift, `separate(path, custom_output_names)`, `demix(mix) -> {instrument: (2, N)}`.  The chunk loop runs on the GPU
 through libb200sep.so (MdxcEngine for TFC_TDF_net checkpoints, RoformerEngine for BS-Roformer and Mel-Band Roformer checkpoints -- the Roformer branch of
-demix, mdxc_separator.py:272-343).  Pitch shifting is not part of this path.
+demix, mdxc_separator.py:272-343).
+
+arch key `pitch_shift` (semitones, both model families): demix resamples the mix on the GPU from sr to sr * 2**(-s/12), runs the engine on
+the result, resamples every stem back by 2**(s/12) and fits it to the mix length (spec_utils.change_pitch_semitones + match_array_shapes,
+mdxc_separator.py:230-244, :268-270).  The resampler is b200/resample.py's res_type "sinc_fastest", the reference's choice on Linux
+(spec_utils.py:33-37); its choice on macOS / ARM (kaiser_best) is not mirrored.
 
 arch key `b200_sharded` (both model families): one process per GPU under an initialised torch.distributed group (nccl); every rank calls
 `separate(path)` on the same file, each track is split by time over the ranks (b200/sharded.py), and rank 0 writes the stem files and returns
@@ -16,8 +21,11 @@ import numpy as np
 import torch
 
 from ..b200.engine import MdxcEngine, TfcNet
+from ..b200.resample import match_length, resample
 from ..b200.roformer import BSRoformerConfig, BSRoformerNet, MelBandRoformerConfig, RoformerEngine
 from ..common_separator import CommonSeparator, normalize, tensor_core_math
+
+PITCH_RES_TYPE = "sinc_fastest"  # spec_utils.wav_resolution_float_resampling on Linux
 
 
 class MDXCSeparator(CommonSeparator):
@@ -32,8 +40,6 @@ class MDXCSeparator(CommonSeparator):
         self.process_all_stems = arch_config.get("process_all_stems", True)
         self.is_roformer = bool(self.is_roformer_model)
         self.sharded = bool(arch_config.get("b200_sharded", False))  # one process per GPU (torch.distributed, nccl): time-shard every track over the ranks
-        if self.pitch_shift:
-            raise NotImplementedError("pitch_shift is not part of the accelerated path")
         if not torch.cuda.is_available():
             raise RuntimeError("MDXCSeparator (H100 build) needs a CUDA device: there is no CPU path in this package")
         self.dist = None
@@ -107,10 +113,20 @@ class MDXCSeparator(CommonSeparator):
 
     def _demix_stems(self, orig):
         """(2, N) float32 ndarray -> (n_out, 2, N) ndarray.  Sharded: every rank runs its part of the chunk grid, rank 0 gathers and gets the
-        stems, the other ranks get None."""
-        part = self.engine.demix_device(torch.as_tensor(orig).to(self.torch_device))
-        full = self.engine.gather(part, orig.shape[1])
-        return None if full is None else full.cpu().numpy()
+        stems, the other ranks get None.  With pitch_shift every rank pitches the whole mix (the resampler is deterministic), the engine runs
+        on the pitched length, and rank 0 pitches every stem back and fits it to N (pitch_fix, :230-244)."""
+        mix = torch.as_tensor(orig).to(self.torch_device)
+        if self.pitch_shift:
+            sr_pitched = self.sample_rate * 2 ** (-self.pitch_shift / 12)  # change_pitch_semitones(mix, sr, -pitch_shift) (:268-270)
+            mix = resample(mix, self.sample_rate, sr_pitched, PITCH_RES_TYPE)
+        part = self.engine.demix_device(mix)
+        full = self.engine.gather(part, mix.shape[1])
+        if full is None:
+            return None
+        if self.pitch_shift:
+            sr_back = sr_pitched * 2 ** (self.pitch_shift / 12)
+            full = torch.stack([match_length(resample(stem, sr_pitched, sr_back, PITCH_RES_TYPE), orig.shape[1]) for stem in full])
+        return full.cpu().numpy()
 
     def _demix_roformer(self, mix):
         """Roformer branch of demix + the stem dictionary (mdxc_separator.py:272-343, :406-468)."""

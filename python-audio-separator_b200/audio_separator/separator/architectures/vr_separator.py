@@ -49,8 +49,6 @@ class VRSeparator(CommonSeparator):
             self.dist = dist
         self.torch_device = torch.device("cuda", torch.cuda.current_device())
         self.model_samplerate = self.model_params["sr"]
-        if self.model_samplerate != 44100:
-            raise NotImplementedError("VR models whose output must be resampled to 44100 Hz are not covered")
         self.load_model()
 
     def load_model(self):
@@ -77,10 +75,11 @@ class VRSeparator(CommonSeparator):
     def separate(self, audio_file_path, custom_output_names=None):
         self.audio_file_path = audio_file_path
         self.audio_file_base = os.path.splitext(os.path.basename(audio_file_path))[0]
-        wave = self.prepare_mix(audio_file_path)  # librosa.load(mono=False, sr=44100) of a 44.1 kHz file (vr_separator.py:271)
+        wave = self.prepare_mix(audio_file_path)  # the file at 44.1 kHz; librosa.load(sr=<top band's rate>) resamples it (vr_separator.py:273)
+        # a model at another rate (e.g. 32 / 48 kHz) gets the mix resampled on the device, and its stems come back at 44.1 kHz (:221-222, :239-240)
         stems = self.engine.separate(np.asarray(wave, dtype=np.float32), enable_tta=bool(self.enable_tta),
                                      post_process_threshold=self.post_process_threshold if self.enable_post_process else None,
-                                     high_end_process=bool(self.high_end_process))
+                                     high_end_process=bool(self.high_end_process), sr=44100)
         output_files = []
         if stems is None:  # sharded, rank != 0: rank 0 holds the stems and writes the files
             return output_files

@@ -1,13 +1,15 @@
 """VR architecture (CascadedASPPNet, "VR arch" v4 / v5.0 models) on the operator kernels of libb200sep.so.
 
 VRNet.predict_mask replaces CascadedASPPNet.predict_mask (uvr_lib_v5/vr_network/nets.py:96-175, layers.py:8-294); VREngine replaces
-VRSeparator.loading_mix / inference_vr / spec_to_wav (architectures/vr_separator.py:255-375) with the multi-band STFT, the polyphase
-band resampling, the patch loop, the mask post-processing and the band synthesis all on the GPU.
+VRSeparator.loading_mix / inference_vr / spec_to_wav (architectures/vr_separator.py:255-375) with the multi-band STFT, the band
+resampling, the patch loop, the mask post-processing and the band synthesis all on the GPU.
 This file is the graph builder: device buffers + launch order.  All arithmetic is behind the C ABI (include/b200sep.h).
 
-VR 5.1 models (nets_new.CascadedNet, LSTM branch) run through VRNet51.  enable_tta, enable_post_process and high_end_process are supported.  Not covered (raises): `reverse` model
-parameters, analysis bands resampled with anything but res_type "polyphase".  The band UP-sampling of the synthesis side uses the
-same Kaiser polyphase design (the reference calls libsamplerate "sinc_fastest" there; see DESIGN.md: parity unpinned for that step).
+VR 5.1 models (nets_new.CascadedNet, LSTM branch) run through VRNet51.  enable_tta, enable_post_process and high_end_process are supported, and so are models whose parameters run at
+another rate than the file's (e.g. 32 / 48 kHz): the mix and the analysis bands are resampled with each band's res_type (b200/resample.py)
+and the stems are resampled back to 44.1 kHz.  Not covered (raises): `reverse` model parameters, a top band whose rate is not the model's, a
+res_type b200/resample.py has no filter for.  The band UP-sampling of the synthesis side uses the Kaiser polyphase design of res_type
+"polyphase" (the reference calls libsamplerate "sinc_fastest" there; see DESIGN.md: parity unpinned for that step).
 
 VREngine(dist=...) splits the patches of one track over the GPUs of a box (b200/sharded.py `plan_patch_shards`): the patches do not overlap, so
 there is no halo; rank 0 gathers the mask and runs the mask post-processing and the synthesis.
@@ -22,6 +24,7 @@ import torch
 from ._lib import LAYOUT_CFT, MATH_BF16X3, check, lib
 from .demucs import ACT_NONE, ACT_RELU, _new, block_conv_weight, conv2d, ew, linear
 from .engine import StftPlan, _ptr, _require_cuda, _stream
+from .resample import resample, resample_poly_design  # noqa: F401  (resample_poly_design: the polyphase FIR, re-exported)
 from .sharded import ShardRunner, shard_patches
 
 ACT_LEAKY, ACT_SIGMOID = 3, 4
@@ -35,23 +38,6 @@ def copy_view(src: torch.Tensor, dst: torch.Tensor):
     assert src.dim() == 4 and tuple(src.shape) == tuple(dst.shape), (src.shape, dst.shape)
     d = src.shape
     check(lib.b200sep_copy4_f32(src.data_ptr(), dst.data_ptr(), d[0], d[1], d[2], d[3], *src.stride(), *dst.stride(), _stream()), "copy4_f32")
-
-
-def resample_poly_design(up: int, down: int):
-    """The FIR scipy.signal.resample_poly designs (window=("kaiser", 5.0)) and the alignment of its output:
-    -> (taps float32 zero-padded in front and scaled by `up`, n_pre_remove)."""
-    g = math.gcd(up, down)
-    up, down = up // g, down // g
-    max_rate = max(up, down)
-    f_c = 1.0 / max_rate
-    half_len = 10 * max_rate
-    n = 2 * half_len + 1
-    m = np.arange(n, dtype=np.float64) - half_len
-    h = f_c * np.sinc(f_c * m) * np.kaiser(n, 5.0)  # firwin: windowed ideal low-pass, unit gain at DC
-    h = h / h.sum() * up
-    n_pre_pad = down - half_len % down
-    n_pre_remove = (half_len + n_pre_pad) // down
-    return np.concatenate([np.zeros(n_pre_pad), h]).astype(np.float32), n_pre_remove, up, down
 
 
 def lp_gain(n_bins, start, stop):
@@ -407,7 +393,6 @@ class VREngine:
         if net.output_bin != p["bins"] + 1:
             raise ValueError("network bin count does not match the model parameters")
         self.plans = {d: StftPlan(bp["n_fft"], bp["hl"]) for d, bp in p["band"].items()}
-        self._taps = {}
         # pre-filter of combine_spectrograms (spec_utils.py:266-277) as a per-bin gain
         g = np.ones(p["bins"] + 1, np.float64)
         if p["pre_filter_start"] > 0:
@@ -439,22 +424,6 @@ class VREngine:
         from .graphs import GraphedForward
 
         self.graphed = GraphedForward(self.net.predict_mask)
-
-    # ---- resampling
-    def _resample(self, x: torch.Tensor, orig_sr: int, target_sr: int) -> torch.Tensor:
-        if orig_sr == target_sr:
-            return x
-        g = math.gcd(int(orig_sr), int(target_sr))
-        up, down = int(target_sr) // g, int(orig_sr) // g
-        if (up, down) not in self._taps:
-            taps, pre, _, _ = resample_poly_design(up, down)
-            self._taps[(up, down)] = (torch.from_numpy(taps).to(self.device), pre)
-        taps, pre = self._taps[(up, down)]
-        C, n_in = x.shape
-        n_out = -(-n_in * up // down)
-        y = _new((C, n_out), x)
-        check(lib.b200sep_resample_poly_f32(_ptr(x), _ptr(taps), taps.numel(), up, down, pre, C, n_in, n_out, _ptr(y), _stream()), "resample_poly_f32")
-        return y
 
     # ---- analysis
     def _wave_to_spec(self, wave: torch.Tensor, d: int) -> torch.Tensor:
@@ -499,10 +468,7 @@ class VREngine:
             if d == n:
                 waves[d] = wave.contiguous()
             else:
-                up_sr = p["band"][d + 1]["sr"]
-                if bp["sr"] != up_sr and bp.get("res_type") != "polyphase":
-                    raise NotImplementedError(f"band {d} is resampled with res_type={bp.get('res_type')}: only polyphase is covered")
-                waves[d] = self._resample(waves[d + 1], up_sr, bp["sr"])
+                waves[d] = resample(waves[d + 1], p["band"][d + 1]["sr"], bp["sr"], bp["res_type"])
             specs[d] = self._wave_to_spec(waves[d], d)
         if keep_high_end:  # high_end_process (vr_separator.py:287-289): the top band's bins above its crop, as loaded
             bp = p["band"][n]
@@ -692,15 +658,27 @@ class VREngine:
             else:
                 if d > 1:
                     w_d = ew(wave, w_d, w_d)
-                wave = self._resample(w_d, bp["sr"], p["band"][d + 1]["sr"])
+                wave = resample(w_d, bp["sr"], p["band"][d + 1]["sr"], "polyphase")  # the stand-in for the reference's sinc_fastest up-sampling
         return wave
 
-    def separate(self, wave: np.ndarray, enable_tta=False, post_process_threshold=None, high_end_process=False):
-        """(2, N) host -> primary (2, M), secondary (2, M) host float32, M = hop_top * (frames - 1); None on the ranks other than 0 of a sharded run."""
+    def separate(self, wave: np.ndarray, enable_tta=False, post_process_threshold=None, high_end_process=False, sr=None):
+        """(2, N) host -> primary (2, M), secondary (2, M) host float32, M = hop_top * (frames - 1); None on the ranks other than 0 of a sharded run.
+        sr: the rate of `wave` when it is not the model's (VRSeparator passes 44100).  The mix is then resampled to the top band's rate with that
+        band's res_type, as librosa.load(sr=band sr) does (vr_separator.py:273), and both stems are resampled back to `sr` with librosa's default
+        soxr_hq (:221-222, :239-240), M = ceil(M_model * sr / model sr).  Sharded: every rank resamples the mix, rank 0 the stems."""
         wd = torch.from_numpy(np.ascontiguousarray(wave, dtype=np.float32)).to(self.device)
+        top = self.p["band"][self.n_bands]
+        model_sr = self.p["sr"]
+        if sr is not None:
+            wd = resample(wd, sr, top["sr"], top["res_type"])
         spec = self.loading_mix(wd, keep_high_end=high_end_process)
         yv = self.inference(spec, enable_tta, post_process_threshold)
         if yv is None:
             return None
-        y, v = yv
-        return self.spec_to_wav(y, high_end_process).cpu().numpy(), self.spec_to_wav(v, high_end_process).cpu().numpy()
+        out = []
+        for s in yv:
+            w = self.spec_to_wav(s, high_end_process)
+            if sr is not None:
+                w = resample(w, model_sr, sr, "soxr_hq")
+            out.append(w.cpu().numpy())
+        return tuple(out)
