@@ -46,9 +46,11 @@ __device__ __forceinline__ float2 block_sum2(float a, float b, float* red) {
 
 // GroupNorm(num_groups=1, C) over one sample of n = C*L elements, affine per channel, optional activation (hdemucs.py:79-80 norm_fn,
 // demucs.py:139-141; eps 1e-5, biased variance).  Two kernels so that a single huge sample (the time branch: 96 x 85995) still fills
-// the GPU: (1) `nblk` CTAs per sample reduce shifted sums  sum(x - x0), sum((x - x0)^2)  (x0 = the sample's first element, which
-// removes the E[x^2] - mean^2 cancellation) into double partials; (2) every CTA re-reduces the partials of its sample in a fixed
-// order (deterministic) and normalises its slice.
+// the GPU: (1) `nblk` CTAs per sample reduce shifted sums  sum(x - x0), sum((x - x0)^2)  (x0 = the sample's first element) into double
+// partials; (2) every CTA re-reduces the partials of its sample in a fixed order (deterministic) and normalises its slice.
+// Every thread accumulates in double: the shift removes the E[x^2] - mean^2 cancellation only when x0 is typical, and with an outlier
+// x0 (30 sigma) fp32 per-thread sums of ~256 squares already cost 4e-6 of rstd.  The mean is applied as a float hi + lo pair, so a
+// large mean (1e3 at std 1) is not rounded to fp32 before the subtraction.
 // Layouts: channel-first (B, C, Fr, L) where sample (b, fr) owns x[((b*C + c)*Fr + fr)*L + l]  (Fr = 1: plain (B, C, L); Fr > 1: DConv
 // applied per frequency row of a (B, C, Fr, T) tensor without the permute of hdemucs.py:141-146), or channel-last (samples, L, C)
 // (MyGroupNorm on (B, T, C) tokens, transformer.py:184-193).
@@ -69,13 +71,12 @@ __global__ void __launch_bounds__(256) gn_partial_kernel(const float* __restrict
   const int sample = blockIdx.y;
   const float x0 = __ldg(&x[gn_index(g, sample, 0)]);
   const uint32_t lo = blockIdx.x * g.chunk, hi = min(g.n, lo + g.chunk);
-  float s = 0.f, q = 0.f;
+  double ds = 0.0, dq = 0.0;
   for (uint32_t i = lo + threadIdx.x; i < hi; i += 256) {
-    const float d = __ldg(&x[gn_index(g, sample, i)]) - x0;
-    s += d;
-    q = fmaf(d, d, q);
+    const double d = (double)__ldg(&x[gn_index(g, sample, i)]) - (double)x0;
+    ds += d;
+    dq = fma(d, d, dq);
   }
-  double ds = s, dq = q;
   for (int o = 16; o > 0; o >>= 1) {
     ds += __shfl_xor_sync(0xffffffffu, ds, o);
     dq += __shfl_xor_sync(0xffffffffu, dq, o);
@@ -99,7 +100,7 @@ __global__ void __launch_bounds__(256) gn_partial_kernel(const float* __restrict
 
 __global__ void __launch_bounds__(256) gn_apply_kernel(const float* __restrict__ x, const float* __restrict__ gamma, const float* __restrict__ beta,
                                                       float* __restrict__ y, GnGeom g, const double2* __restrict__ part, int act) {
-  __shared__ float stat[2];
+  __shared__ float stat[3];
   const int sample = blockIdx.y;
   if (threadIdx.x == 0) {
     double S = 0.0, Q = 0.0;
@@ -111,16 +112,18 @@ __global__ void __launch_bounds__(256) gn_apply_kernel(const float* __restrict__
     const double md = S / (double)g.n;  // mean of (x - x0)
     double var = Q / (double)g.n - md * md;
     if (var < 0.0) var = 0.0;
-    stat[0] = (float)(ps[gridDim.x].x + md);
-    stat[1] = (float)(1.0 / sqrt(var + 1e-5));
+    const double mean = ps[gridDim.x].x + md;
+    stat[0] = (float)mean;
+    stat[1] = (float)(mean - (double)stat[0]);
+    stat[2] = (float)(1.0 / sqrt(var + 1e-5));
   }
   __syncthreads();
-  const float mean = stat[0], rstd = stat[1];
+  const float mean_hi = stat[0], mean_lo = stat[1], rstd = stat[2];
   const uint32_t lo = blockIdx.x * g.chunk, hi = min(g.n, lo + g.chunk);
   for (uint32_t i = lo + threadIdx.x; i < hi; i += 256) {
     const int c = (g.channel_last ? (int)(i % (uint32_t)g.C) : (int)(i / g.L)) + (sample % g.groups) * g.C;
     const int64_t o = gn_index(g, sample, i);
-    y[o] = f32_act((x[o] - mean) * rstd * __ldg(&gamma[c]) + __ldg(&beta[c]), act);
+    y[o] = f32_act(((x[o] - mean_hi) - mean_lo) * rstd * __ldg(&gamma[c]) + __ldg(&beta[c]), act);
   }
 }
 
@@ -162,26 +165,28 @@ __global__ void glu_kernel(const float* __restrict__ a, const float* __restrict_
   }
 }
 
-// LayerNorm over the last dimension C of (rows, C); one warp per row.  eps 1e-5.
+// LayerNorm over the last dimension C of (rows, C); one warp per row.  eps 1e-5.  The sums are taken in double and the mean is applied as a
+// float hi + lo pair, as in GroupNorm above: with a row mean of 100 at std 1, fp32 sums of the raw values and an fp32-rounded mean cost 2e-5.
 __global__ void layernorm_kernel(const float* __restrict__ x, const float* __restrict__ gamma, const float* __restrict__ beta, float* __restrict__ y, int64_t rows,
                                  int C) {
   const int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (row >= rows) return;
   const int lane = threadIdx.x & 31;
   const float* xr = x + row * C;
-  float s = 0.f;
-  for (int c = lane; c < C; c += 32) s += xr[c];
+  double s = 0.0;
+  for (int c = lane; c < C; c += 32) s += (double)xr[c];
   for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-  const float mean = s / C;
-  float q = 0.f;
+  const double mean = s / C;
+  double q = 0.0;
   for (int c = lane; c < C; c += 32) {
-    const float d = xr[c] - mean;
-    q = fmaf(d, d, q);
+    const double d = (double)xr[c] - mean;
+    q = fma(d, d, q);
   }
   for (int o = 16; o > 0; o >>= 1) q += __shfl_xor_sync(0xffffffffu, q, o);
-  const float rstd = rsqrtf(q / C + 1e-5f);
+  const float mean_hi = (float)mean, mean_lo = (float)(mean - (double)mean_hi);
+  const float rstd = (float)(1.0 / sqrt(q / C + 1e-5));
   float* yr = y + row * C;
-  for (int c = lane; c < C; c += 32) yr[c] = (xr[c] - mean) * rstd * __ldg(&gamma[c]) + __ldg(&beta[c]);
+  for (int c = lane; c < C; c += 32) yr[c] = ((xr[c] - mean_hi) - mean_lo) * rstd * __ldg(&gamma[c]) + __ldg(&beta[c]);
 }
 
 // Batched SGEMM TN: C[z][m][n] = epi( sum_k A[z][m][k] * Bw[z][n][k] ), 128x128x16 tiles, 8x8 per thread.

@@ -121,7 +121,9 @@ __global__ void vr_mask_kernel(const float* __restrict__ mask, int mask_stride, 
     const int64_t o = (int64_t)bin * frames + t;
     const float re = __ldg(&spec[(2 * c) * plane + o]), im = __ldg(&spec[(2 * c + 1) * plane + o]);
     float yr = m * re, yi = m * im, vr = (1.f - m) * re, vi = (1.f - m) * im;
-    // np.nan_to_num(nan=0, posinf=0, neginf=0) (vr_separator.py:187-188)
+    // np.nan_to_num(nan=0, posinf=0, neginf=0) (vr_separator.py:187-188).  The reference forms mask * |X| * exp(i angle X): a non-finite
+    // component makes |X| non-finite, so both components of that entry are non-finite there and both become 0.
+    if (!isfinite(re) || !isfinite(im)) yr = yi = vr = vi = 0.f;
     if (!isfinite(yr)) yr = 0.f;
     if (!isfinite(yi)) yi = 0.f;
     if (!isfinite(vr)) vr = 0.f;
