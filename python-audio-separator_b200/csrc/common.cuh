@@ -41,6 +41,14 @@ void count_launch(int n = 1);
     }                                                                                          \
   } while (0)
 
+// A kernel attribute such as the dynamic shared-memory limit belongs to the function in one device's context, not to the process, so a launch
+// site that remembers having raised one remembers it per device.  Declares `dev`, the current device's slot in such a cache.
+constexpr int kMaxDevices = 64;
+#define B2_DEVICE_SLOT(dev)                                                                                             \
+  int dev = 0;                                                                                                          \
+  B2_CUDA(cudaGetDevice(&dev));                                                                                         \
+  B2_CHECK_ARG(dev >= 0 && dev < ::b200sep::kMaxDevices, "device index %d beyond the %d per-device slots", dev, ::b200sep::kMaxDevices)
+
 static inline int cdiv(int64_t a, int64_t b) { return (int)((a + b - 1) / b); }
 
 constexpr int kNumSMs = 132;  // H100 SXM

@@ -209,10 +209,11 @@ static int launch_gen(const ConvGenParams& p, cudaStream_t st) {
   using G = GenGeom<KH, KW, SH, SW, DW>;
   // the W-transposed mode stages its output tile in shared memory; everything else only needs the operand tiles (keeps the occupancy of the small geometries)
   const int smem = (p.up_axis == 2 ? G::SMEM_FLOATS : G::OPERAND_FLOATS) * (int)sizeof(float);
-  static bool attr_set = false;
-  if (!attr_set) {
+  static bool attr_set[kMaxDevices] = {};
+  B2_DEVICE_SLOT(dev);
+  if (!attr_set[dev]) {
     B2_CUDA(cudaFuncSetAttribute(conv_gen_kernel<KH, KW, SH, SW, DW>, cudaFuncAttributeMaxDynamicSharedMemorySize, G::SMEM_FLOATS * (int)sizeof(float)));
-    attr_set = true;
+    attr_set[dev] = true;
   }
   dim3 grid(cdiv(p.Wo, GTW), cdiv(p.Ho, GTH), p.B * (p.CoutPad / GTCO));
   B2_CHECK_ARG(grid.y <= 65535 && grid.z <= 65535, "conv2d_f32: grid too large (Ho=%d, B*co_tiles=%d)", p.Ho, (int)grid.z);

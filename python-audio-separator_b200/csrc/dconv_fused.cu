@@ -296,12 +296,13 @@ int dconv_launch(DconvParams p, bool have_u, cudaStream_t st) {
   const size_t smem1 = (size_t)HP * p.C * 3 * sizeof(float);
   const size_t smem23 = ((size_t)p.C * 2 * HP + (size_t)p.C * 8) * sizeof(float);
   B2_CHECK_ARG(smem23 <= 200 * 1024 && (have_u || smem1 <= 200 * 1024), "dconv_f32: C=%d hid=%d weights do not fit in shared memory", p.C, HID);
-  static bool attr_set = false;
-  if (!attr_set) {
+  static bool attr_set[kMaxDevices] = {};
+  B2_DEVICE_SLOT(dev);
+  if (!attr_set[dev]) {
     B2_CUDA(cudaFuncSetAttribute(dconv_k1_kernel<HID, P>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     B2_CUDA(cudaFuncSetAttribute(dconv_k23_kernel<HID, P, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     B2_CUDA(cudaFuncSetAttribute(dconv_k23_kernel<HID, P, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    attr_set = true;
+    attr_set[dev] = true;
   }
   // persistent CTAs (the weights are staged once per CTA); as many per SM as the shared-memory image allows
   auto grid_for = [&](size_t smem) {
@@ -497,10 +498,11 @@ size_t dconv_row_smem(int C, int L) {
 template <int HID>
 int dconv_row_launch(const DconvParams& p, cudaStream_t st) {
   const size_t smem = dconv_row_smem<HID>(p.C, p.L);
-  static bool attr_set = false;
-  if (!attr_set) {
+  static bool attr_set[kMaxDevices] = {};
+  B2_DEVICE_SLOT(dev);
+  if (!attr_set[dev]) {
     B2_CUDA(cudaFuncSetAttribute(dconv_row_kernel<HID>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
-    attr_set = true;
+    attr_set[dev] = true;
   }
   const int threads = std::min(kRowMaxThreads, std::max(128, (p.L + 31) / 32 * 32));
   const int per_sm = (int)std::max<size_t>(1, std::min<size_t>(4, (220 * 1024) / smem));

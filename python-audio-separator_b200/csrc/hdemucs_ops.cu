@@ -295,10 +295,11 @@ extern "C" int b200sep_lstm_bidir_wide_f32(const float* x_proj, const float* w_h
         break;
       }
   size_t smem = ((size_t)2 * hid * NS + (size_t)KS * NS * GL + (size_t)2 * NS * UH) * sizeof(float) + (w_in_smem ? wbytes : 0);
-  static size_t attr = 0;
-  if (smem > attr) {
+  static size_t attr[kMaxDevices] = {};  // the largest limit set so far, per device
+  B2_DEVICE_SLOT(dev);
+  if (smem > attr[dev]) {
     B2_CUDA(cudaFuncSetAttribute(lstm_bidir_cluster_kernel<NS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr = smem;
+    attr[dev] = smem;
   }
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3((unsigned)(cdiv(N, NS) * CL), 2);

@@ -159,10 +159,11 @@ template <int KH, int KW, int S>
 static int launch_conv(const ConvParams& p, cudaStream_t stream) {
   using G = ConvGeom<KH, KW, S>;
   const int smem = G::SMEM_FLOATS * (int)sizeof(float);
-  static bool attr_set = false;
-  if (!attr_set) {
+  static bool attr_set[kMaxDevices] = {};
+  B2_DEVICE_SLOT(dev);
+  if (!attr_set[dev]) {
     B2_CUDA(cudaFuncSetAttribute(conv2d_simt_kernel<KH, KW, S>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    attr_set = true;
+    attr_set[dev] = true;
   }
   dim3 grid(cdiv(p.Wo, TW), cdiv(p.Ho, TH), p.B * (p.CoutPad / TCO));
   B2_CHECK_ARG(grid.y <= 65535 && grid.z <= 65535, "conv2d_simt: grid too large (Ho=%d, B*co_tiles=%d)", p.Ho, (int)grid.z);

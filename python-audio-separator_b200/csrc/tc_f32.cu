@@ -438,10 +438,11 @@ __global__ void tc_pack_kernel(const float* __restrict__ src, int conv, int64_t 
 
 template <bool F16>
 int launch_tc_kernel(const TcParams& p, size_t smem, int grid, cudaStream_t st) {
-  static bool attr_set = false;
-  if (!attr_set) {
+  static bool attr_set[kMaxDevices] = {};
+  B2_DEVICE_SLOT(dev);
+  if (!attr_set[dev]) {
     B2_CUDA(cudaFuncSetAttribute(tc_f32_kernel<F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    attr_set = true;
+    attr_set[dev] = true;
   }
   tc_f32_kernel<F16><<<grid, kThreads, smem, st>>>(p);
   B2_LAUNCHED();
@@ -768,10 +769,11 @@ template <bool F16>
 int launch_attention(const AttParams& p, int B, int H, int Lq, cudaStream_t st) {
   using L = AttLayout<F16>;
   const size_t smem = (size_t)L::kSmem + 1024 + 256;
-  static bool attr_set = false;
-  if (!attr_set) {
+  static bool attr_set[kMaxDevices] = {};
+  B2_DEVICE_SLOT(dev);
+  if (!attr_set[dev]) {
     B2_CUDA(cudaFuncSetAttribute(tc_attention_kernel<F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr_set = true;
+    attr_set[dev] = true;
   }
   const int nk = cdiv(p.Lk, kAttKeys);
   const int64_t nq_chunks = (int64_t)B * H * p.mq_tiles * 1024, nk_chunks = (int64_t)B * H * nk * 1024;

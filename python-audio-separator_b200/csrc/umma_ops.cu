@@ -608,10 +608,11 @@ static int launch(const CUtensorMap& a_hi, const CUtensorMap& a_lo, const CUtens
   B2_CHECK_ARG(stages >= 2, "umma: a pipeline stage of %u bytes does not fit twice in shared memory", p.stage_bytes);
   p.stages = stages;
   const size_t smem = (size_t)stages * p.stage_bytes + fixed;
-  static bool attr_set = false;
-  if (!attr_set) {
+  static bool attr_set[kMaxDevices] = {};
+  B2_DEVICE_SLOT(dev);
+  if (!attr_set[dev]) {
     B2_CUDA(cudaFuncSetAttribute(umma_pair_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    attr_set = true;
+    attr_set[dev] = true;
   }
   return launch_persistent(umma_pair_kernel, p.num_tiles, smem, st, a_hi, a_lo, b_hi, b_lo, p);
 }
@@ -837,10 +838,11 @@ static int store_map(const void* base, int F, int T, int C, int box_c, CUtensorM
 
 template <int NC, int ACT, bool RES, bool MUL>
 static int launch_conv3(const CUtensorMap& a_hi, const CUtensorMap& a_lo, const CUtensorMap& o_hi, const CUtensorMap& o_lo, UmmaParams& p, size_t smem, cudaStream_t st) {
-  static bool attr_set = false;
-  if (!attr_set) {
+  static bool attr_set[kMaxDevices] = {};
+  B2_DEVICE_SLOT(dev);
+  if (!attr_set[dev]) {
     B2_CUDA(cudaFuncSetAttribute(umma_conv3_kernel<NC, ACT, RES, MUL>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    attr_set = true;
+    attr_set[dev] = true;
   }
   return launch_persistent(umma_conv3_kernel<NC, ACT, RES, MUL>, p.num_tiles, smem, st, a_hi, a_lo, o_hi, o_lo, p);
 }

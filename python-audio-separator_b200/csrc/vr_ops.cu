@@ -326,10 +326,11 @@ extern "C" int b200sep_resample_poly_f32(const float* x, const float* taps, int 
 extern "C" int b200sep_lstm_bidir_f32(const float* x_proj, const float* w_hh, float* out, int T, int N, int hid, void* stream) {
   B2_CHECK_ARG(x_proj && w_hh && out && T >= 1 && N >= 1 && hid >= 1 && hid <= 96, "lstm_bidir_f32: bad argument (hid must be <= 96)");
   const int smem = (4 * hid * hid + 5 * hid) * (int)sizeof(float);
-  static int attr = 0;
-  if (smem > attr) {
+  static int attr[kMaxDevices] = {};  // the largest limit set so far, per device
+  B2_DEVICE_SLOT(dev);
+  if (smem > attr[dev]) {
     B2_CUDA(cudaFuncSetAttribute(lstm_bidir_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    attr = smem;
+    attr[dev] = smem;
   }
   lstm_bidir_kernel<<<dim3(N, 2), 4 * hid, smem, (cudaStream_t)stream>>>(x_proj, w_hh, out, T, N, hid);
   B2_LAUNCHED();
