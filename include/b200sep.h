@@ -169,6 +169,32 @@ int b200sep_flac_decode(const uint8_t* frames, int64_t n_bytes, void* work, int6
                         int64_t out_ld, int64_t* result, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------
+ * Uncompressed PCM decoding (the data chunk of WAV / RF64, the SSND payload of AIFF / AIFF-C) -> the planar float mix prepare_mix returns,
+ * converted as libsndfile's sf_read_float with normalisation on (what librosa.load returns):
+ *   U8            (u - 128) * 2^-7
+ *   S8 ... S32    (float)v * 2^-(8*bytes-1), one rounding: exact up to 24 bits, round-to-nearest for 32 bits
+ *   F32           the bits as they are (no scaling, no clipping; NaN and Inf pass through)
+ *   F64           round-to-nearest to float (a NaN keeps its sign and the top of its payload, quiet bit set)
+ * data:         the payload, 16-byte aligned and readable up to n_frames * frame_bytes rounded up to a multiple of 16.
+ * frame_bytes:  the block align, at least channels * sample bytes and at most 65535; channel c of frame n starts at byte n * frame_bytes + c * bytes.
+ * out:          out[c * out_ld + n] for c < out_channels (1 <= out_channels <= channels), n < n_frames.
+ * One launch, no host synchronisation. */
+#define B200SEP_PCM_U8 0    /* WAV 8-bit (unsigned) */
+#define B200SEP_PCM_S8 1    /* AIFF 8-bit (signed) */
+#define B200SEP_PCM_S16LE 2
+#define B200SEP_PCM_S16BE 3
+#define B200SEP_PCM_S24LE 4
+#define B200SEP_PCM_S24BE 5
+#define B200SEP_PCM_S32LE 6
+#define B200SEP_PCM_S32BE 7
+#define B200SEP_PCM_F32LE 8
+#define B200SEP_PCM_F32BE 9
+#define B200SEP_PCM_F64LE 10
+#define B200SEP_PCM_F64BE 11
+int b200sep_pcm_decode_f32(const uint8_t* data, int64_t n_frames, int frame_bytes, int channels, int format, int out_channels, float* out,
+                           int64_t out_ld, void* stream);
+
+/* ---------------------------------------------------------------------------------------------------
  * ConvTDFNet (the graph inside UVR-MDX-NET-*.onnx; topology: uvr_lib_v5/mdxnet.py:30-120, modules.py:1-74).
  * Replaces `self.model_run(spek)` = ort.InferenceSession.run (architectures/mdx_separator.py:122-123, :443).
  *

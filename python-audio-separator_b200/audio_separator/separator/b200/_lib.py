@@ -56,6 +56,7 @@ _SIGS = {
     "b200sep_flac_decode_work_bytes": (i64, [i64]),
     "b200sep_flac_locate": (i32, [vp, i64, i32, i32, i32, i32, vp, vp, vp]),
     "b200sep_flac_decode": (i32, [vp, i64, vp, i64, i64, vp, i64, vp, vp]),
+    "b200sep_pcm_decode_f32": (i32, [vp, i64, i32, i32, i32, i32, vp, i64, vp]),
     "b200sep_mdxnet_param_count": (i64, [C.POINTER(MdxNetConfig)]),
     "b200sep_mdxnet_create": (i32, [C.POINTER(vp), C.POINTER(MdxNetConfig), vp, i64]),
     "b200sep_mdxnet_destroy": (None, [vp]),

@@ -3,8 +3,9 @@
 Mirrors what `Separator` and the plugins rely on from the reference's CommonSeparator
 (audio_separator/separator/common_separator.py:57-157 config/stem naming, :217-282 prepare_mix,
 :284-451 write_audio, :453-507 cache + output paths).  Audio decode is NOT part of the accelerated
-path (SURVEY.md section 2, row 2): WAV goes through the stdlib `wave` module, FLAC (recognised by content) is
-decoded on the GPU (b200/flac.py) into a DeviceStem, anything else goes through soundfile/librosa when those wheels are installed.  Output: WAV through `wave`, FLAC encoded on the GPU
+path (SURVEY.md section 2, row 2): 16-32-bit integer PCM WAV goes through the stdlib `wave` module, FLAC (recognised
+by content) is decoded on the GPU (b200/flac.py) into a DeviceStem, as are the other uncompressed WAV, RF64, AIFF and AIFF-C files (b200/pcm_reader.py),
+anything else goes through soundfile/librosa when those wheels are installed.  Output: WAV through `wave`, FLAC encoded on the GPU
 (b200/flac.py), anything else through soundfile.
 """
 import gc
@@ -150,6 +151,31 @@ class CommonSeparator:
         self.input_bit_depth, self.input_subtype = depth, subtype
         return mix
 
+    def _read_pcm(self, path):
+        """Uncompressed WAV / RF64 / AIFF / AIFF-C (recognised by content) decoded on the GPU (b200/pcm_reader.py): (C, N) float32 CUDA tensor,
+        C = min(channels, 2); None for another container, another sample rate or a compressed payload (those take the librosa path)."""
+        from .b200 import pcm_reader
+
+        with open(path, "rb") as f:
+            if not pcm_reader.is_pcm_container(f.read(12)):
+                return None
+            f.seek(0)
+            data = f.read()
+        try:
+            info = pcm_reader.parse(data)
+        except NotImplementedError:
+            return None
+        if info["sample_rate"] != self.sample_rate:
+            return None
+        for w in info["warnings"]:
+            self.logger.warning(f"{path}: {w}")
+        depth, subtype = pcm_reader.input_bit_depth(info)
+        if subtype == "PCM_U8":
+            self.logger.warning(f"Unknown audio subtype {subtype}, defaulting to 16-bit output")
+        mix, _ = pcm_reader.decode(data, self.torch_device if self.torch_device is not None and self.torch_device.type == "cuda" else "cuda")
+        self.input_bit_depth, self.input_subtype = depth, subtype
+        return mix
+
     def _read_audio(self, path):
         from .b200 import flac
 
@@ -173,6 +199,9 @@ class CommonSeparator:
                     return data[0] if ch == 1 else np.ascontiguousarray(data[:2])
             except _wave.Error:
                 pass
+        mix = self._read_pcm(path)
+        if mix is not None:
+            return mix
         try:
             import librosa
             import soundfile as sf
