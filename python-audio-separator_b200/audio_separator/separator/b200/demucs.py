@@ -19,9 +19,14 @@ import torch
 
 from ._lib import LAYOUT_CFT, MATH_BF16X3, check, lib
 from .engine import StftPlan, _ptr, _require_cuda, _stream, _window
+from .ops import (ACT_GELU, ACT_NONE, _new, block_conv_weight, block_convtr_weight, conv2d, conv_transpose, ew, gemm, glu, groupnorm1, layernorm, linear,
+                  to_device)
 from .sharded import ShardRunner, plan_range_shards
 
-ACT_NONE, ACT_RELU, ACT_GELU = 0, 1, 2
+# Code written against this module imports the operator wrappers from it: they stay importable here, defined once in ops.py.
+from .ops import ACT_RELU, _packed_conv, _packed_linear  # noqa: F401
+from .ops import gemm as _gemm_raw  # noqa: F401
+
 _DCONV_FUSED_HID = (4, 6, 8, 12, 16, 24, 32, 48)  # hidden widths b200sep_dconv_f32 is instantiated for
 
 
@@ -69,31 +74,6 @@ class HTDemucsConfig:
             raise ValueError("nfft/2 must be divisible by stride**depth")
 
 
-# --------------------------------------------------------------------------------------------------------- host-side weight prep
-def _ceil48(n):
-    return -(-n // 48) * 48
-
-
-def block_conv_weight(w: np.ndarray) -> np.ndarray:
-    """(Cout, Cin, KH, KW) -> [Cin][KH*KW][ceil48(Cout)], the layout b200sep_conv2d_f32 streams through shared memory."""
-    co, ci, kh, kw = w.shape
-    out = np.zeros((ci, kh * kw, _ceil48(co)), np.float32)
-    out[:, :, :co] = w.transpose(1, 2, 3, 0).reshape(ci, kh * kw, co)
-    return out
-
-
-def block_convtr_weight(w: np.ndarray, stride: int) -> np.ndarray:
-    """ConvTranspose weight (Cin, Cout, K) with K = 2*stride -> the 2-tap convolution over the coarse index q whose GEMM column
-    r*Cout + co produces output sample q*stride + r:   y[q*s + r] = x[q-1] . W[:, :, r + s] + x[q] . W[:, :, r]."""
-    ci, co, k = w.shape
-    assert k == 2 * stride
-    out = np.zeros((ci, 2, _ceil48(stride * co)), np.float32)
-    for r in range(stride):
-        out[:, 0, r * co : (r + 1) * co] = w[:, :, r + stride]
-        out[:, 1, r * co : (r + 1) * co] = w[:, :, r]
-    return out
-
-
 def sin_embedding_1d(length: int, dim: int, max_period: float) -> np.ndarray:
     """create_sin_embedding (transformer.py:19-26) as (length, dim): [cos(phase) | sin(phase)]."""
     half = dim // 2
@@ -118,131 +98,12 @@ def sin_embedding_2d_tokens(dim: int, height: int, width: int, max_period: float
     return pe.reshape(width * height, dim)
 
 
-# --------------------------------------------------------------------------------------------------------- operator wrappers
-def _new(shape, like=None, device=None):
-    return torch.empty(shape, dtype=torch.float32, device=like.device if like is not None else device)
+# --------------------------------------------------------------------------------------------------------- the networks
+class HybridDemucsNet:
+    """What the hybrid (spectrogram + waveform) Demucs nets share: device, math mode, STFT plan and weights, the plain DConv branch, and the
+    spectral front and back ends of the forward.  HTDemucsNet and HDemucsNet add their layers and launch order."""
 
-
-def _packed_cache(w):
-    """{math mode: packed image} of one weight tensor"""
-    cache = getattr(w, "_b200_packed", None)
-    if cache is None:
-        cache = w._b200_packed = {}
-    return cache
-
-
-def _packed_conv(wb, cin, taps, cout, math=MATH_BF16X3):
-    """The tensor-core image of a blocked convolution weight (bf16 hi/lo planes, or one fp16 plane, in the kernel's shared-memory layout), built once
-    per tensor and math mode."""
-    cache = _packed_cache(wb)
-    pk = cache.get(math)
-    if pk is None and cin * taps >= 32 and cout >= 16:
-        cin8 = -(-cin // 8) * 8
-        pk = _new((lib.b200sep_tc_packed_floats_math(cout, cin8 * taps, math),), wb)
-        check(lib.b200sep_tc_pack_conv_weights_math(_ptr(wb), cin, taps, cout, _ptr(pk), math, _stream()), "tc_pack_conv_weights")
-        cache[math] = pk
-    return pk
-
-
-def _packed_linear(w, math=MATH_BF16X3):
-    cache = _packed_cache(w)
-    pk = cache.get(math)
-    if pk is None and w.shape[0] >= 32 and w.shape[1] >= 32:
-        pk = _new((lib.b200sep_tc_packed_floats_math(w.shape[0], w.shape[1], math),), w)
-        check(lib.b200sep_tc_pack_linear_weights_math(_ptr(w), w.shape[0], w.shape[1], w.shape[1], _ptr(pk), math, _stream()), "tc_pack_linear_weights")
-        cache[math] = pk
-    return pk
-
-
-def conv2d(x, wb, bias, cout, k, s=(1, 1), p=(0, 0), dw=1, act=ACT_NONE, add=None, add_before_act=False, out_hw=None, out=None, out_c_off=0, dh=1, math=MATH_BF16X3):
-    """x (B,Cin,H,W) -> (B,cout,Ho,Wo);  out_hw overrides the implied output size (right/bottom zero padding is implicit);
-    out/out_c_off: write into channels [out_c_off, out_c_off + cout) of an existing (B, C_total, Ho, Wo) tensor (a fused torch.cat).
-    math: MATH_BF16X3 or MATH_FP16 (tensor-core arithmetic; the SIMT fallback for small shapes is fp32 either way)."""
-    B, cin, H, W = x.shape
-    if out_hw is None:
-        Ho = (H + 2 * p[0] - dh * (k[0] - 1) - 1) // s[0] + 1
-        Wo = (W + 2 * p[1] - dw * (k[1] - 1) - 1) // s[1] + 1
-    else:
-        Ho, Wo = out_hw
-    if out is None:
-        y, ct = _new((B, cout, Ho, Wo), x), 0
-    else:
-        assert out.shape[0] == B and tuple(out.shape[2:]) == (Ho, Wo), (out.shape, (B, cout, Ho, Wo))
-        y, ct = out, out.shape[1]
-    pk = _packed_conv(wb, cin, k[0] * k[1], cout, math)
-    check(lib.b200sep_conv2d_f32_math(_ptr(x), _ptr(wb), _ptr(bias) if bias is not None else None, _ptr(add) if add is not None else None, _ptr(y), B, cin, H, W, cout,
-                                      Ho, Wo, k[0], k[1], s[0], s[1], p[0], p[1], dh, dw, act, int(add_before_act), 0, 1, 0, 0, ct, out_c_off,
-                                      _ptr(pk) if pk is not None else None, math, _stream()), "conv2d_f32")
-    return y
-
-
-def conv_transpose(x, wb, bias, cout, axis, stride, trim, out_len, act=ACT_NONE, math=MATH_BF16X3):
-    """nn.ConvTranspose1d/2d with kernel 2*stride along `axis` (1 = H, 2 = W), output cropped to [trim, trim + out_len)."""
-    B, cin, H, W = x.shape
-    if axis == 1:
-        y = _new((B, cout, out_len, W), x)
-        k, p, hw = (2, 1), (1, 0), (H + 1, W)
-    else:
-        y = _new((B, cout, H, out_len), x)
-        k, p, hw = (1, 2), (0, 1), (H, W + 1)
-    pk = _packed_conv(wb, cin, 2, stride * cout, math)
-    check(lib.b200sep_conv2d_f32_math(_ptr(x), _ptr(wb), _ptr(bias), None, _ptr(y), B, cin, H, W, stride * cout, hw[0], hw[1], k[0], k[1], 1, 1, p[0], p[1], 1, 1, act,
-                                      0, axis, stride, trim, out_len, 0, 0, _ptr(pk) if pk is not None else None, math, _stream()), "conv2d_f32(transposed)")
-    return y
-
-
-def groupnorm1(x, gamma, beta, act=ACT_NONE, channel_last=False):
-    """in place; x (B,C,Fr,L) channel-first (one sample per (b, fr)) or (B,L,C) channel_last."""
-    if channel_last:
-        B, L, Cc = x.shape
-        Fr = 1
-    else:
-        B, Cc, Fr, L = x.shape
-    work = _new((lib.b200sep_groupnorm1_work_floats(B, Cc, Fr, L),), x)
-    check(lib.b200sep_groupnorm1_f32(_ptr(x), _ptr(gamma), _ptr(beta), _ptr(x), B, Cc, Fr, L, act, int(channel_last), _ptr(work), _stream()), "groupnorm1_f32")
-    return x
-
-
-def glu(a, res=None, scale=None):
-    B, c2, H, W = a.shape
-    y = _new((B, c2 // 2, H, W), a)
-    check(lib.b200sep_glu_f32(_ptr(a), _ptr(res) if res is not None else None, _ptr(scale) if scale is not None else None, _ptr(y), B, c2 // 2, H * W, _stream()), "glu_f32")
-    return y
-
-
-def layernorm(x, gamma, beta):
-    y = torch.empty_like(x)
-    check(lib.b200sep_layernorm_f32(_ptr(x), _ptr(gamma), _ptr(beta), _ptr(y), x.numel() // x.shape[-1], x.shape[-1], _stream()), "layernorm_f32")
-    return y
-
-
-def ew(a, b, out, alpha=1.0, beta=1.0, op=0):
-    check(lib.b200sep_ew_f32(_ptr(a), _ptr(b) if b is not None else None, _ptr(out), a.numel(), alpha, beta, op, _stream()), "ew_f32")
-    return out
-
-
-def linear(x2d, w, bias, act=ACT_NONE, res=None, res_scale=None, math=MATH_BF16X3):
-    """(M,K) @ w(N,K)^T + bias -> (M,N); optional res + res_scale[n] * (.)"""
-    M, K = x2d.shape
-    N = w.shape[0]
-    y = _new((M, N), x2d)
-    pk = _packed_linear(w, math)
-    check(lib.b200sep_gemm_f32_math(_ptr(x2d), _ptr(w), _ptr(y), M, N, K, K, K, N, 1, 0, 0, 0, 1.0, _ptr(bias) if bias is not None else None, None, act,
-                                    _ptr(res) if res is not None else None, _ptr(res_scale) if res_scale is not None else None, _ptr(pk) if pk is not None else None,
-                                    math, _stream()), "gemm_f32")
-    return y
-
-
-def _gemm_raw(a_ptr, b_ptr, c_ptr, M, N, K, lda, ldb, ldc, batch, sA, sB, sC, alpha=1.0, bias_n=None, bias_m=None, math=MATH_BF16X3):
-    check(lib.b200sep_gemm_f32_math(a_ptr, b_ptr, c_ptr, M, N, K, lda, ldb, ldc, batch, sA, sB, sC, alpha, bias_n, bias_m, 0, None, None, None, math, _stream()),
-          "gemm_f32")
-
-
-# --------------------------------------------------------------------------------------------------------- the network
-class HTDemucsNet:
-    """Device-resident HTDemucs weights (re-blocked for the conv kernel) + the launch sequence of one forward."""
-
-    def __init__(self, cfg: HTDemucsConfig, state: dict, device=None, math=MATH_BF16X3):
+    def __init__(self, cfg, device=None, math=MATH_BF16X3):
         """math: MATH_BF16X3 (default, ~fp32) or MATH_FP16 (torch.autocast precision) for every tensor-core GEMM, convolution and attention of
         this net, fixed for its lifetime (the graphs GraphedForward captures record the mode of each launch)."""
         _require_cuda()
@@ -253,11 +114,92 @@ class HTDemucsNet:
         self.S = len(cfg.sources)
         self.stft = StftPlan(cfg.nfft, cfg.hop)
         self.W = {}
+
+    def _put(self, name, a):
+        self.W[name] = to_device(a, self.device)
+
+    def _dconv(self, x, prefix):
+        """DConv.forward (demucs.py:166-168) on x (B,C,Fr,T): conv1d k3 dilated -> GroupNorm(1)+GELU -> 1x1 -> GroupNorm(1) -> GLU, LayerScale residual."""
+        W = self.W
+        C_ = x.shape[1]
+        if f"{prefix}.dconv.layers.0.0.weight" not in W:  # dconv_mode without DConv on this side (hdemucs.py:83-84, :268-269)
+            return x
+        B, _, Fr, L = x.shape
+        for d in range(self.cfg.dconv_depth):
+            p = f"{prefix}.dconv.layers.{d}"
+            dil = 2**d
+            hid = W[f"{p}.0.bias"].numel()
+            if hid in _DCONV_FUSED_HID and C_ * 2 * (-(-hid // 4) * 4 + 4) * 4 <= 200 * 1024:
+                # one fused residual layer (csrc/dconv_fused.cu); the C -> hid convolution of the widest layers stays on the tensor cores
+                u_in = None
+                if 3 * C_ * (-(-hid // 4) * 4) * 4 > 200 * 1024:
+                    u_in = conv2d(x, W[f"{p}.0.weight"], W[f"{p}.0.bias"], hid, (1, 3), p=(0, dil), dw=dil, math=self.math)
+                work = _new((lib.b200sep_dconv_work_floats(B, C_, Fr, L, hid),), x)
+                check(lib.b200sep_dconv_f32(_ptr(x), _ptr(x), _ptr(W[f"{p}.0.weight:raw"]), _ptr(W[f"{p}.0.bias"]), _ptr(W[f"{p}.1.weight"]), _ptr(W[f"{p}.1.bias"]),
+                                            _ptr(W[f"{p}.3.weight:raw"]), _ptr(W[f"{p}.3.bias"]), _ptr(W[f"{p}.4.weight"]), _ptr(W[f"{p}.4.bias"]), _ptr(W[f"{p}.6.scale"]),
+                                            B, C_, Fr, L, hid, dil, _ptr(u_in) if u_in is not None else None, _ptr(work), _stream()), "dconv_f32")
+                continue
+            h = conv2d(x, W[f"{p}.0.weight"], W[f"{p}.0.bias"], hid, (1, 3), p=(0, dil), dw=dil, math=self.math)
+            groupnorm1(h, W[f"{p}.1.weight"], W[f"{p}.1.bias"], ACT_GELU)
+            h = conv2d(h, W[f"{p}.3.weight"], W[f"{p}.3.bias"], 2 * C_, (1, 1), math=self.math)
+            groupnorm1(h, W[f"{p}.4.weight"], W[f"{p}.4.bias"])
+            x = glu(h, res=x, scale=W[f"{p}.6.scale"])
+        return x
+
+    def spec_in(self, mix, pad_mode):
+        """_spec + _magnitude and the input normalisation (htdemucs.py:383-403, :415-424, :501-510; hdemucs.py:529-548, :570-579) on mix
+        (B, 2, L) contiguous: the normalised STFT, frames 2 .. 2+le of the (3*hop/2, 3*hop/2 + le*hop - L)-padded signal (pad_mode 0 reflect, 1 zero),
+        bins 0 .. nfft/2-1.  -> x (B, 4, nfft/2, le) and xt (B, 2, 1, L), standardised per sample, and stats (B, 4): per sample the mean and std of
+        the spectrogram, then of the waveform."""
+        B, _, length = mix.shape
+        hl, nfft = self.cfg.hop, self.cfg.nfft
+        le = -(-length // hl)
+        Fq = nfft // 2
+        spec = _new((B, 4, Fq, le), mix)
+        check(lib.b200sep_stft_forward_ex(self.stft.handle, _ptr(mix), 2 * length, length, 0, B, length, le, hl // 2 * 3, 1.0 / math.sqrt(nfft), Fq, 0, LAYOUT_CFT,
+                                          pad_mode, _ptr(spec), _stream()), "stft_forward_ex")
+        stats = _new((B, 4), mix)
+        x = _new(spec.shape, mix)
+        xt = _new((B, 2, 1, length), mix)
+        fs = 4
+        mswork = _new((lib.b200sep_meanstd_work_floats(B),), mix)
+        check(lib.b200sep_meanstd_batch_f32(_ptr(spec), spec[0].numel(), B, spec[0].numel(), _ptr(stats), 4, _ptr(mswork), _stream()), "meanstd_batch_f32")
+        check(lib.b200sep_meanstd_batch_f32(_ptr(mix), mix[0].numel(), B, mix[0].numel(), stats.data_ptr() + 2 * fs, 4, _ptr(mswork), _stream()), "meanstd_batch_f32")
+        for b in range(B):
+            check(lib.b200sep_ew_f32(_ptr(spec[b]), stats.data_ptr() + (4 * b) * fs, _ptr(x[b]), spec[b].numel(), 1.0, 0.0, 2, _stream()), "ew_f32")
+            check(lib.b200sep_ew_f32(_ptr(mix[b]), stats.data_ptr() + (4 * b + 2) * fs, _ptr(xt[b]), mix[b].numel(), 1.0, 0.0, 2, _stream()), "ew_f32")
+        return x, xt, stats
+
+    def spec_out(self, x, xt, stats, length, ola_offset):
+        """The output end (htdemucs.py:405-413; hdemucs.py:550-568): x (B, S*4, nfft/2, le) * std + mean -> _mask (cac) -> _ispec, an
+        iSTFT with the Nyquist bin and two frames per side zero whose overlap-add starts at sample ola_offset, plus the time branch xt * std + mean
+        -> (B, S, 2, length).  De-normalises x and xt in place."""
+        S = self.S
+        B, _, Fq, le = x.shape
+        out = _new((B, S, 2, length), x)
+        nwork = lib.b200sep_stft_inverse_work_floats(self.stft.handle, S, le, Fq, LAYOUT_CFT)
+        work = _new((nwork,), x)
+        xi = _new((S, 2, length), x)
+        fs = 4
+        for b in range(B):
+            check(lib.b200sep_ew_f32(_ptr(x[b]), stats.data_ptr() + (4 * b) * fs, _ptr(x[b]), x[b].numel(), 1.0, 0.0, 3, _stream()), "ew_f32")
+            check(lib.b200sep_stft_inverse_ex(self.stft.handle, _ptr(x[b]), S, le, Fq, LAYOUT_CFT, length, ola_offset, 2, math.sqrt(self.cfg.nfft), _ptr(xi), _ptr(work),
+                                              _stream()), "stft_inverse_ex")
+            check(lib.b200sep_ew_f32(_ptr(xt[b]), stats.data_ptr() + (4 * b + 2) * fs, _ptr(out[b]), xt[b].numel(), 1.0, 0.0, 3, _stream()), "ew_f32")
+            ew(out[b], xi, out[b])
+        return out
+
+
+class HTDemucsNet(HybridDemucsNet):
+    """Device-resident HTDemucs weights (re-blocked for the conv kernel) + the launch sequence of one forward."""
+
+    def __init__(self, cfg: HTDemucsConfig, state: dict, device=None, math=MATH_BF16X3):
+        super().__init__(cfg, device, math)
         st = {k: np.asarray(v, dtype=np.float32) for k, v in state.items()}
         self._check_structure(st)
         for name, a in st.items():
             if ".dconv.layers." in name and name.endswith((".0.weight", ".3.weight")):  # the fused DConv kernel takes the plain (out, in[, k]) matrices
-                self.W[name + ":raw"] = torch.from_numpy(np.ascontiguousarray(a.reshape(a.shape[0], -1) if name.endswith(".3.weight") else a)).to(self.device)
+                self._put(name + ":raw", a.reshape(a.shape[0], -1) if name.endswith(".3.weight") else a)
             if name.endswith("conv_tr.weight"):
                 a = block_convtr_weight(a.reshape(a.shape[0], a.shape[1], cfg.kernel_size), cfg.stride)
             elif name.endswith(".weight") and a.ndim >= 3 and "crosstransformer" not in name:
@@ -269,12 +211,12 @@ class HTDemucsNet:
                 D = a.shape[0] // 3
                 kind = "weight" if name.endswith("weight") else "bias"
                 for j, nm in enumerate("qkv"):
-                    self.W[name.replace(f"in_proj_{kind}", f"{nm}_{kind}")] = torch.from_numpy(np.ascontiguousarray(a[j * D : (j + 1) * D])).to(self.device)
+                    self._put(name.replace(f"in_proj_{kind}", f"{nm}_{kind}"), a[j * D : (j + 1) * D])
                 continue
-            self.W[name] = torch.from_numpy(np.ascontiguousarray(a)).to(self.device)
+            self._put(name, a)
         # ScaledEmbedding.forward * freq_emb weight (hdemucs.py:62-64, htdemucs.py:539-541): added after encoder 0, shape (C, Fr)
         emb = st["freq_emb.embedding.weight"] * np.float32(cfg.emb_scale)  # (Fr, C)
-        self.freq_emb_t = torch.from_numpy(np.ascontiguousarray((np.float32(cfg.freq_emb) * emb).T)).to(self.device)
+        self.freq_emb_t = to_device((np.float32(cfg.freq_emb) * emb).T, self.device)
         self._pe_cache = {}
         self._emb_cache = {}
         from .graphs import GraphedForward
@@ -306,34 +248,6 @@ class HTDemucsNet:
             raise ValueError("config.bottom_channels does not match the checkpoint")
 
     # ---- sub-graphs --------------------------------------------------------------------------------------------
-    def _dconv(self, x, prefix):
-        """DConv.forward (demucs.py:166-168) on x (B,C,Fr,T): conv1d k3 dilated -> GroupNorm(1)+GELU -> 1x1 -> GroupNorm(1) -> GLU, LayerScale residual."""
-        W = self.W
-        C_ = x.shape[1]
-        if f"{prefix}.dconv.layers.0.0.weight" not in W:  # dconv_mode without DConv on this side (hdemucs.py:83-84, :268-269)
-            return x
-        B, _, Fr, L = x.shape
-        for d in range(self.cfg.dconv_depth):
-            p = f"{prefix}.dconv.layers.{d}"
-            dil = 2**d
-            hid = W[f"{p}.0.bias"].numel()
-            if hid in _DCONV_FUSED_HID and C_ * 2 * (-(-hid // 4) * 4 + 4) * 4 <= 200 * 1024:
-                # one fused residual layer (csrc/dconv_fused.cu); the C -> hid convolution of the widest layers stays on the tensor cores
-                u_in = None
-                if 3 * C_ * (-(-hid // 4) * 4) * 4 > 200 * 1024:
-                    u_in = conv2d(x, W[f"{p}.0.weight"], W[f"{p}.0.bias"], hid, (1, 3), p=(0, dil), dw=dil, math=self.math)
-                work = _new((lib.b200sep_dconv_work_floats(B, C_, Fr, L, hid),), x)
-                check(lib.b200sep_dconv_f32(_ptr(x), _ptr(x), _ptr(W[f"{p}.0.weight:raw"]), _ptr(W[f"{p}.0.bias"]), _ptr(W[f"{p}.1.weight"]), _ptr(W[f"{p}.1.bias"]),
-                                            _ptr(W[f"{p}.3.weight:raw"]), _ptr(W[f"{p}.3.bias"]), _ptr(W[f"{p}.4.weight"]), _ptr(W[f"{p}.4.bias"]), _ptr(W[f"{p}.6.scale"]),
-                                            B, C_, Fr, L, hid, dil, _ptr(u_in) if u_in is not None else None, _ptr(work), _stream()), "dconv_f32")
-                continue
-            h = conv2d(x, W[f"{p}.0.weight"], W[f"{p}.0.bias"], hid, (1, 3), p=(0, dil), dw=dil, math=self.math)
-            groupnorm1(h, W[f"{p}.1.weight"], W[f"{p}.1.bias"], ACT_GELU)
-            h = conv2d(h, W[f"{p}.3.weight"], W[f"{p}.3.bias"], 2 * C_, (1, 1), math=self.math)
-            groupnorm1(h, W[f"{p}.4.weight"], W[f"{p}.4.bias"])
-            x = glu(h, res=x, scale=W[f"{p}.6.scale"])
-        return x
-
     def _enc(self, x, prefix, freq):
         """HEncLayer.forward (hdemucs.py:119-153), norm = Identity, empty = False."""
         W, cfg = self.W, self.cfg
@@ -376,7 +290,7 @@ class HTDemucsNet:
         # V^T per batch: (D, Lk) = Wv (D,D) @ kv^T, bias per row
         vt = _new((B, D, Lk), q_in)
         wv, bv = W[f"{p}.v_weight"], W[f"{p}.v_bias"]
-        _gemm_raw(_ptr(wv), _ptr(kv_in), _ptr(vt), D, Lk, D, D, D, Lk, B, 0, Lk * D, D * Lk, bias_m=_ptr(bv), math=self.math)
+        gemm(_ptr(wv), _ptr(kv_in), _ptr(vt), D, Lk, D, D, D, Lk, B, 0, Lk * D, D * Lk, bias_m=_ptr(bv), math=self.math)
         o = _new((B, Lq, D), q_in)
         if hd == 64:  # one kernel, the (H, Lq, Lk) scores stay on chip
             work = _new((lib.b200sep_attention_work_floats_math(B, H, Lq, Lk, self.math),), q_in)  # tile images of Q, K, V^T (split once, not once per consumer)
@@ -387,9 +301,9 @@ class HTDemucsNet:
         sc = _new((H, Lq, Lk), q_in)
         fs = 4  # bytes per float
         for b in range(B):
-            _gemm_raw(q.data_ptr() + b * Lq * D * fs, k.data_ptr() + b * Lk * D * fs, _ptr(sc), Lq, Lk, hd, D, D, Lk, H, hd, hd, Lq * Lk, alpha=1.0 / math.sqrt(hd), math=self.math)
+            gemm(q.data_ptr() + b * Lq * D * fs, k.data_ptr() + b * Lk * D * fs, _ptr(sc), Lq, Lk, hd, D, D, Lk, H, hd, hd, Lq * Lk, alpha=1.0 / math.sqrt(hd), math=self.math)
             check(lib.b200sep_softmax_rows_f32(_ptr(sc), H * Lq, Lk, Lk, _stream()), "softmax_rows_f32")
-            _gemm_raw(_ptr(sc), vt.data_ptr() + b * D * Lk * fs, o.data_ptr() + b * Lq * D * fs, Lq, hd, Lk, Lk, Lk, D, H, Lq * Lk, hd * Lk, hd, math=self.math)
+            gemm(_ptr(sc), vt.data_ptr() + b * D * Lk * fs, o.data_ptr() + b * Lq * D * fs, Lq, hd, Lk, Lk, Lk, D, H, Lq * Lk, hd * Lk, hd, math=self.math)
         y = linear(o.view(B * Lq, D), W[f"{p}.out_proj.weight"], W[f"{p}.out_proj.bias"], res=res.view(B * Lq, D), res_scale=res_scale, math=self.math)
         return y.view(B, Lq, D)
 
@@ -464,7 +378,7 @@ class HTDemucsNet:
     def forward(self, mix: torch.Tensor) -> torch.Tensor:
         """mix (B, 2, L <= seg_len) float32 cuda -> (B, S, 2, L).  (eval mode, use_train_segment: shorter inputs are zero-padded
         to the training segment and the output is cut back, htdemucs.py:486-493, :614-618.)"""
-        cfg, S = self.cfg, self.S
+        cfg = self.cfg
         assert mix.dim() == 3 and mix.shape[1] == 2 and mix.dtype == torch.float32 and mix.is_cuda
         B, _, L0 = mix.shape
         T_len = cfg.seg_len
@@ -475,23 +389,7 @@ class HTDemucsNet:
             mp[..., :L0].copy_(mix)
         else:
             mp = mix.contiguous()
-        hl, nfft = cfg.hop, cfg.nfft
-        le = -(-T_len // hl)
-        Fq = nfft // 2
-        # _spec + _magnitude (htdemucs.py:383-403, :415-424): normalized STFT, frames 2..2+le of the 3*hop/2-reflect-padded signal, bins 0..nfft/2-1
-        spec = _new((B, 4, Fq, le), mp)
-        check(lib.b200sep_stft_forward_ex(self.stft.handle, _ptr(mp), 2 * T_len, T_len, 0, B, T_len, le, hl // 2 * 3, 1.0 / math.sqrt(nfft), Fq, 0, LAYOUT_CFT,
-                                          0, _ptr(spec), _stream()), "stft_forward_ex")
-        stats = _new((B, 4), mp)  # per sample: mean, std of the spectrogram; mean, std of the waveform
-        x = _new(spec.shape, mp)
-        xt = _new((B, 2, 1, T_len), mp)
-        fs = 4
-        mswork = _new((lib.b200sep_meanstd_work_floats(B),), mp)
-        check(lib.b200sep_meanstd_batch_f32(_ptr(spec), spec[0].numel(), B, spec[0].numel(), _ptr(stats), 4, _ptr(mswork), _stream()), "meanstd_batch_f32")
-        check(lib.b200sep_meanstd_batch_f32(_ptr(mp), mp[0].numel(), B, mp[0].numel(), stats.data_ptr() + 2 * fs, 4, _ptr(mswork), _stream()), "meanstd_batch_f32")
-        for b in range(B):
-            check(lib.b200sep_ew_f32(_ptr(spec[b]), stats.data_ptr() + (4 * b) * fs, _ptr(x[b]), spec[b].numel(), 1.0, 0.0, 2, _stream()), "ew_f32")
-            check(lib.b200sep_ew_f32(_ptr(mp[b]), stats.data_ptr() + (4 * b + 2) * fs, _ptr(xt[b]), mp[b].numel(), 1.0, 0.0, 2, _stream()), "ew_f32")
+        x, xt, stats = self.spec_in(mp, 0)  # reflect-padded
         saved, saved_t, lengths_t = [], [], []
         for i in range(cfg.depth):  # htdemucs.py:520-544 (every time encoder runs: no "empty" layers at depth 4)
             lengths_t.append(xt.shape[-1])
@@ -510,17 +408,7 @@ class HTDemucsNet:
             last = j == cfg.depth - 1
             x = self._dec(x, saved.pop(-1), 0, f"decoder.{j}", True, last)
             xt = self._dec(xt, saved_t.pop(-1), lengths_t.pop(-1), f"tdecoder.{j}", False, last)
-        # x (B, S*4, Fq, le) * std + mean -> _mask (cac) -> _ispec (:405-413): iSTFT with the Nyquist bin and two frames per side zero
-        out = _new((B, S, 2, T_len), mp)
-        nwork = lib.b200sep_stft_inverse_work_floats(self.stft.handle, S, le, Fq, LAYOUT_CFT)
-        work = _new((nwork,), mp)
-        xi = _new((S, 2, T_len), mp)
-        for b in range(B):
-            check(lib.b200sep_ew_f32(_ptr(x[b]), stats.data_ptr() + (4 * b) * fs, _ptr(x[b]), x[b].numel(), 1.0, 0.0, 3, _stream()), "ew_f32")
-            check(lib.b200sep_stft_inverse_ex(self.stft.handle, _ptr(x[b]), S, le, Fq, LAYOUT_CFT, T_len, hl // 2 * 3, 2, math.sqrt(nfft), _ptr(xi), _ptr(work), _stream()),
-                  "stft_inverse_ex")
-            check(lib.b200sep_ew_f32(_ptr(xt[b]), stats.data_ptr() + (4 * b + 2) * fs, _ptr(out[b]), xt[b].numel(), 1.0, 0.0, 3, _stream()), "ew_f32")
-            ew(out[b], xi, out[b])
+        out = self.spec_out(x, xt, stats, T_len, cfg.hop // 2 * 3)
         return out[..., :L0] if L0 < T_len else out
 
     def _freq_emb_full(self, Fr, Tt, Cc):

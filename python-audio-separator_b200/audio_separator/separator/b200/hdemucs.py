@@ -10,15 +10,16 @@ Graph builder only: device buffers and the ORDER of the operator launches; every
 """
 from __future__ import annotations
 
-import math
 from dataclasses import dataclass
 
 import numpy as np
 import torch
 
-from ._lib import LAYOUT_CFT, MATH_BF16X3, check, lib
-from .demucs import (ACT_GELU, ACT_NONE, HTDemucsNet, _gemm_raw, _new, block_conv_weight, block_convtr_weight, conv2d, conv_transpose, ew, glu, groupnorm1, linear)
-from .engine import StftPlan, _ptr, _require_cuda, _stream
+from ._lib import MATH_BF16X3, check, lib
+from .demucs import HybridDemucsNet
+from .engine import _ptr, _stream
+from .ops import (ACT_GELU, ACT_NONE, _new, block_conv_weight, block_convtr_weight, conv2d, conv_transpose, ew, glu, groupnorm, groupnorm1, linear, lstm_bidir,
+                  lstm_bidir_weights)
 
 
 @dataclass
@@ -107,26 +108,11 @@ def layer_plan(cfg: HDemucsConfig):
     return plan
 
 
-def groupnorm(x, groups, gamma, beta, act=ACT_NONE):
-    """nn.GroupNorm(groups, C) in place on contiguous channel-first x (B, C, ...)."""
-    B, C = x.shape[:2]
-    X = x[0, 0].numel()
-    work = _new((lib.b200sep_groupnorm_work_floats(B, C, groups, X),), x)
-    check(lib.b200sep_groupnorm_f32(_ptr(x), _ptr(gamma), _ptr(beta), _ptr(x), B, C, groups, X, act, _ptr(work), _stream()), "groupnorm_f32")
-    return x
+class HDemucsNet(HybridDemucsNet):
+    """Device-resident HDemucs weights + the launch sequence of one forward."""
 
-
-class HDemucsNet(HTDemucsNet):
-    """Device-resident HDemucs weights + the launch sequence of one forward.  (Sub-classes HTDemucsNet for its plain DConv branch.)"""
-
-    def __init__(self, cfg: HDemucsConfig, state: dict, device=None, math=MATH_BF16X3):  # noqa: super().__init__ builds the HTDemucs graph; this class has its own
-        _require_cuda()
-        cfg.validate()
-        self.cfg = cfg
-        self.math = int(math)  # as HTDemucsNet
-        self.device = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
-        self.S = len(cfg.sources)
-        self.stft = StftPlan(cfg.nfft, cfg.hop)
+    def __init__(self, cfg: HDemucsConfig, state: dict, device=None, math=MATH_BF16X3):
+        super().__init__(cfg, device, math)
         self.plan = layer_plan(cfg)
         self.encs = [(f"encoder.{i}", P["enc"]) for i, P in enumerate(self.plan)]
         self.decs = [(f"decoder.{j}", P["dec"]) for j, P in enumerate(self.plan[::-1])]
@@ -136,44 +122,28 @@ class HDemucsNet(HTDemucsNet):
         self.tdecs = [(f"tdecoder.{j}", L) for j, L in enumerate(tdecs)]
         st = {k: np.asarray(v, dtype=np.float32) for k, v in state.items()}
         self._check_structure(st)
-        self.W = {}
-
-        def put(name, a):
-            self.W[name] = torch.from_numpy(np.ascontiguousarray(a, dtype=np.float32)).to(self.device)
-
         for name, a in st.items():
             if ".lstm." in name:
                 continue  # repacked below
             if ".dconv.layers." in name and name.endswith((".0.weight", ".3.weight")) and a.ndim == 3 and a.shape[-1] in (1, 3):
                 # the fused plain DConv kernel takes the (out, in[, k]) matrices as they are (layers without LSTM / LocalState: index 3 is the 1x1)
-                put(name + ":raw", a.reshape(a.shape[0], -1) if name.endswith(".3.weight") else a)
+                self._put(name + ":raw", a.reshape(a.shape[0], -1) if name.endswith(".3.weight") else a)
             if name.endswith("conv_tr.weight"):
                 a = block_convtr_weight(a.reshape(a.shape[0], a.shape[1], -1), a.reshape(a.shape[0], a.shape[1], -1).shape[2] // 2)
             elif name.endswith(".linear.weight"):
                 pass  # BLSTM.linear: a plain (out, in) matrix for gemm_f32
             elif name.endswith(".weight") and a.ndim >= 3:
                 a = block_conv_weight(a if a.ndim == 4 else a.reshape(a.shape[0], a.shape[1], 1, a.shape[2]))
-            put(name, a)
-        # nn.LSTM parameters -> per layer: input projections of both directions (biases summed), recurrent matrices in both kernel layouts
-        for name in st:
-            if not name.endswith(".lstm.weight_ih_l0"):
-                continue
-            p = name[: -len(".weight_ih_l0")]
-            for layer in range(cfg.lstm_layers):
-                whh = []
-                for d, sfx in enumerate(("", "_reverse")):
-                    put(f"{p}.wih{layer}{d}", st[f"{p}.weight_ih_l{layer}{sfx}"])
-                    put(f"{p}.b{layer}{d}", st[f"{p}.bias_ih_l{layer}{sfx}"].astype(np.float64) + st[f"{p}.bias_hh_l{layer}{sfx}"].astype(np.float64))
-                    whh.append(st[f"{p}.weight_hh_l{layer}{sfx}"])
-                hid = whh[0].shape[1]
-                if hid <= 96:
-                    put(f"{p}.whh{layer}", np.stack(whh))  # (2, 4*hid, hid): lstm_bidir_f32
-                else:
-                    put(f"{p}.whh_t{layer}", np.stack([w.T for w in whh]))  # (2, hid, 4*hid): lstm_bidir_wide_f32
+            self._put(name, a)
+        for name in st:  # nn.LSTM parameters, per layer
+            if name.endswith(".lstm.weight_ih_l0"):
+                p = name[: -len(".weight_ih_l0")]
+                for layer in range(cfg.lstm_layers):
+                    self.W[f"{p}.{layer}"] = lstm_bidir_weights(st, p, layer, self.device)
         if cfg.freq_emb:
             # ScaledEmbedding.forward * freq_emb_scale (hdemucs.py:62-64, :708-713) as one value per (channel, frequency) row
             emb = st["freq_emb.embedding.weight"] * np.float32(cfg.emb_scale)  # (Fr, C)
-            put("freq_emb:rows", (np.float32(cfg.freq_emb) * emb).T.reshape(-1))
+            self._put("freq_emb:rows", (np.float32(cfg.freq_emb) * emb).T.reshape(-1))
         self.graphed = self.forward  # variable lengths: launched directly
 
     def _check_structure(self, st):
@@ -213,17 +183,7 @@ class HDemucsNet(HTDemucsNet):
         check(lib.b200sep_lstm_frames_gather_f32(_ptr(h), _ptr(fr), B, C, T, nf, width, stride, _stream()), "lstm_frames_gather_f32")
         x2 = fr.view(width * N, C)
         for layer in range(cfg.lstm_layers):
-            K = x2.shape[1]
-            xp = _new((2, width * N, 4 * C), h)
-            for d in range(2):
-                wih = W[f"{p}.lstm.wih{layer}{d}"]
-                _gemm_raw(_ptr(x2), _ptr(wih), xp[d].data_ptr(), width * N, 4 * C, K, K, K, 4 * C, 1, 0, 0, 0, bias_n=_ptr(W[f"{p}.lstm.b{layer}{d}"]), math=self.math)
-            out = _new((width, N, 2 * C), h)
-            if C <= 96:
-                check(lib.b200sep_lstm_bidir_f32(_ptr(xp), _ptr(W[f"{p}.lstm.whh{layer}"]), _ptr(out), width, N, C, _stream()), "lstm_bidir_f32")
-            else:
-                check(lib.b200sep_lstm_bidir_wide_f32(_ptr(xp), _ptr(W[f"{p}.lstm.whh_t{layer}"]), _ptr(out), width, N, C, _stream()), "lstm_bidir_wide_f32")
-            x2 = out.view(width * N, 2 * C)
+            x2 = lstm_bidir(x2, N, W[f"{p}.lstm.{layer}"], self.math)
         lin = linear(x2, W[f"{p}.linear.weight"], W[f"{p}.linear.bias"], math=self.math)
         y = _new(h.shape, h)
         check(lib.b200sep_lstm_frames_scatter_f32(_ptr(lin), _ptr(h), _ptr(y), B, C, T, nf, width, stride if nf > 1 else 2, _stream()), "lstm_frames_scatter_f32")
@@ -243,7 +203,7 @@ class HDemucsNet(HTDemucsNet):
         return conv2d(res, W[f"{p}.proj.weight"], W[f"{p}.proj.bias"], C, (1, 1), add=h, math=self.math)
 
     def _dconv_layer(self, x, prefix, L):
-        """DConv.forward (demucs.py:166-168) for the layer kinds of this model: the plain branch of HTDemucsNet, or conv -> GroupNorm+GELU ->
+        """DConv.forward (demucs.py:166-168) for the layer kinds of this model: the plain branch (HybridDemucsNet._dconv), or conv -> GroupNorm+GELU ->
         BLSTM -> LocalState -> 1x1 -> GroupNorm -> GLU with the LayerScale residual."""
         if not (L["lstm"] or L["attn"]):
             return self._dconv(x, prefix)
@@ -336,28 +296,11 @@ class HDemucsNet(HTDemucsNet):
     # ---- forward -------------------------------------------------------------------------------------------------------------
     def forward(self, mix: torch.Tensor) -> torch.Tensor:
         """mix (B, 2, L) float32 cuda -> (B, S, 2, L)."""
-        cfg, S, W = self.cfg, self.S, self.W
+        cfg, W = self.cfg, self.W
         assert mix.dim() == 3 and mix.shape[1] == 2 and mix.dtype == torch.float32 and mix.is_cuda
         mp = mix.contiguous()
         B, _, length = mp.shape
-        hl, nfft = cfg.hop, cfg.nfft
-        le = -(-length // hl)
-        Fq = nfft // 2
-        pad = hl // 2 * 3
-        # _spec + _magnitude (hdemucs.py:529-548, :570-579): frames 2 .. 2+le of the (pad, pad + le*hl - length) reflect- (hybrid_old: zero-) padded signal
-        spec = _new((B, 4, Fq, le), mp)
-        check(lib.b200sep_stft_forward_ex(self.stft.handle, _ptr(mp), 2 * length, length, 0, B, length, le, pad, 1.0 / math.sqrt(nfft), Fq, 0, LAYOUT_CFT,
-                                          1 if cfg.hybrid_old else 0, _ptr(spec), _stream()), "stft_forward_ex")
-        stats = _new((B, 4), mp)  # per sample: mean, std of the spectrogram; mean, std of the waveform
-        x = _new(spec.shape, mp)
-        xt = _new((B, 2, 1, length), mp)
-        fs = 4
-        mswork = _new((lib.b200sep_meanstd_work_floats(B),), mp)
-        check(lib.b200sep_meanstd_batch_f32(_ptr(spec), spec[0].numel(), B, spec[0].numel(), _ptr(stats), 4, _ptr(mswork), _stream()), "meanstd_batch_f32")
-        check(lib.b200sep_meanstd_batch_f32(_ptr(mp), mp[0].numel(), B, mp[0].numel(), stats.data_ptr() + 2 * fs, 4, _ptr(mswork), _stream()), "meanstd_batch_f32")
-        for b in range(B):
-            check(lib.b200sep_ew_f32(_ptr(spec[b]), stats.data_ptr() + (4 * b) * fs, _ptr(x[b]), spec[b].numel(), 1.0, 0.0, 2, _stream()), "ew_f32")
-            check(lib.b200sep_ew_f32(_ptr(mp[b]), stats.data_ptr() + (4 * b + 2) * fs, _ptr(xt[b]), mp[b].numel(), 1.0, 0.0, 2, _stream()), "ew_f32")
+        x, xt, stats = self.spec_in(mp, 1 if cfg.hybrid_old else 0)  # hybrid_old: zero- instead of reflect-padded
         saved, saved_t, lengths, lengths_t = [], [], [], []
         for idx, (prefix, L) in enumerate(self.encs):  # hdemucs.py:697-716
             lengths.append(x.shape[-1])
@@ -387,17 +330,6 @@ class HDemucsNet(HTDemucsNet):
                 else:
                     xt, _ = self._dec_layer(xt, saved_t.pop(-1), length_t, tp, Lt)
         assert not saved and not saved_t and not lengths_t
-        # x (B, S*4, Fq, le) * std + mean -> _mask (cac) -> _ispec (hdemucs.py:550-568): iSTFT with the Nyquist bin and two frames per side zero
-        out = _new((B, S, 2, length), mp)
-        nwork = lib.b200sep_stft_inverse_work_floats(self.stft.handle, S, le, Fq, LAYOUT_CFT)
-        work = _new((nwork,), mp)
-        xi = _new((S, 2, length), mp)
-        for b in range(B):
-            check(lib.b200sep_ew_f32(_ptr(x[b]), stats.data_ptr() + (4 * b) * fs, _ptr(x[b]), x[b].numel(), 1.0, 0.0, 3, _stream()), "ew_f32")
-            check(lib.b200sep_stft_inverse_ex(self.stft.handle, _ptr(x[b]), S, le, Fq, LAYOUT_CFT, length, 0 if cfg.hybrid_old else pad, 2, math.sqrt(nfft), _ptr(xi), _ptr(work),
-                                              _stream()), "stft_inverse_ex")
-            check(lib.b200sep_ew_f32(_ptr(xt[b]), stats.data_ptr() + (4 * b + 2) * fs, _ptr(out[b]), xt[b].numel(), 1.0, 0.0, 3, _stream()), "ew_f32")
-            ew(out[b], xi, out[b])
-        return out
+        return self.spec_out(x, xt, stats, length, 0 if cfg.hybrid_old else cfg.hop // 2 * 3)
 
     __call__ = forward

@@ -17,11 +17,10 @@ import numpy as np
 import torch
 
 from ._lib import LAYOUT_CFT, MATH_BF16X3, check, lib
-from .demucs import ACT_GELU, ACT_NONE, _new, _packed_linear
 from .engine import StftPlan, _ptr, _require_cuda, _stream
+from .ops import ACT_GELU, ACT_NONE, ACT_TANH, _new, gemm, linear, to_device
 from .sharded import ShardRunner, plan_start_shards
 
-ACT_TANH = 5
 DEFAULT_FREQS_PER_BANDS = (2,) * 24 + (4,) * 12 + (12,) * 8 + (24,) * 8 + (48,) * 8 + (128, 129)
 
 
@@ -150,14 +149,6 @@ def mel_band_layout(cfg: "MelBandRoformerConfig"):
     return mask, idx.astype(np.int64), mask.sum(1), mask.sum(0)
 
 
-def gemm(a_ptr, w, c_ptr, M, lda, ldc, bias=None, act=ACT_NONE, res_ptr=None, math=MATH_BF16X3):
-    """rows x K (row stride lda) @ w (N, K)^T + bias -> rows x N at row stride ldc (+ res with the same strides)."""
-    N, K = w.shape
-    pk = _packed_linear(w, math)
-    check(lib.b200sep_gemm_f32_math(a_ptr, _ptr(w), c_ptr, M, N, K, lda, K, ldc, 1, 0, 0, 0, 1.0, _ptr(bias) if bias is not None else None, None, act, res_ptr, None,
-                                    _ptr(pk) if pk is not None else None, math, _stream()), "gemm_f32")
-
-
 def rmsnorm(x, gamma, rows, C, ld_in=None, out=None):
     y = out if out is not None else _new((rows, C), x)
     check(lib.b200sep_rmsnorm_f32(x.data_ptr() if isinstance(x, torch.Tensor) else x, _ptr(gamma), _ptr(y), rows, C, ld_in or C, C, _stream()), "rmsnorm_f32")
@@ -179,8 +170,7 @@ class BSRoformerNet:
         self.stft = StftPlan(cfg.stft_n_fft, cfg.stft_hop_length)
         self.W = {}
         for k, v in state.items():
-            a = np.asarray(v, dtype=np.float32) if not isinstance(v, torch.Tensor) else v.detach().to(torch.float32).numpy()
-            self.W[k] = torch.from_numpy(np.ascontiguousarray(a)).to(self.device)
+            self.W[k] = to_device(v.detach().to(torch.float32).numpy() if isinstance(v, torch.Tensor) else v, self.device)
         for n in ("band_split.to_features.0.1.weight", "layers.0.0.layers.0.0.to_qkv.weight", "mask_estimators.0.to_freqs.0.0.0.weight"):
             if n not in self.W:
                 raise ValueError(f"state dict lacks {n}: not a Roformer checkpoint")
@@ -213,8 +203,7 @@ class BSRoformerNet:
         for l in range(depth):
             a, f = f"{p}.layers.{l}.0", f"{p}.layers.{l}.1"
             xn = rmsnorm(x, W[f"{a}.norm.gamma"], rows, d)
-            qkv = _new((rows, 3 * inner), x)
-            gemm(_ptr(xn), W[f"{a}.to_qkv.weight"], _ptr(qkv), rows, d, 3 * inner, math=self.math)
+            qkv = linear(xn, W[f"{a}.to_qkv.weight"], None, math=self.math)
             q, k, v = _new((Bq, H, n, dh), x), _new((Bq, H, n, dh), x), _new((Bq, H, n, dh), x)
             check(lib.b200sep_rope_split_heads_f32(_ptr(qkv), _ptr(W[f"{a}.rotary_embed.freqs"]), _ptr(q), _ptr(k), _ptr(v), Bq, n, H, dh, _stream()), "rope_split_heads_f32")
             o = _new((Bq, H, n, dh), x)
@@ -224,22 +213,16 @@ class BSRoformerNet:
                                                      1, _ptr(work), self.math, _stream()), "attention_f32")
             else:
                 sc = _new((Bq * H, n, ldv), x)  # padding columns n..ldv-1 are never read: the P@V GEMM runs K = n over rows of stride ldv
-                check(lib.b200sep_gemm_f32_math(_ptr(q), _ptr(k), _ptr(sc), n, n, dh, dh, dh, ldv, Bq * H, n * dh, n * dh, n * ldv, dh**-0.5, None, None, 0, None, None,
-                                                None, self.math, _stream()), "gemm_f32(scores)")
+                gemm(_ptr(q), _ptr(k), _ptr(sc), n, n, dh, dh, dh, ldv, Bq * H, n * dh, n * dh, n * ldv, alpha=dh**-0.5, math=self.math)
                 check(lib.b200sep_softmax_rows_f32(_ptr(sc), Bq * H * n, n, ldv, _stream()), "softmax_rows_f32")
                 check(lib.b200sep_gemm_kn_f32(_ptr(sc), _ptr(v), _ptr(o), n, dh, n, ldv, dh, dh, Bq * H, n * ldv, n * dh, n * dh, 1.0, _stream()), "gemm_kn_f32(PV)")
-            gates = _new((rows, H), x)
-            gemm(_ptr(xn), W[f"{a}.to_gates.weight"], _ptr(gates), rows, d, H, bias=W[f"{a}.to_gates.bias"], math=self.math)
+            gates = linear(xn, W[f"{a}.to_gates.weight"], W[f"{a}.to_gates.bias"], math=self.math)
             merged = _new((rows, inner), x)
             check(lib.b200sep_gate_merge_heads_f32(_ptr(o), _ptr(gates), _ptr(merged), Bq, n, H, dh, _stream()), "gate_merge_heads_f32")
-            x2 = _new((rows, d), x)
-            gemm(_ptr(merged), W[f"{a}.to_out.0.weight"], _ptr(x2), rows, inner, d, res_ptr=_ptr(x), math=self.math)  # attn(x) + x
+            x2 = linear(merged, W[f"{a}.to_out.0.weight"], None, res=x, math=self.math)  # attn(x) + x
             hn = rmsnorm(x2, W[f"{f}.net.0.gamma"], rows, d)
-            hid = W[f"{f}.net.1.bias"].numel()
-            h = _new((rows, hid), x)
-            gemm(_ptr(hn), W[f"{f}.net.1.weight"], _ptr(h), rows, d, hid, bias=W[f"{f}.net.1.bias"], act=ACT_GELU, math=self.math)
-            x = _new((rows, d), x)
-            gemm(_ptr(h), W[f"{f}.net.4.weight"], _ptr(x), rows, hid, d, bias=W[f"{f}.net.4.bias"], res_ptr=_ptr(x2), math=self.math)  # ff(x) + x
+            h = linear(hn, W[f"{f}.net.1.weight"], W[f"{f}.net.1.bias"], act=ACT_GELU, math=self.math)
+            x = linear(h, W[f"{f}.net.4.weight"], W[f"{f}.net.4.bias"], res=x2, math=self.math)  # ff(x) + x
         if f"{p}.norm.gamma" in W:  # Transformer(norm_output=True): the Mel-Band variant (mel_band_roformer.py:82-101)
             x = rmsnorm(x, W[f"{p}.norm.gamma"], rows, d)
         return x
@@ -266,7 +249,7 @@ class BSRoformerNet:
         off = 0
         for bi, d_in in enumerate(self.band_dims):  # BandSplit (bs_roformer.py:134-150)
             xn = rmsnorm(src.data_ptr() + off * 4, W[f"band_split.to_features.{bi}.0.gamma"], rows, d_in, ld_in=nfeat, out=_new((rows, d_in), spec))
-            gemm(_ptr(xn), W[f"band_split.to_features.{bi}.1.weight"], x.data_ptr() + bi * d * 4, rows, d_in, nb * d, bias=W[f"band_split.to_features.{bi}.1.bias"], math=self.math)
+            linear(xn, W[f"band_split.to_features.{bi}.1.weight"], W[f"band_split.to_features.{bi}.1.bias"], math=self.math, out=x.view(rows, nb * d)[:, bi * d : (bi + 1) * d])
             off += d_in
         for i in range(cfg.depth):
             xt = _new((b, nb, T, d), x)  # "b t f d -> (b f) t d"
@@ -280,17 +263,12 @@ class BSRoformerNet:
         for si in range(S):  # MaskEstimator (bs_roformer.py:165-190)
             off = 0
             for bi, d_in in enumerate(self.band_dims):
-                h_ptr, lda, kdim = xf.data_ptr() + bi * d * 4, nb * d, d
+                h = xf.view(rows, nb * d)[:, bi * d : (bi + 1) * d]
                 for li in range(self.n_mask_linear):  # BS: mask_estimator_depth linears, Mel-Band: depth + 1 (their MLP helpers differ)
                     p = f"mask_estimators.{si}.to_freqs.{bi}.0.{2 * li}"
-                    w = W[f"{p}.weight"]
-                    last = li == self.n_mask_linear - 1
-                    y = _new((rows, w.shape[0]), spec)
-                    gemm(h_ptr, w, _ptr(y), rows, lda, w.shape[0], bias=W[f"{p}.bias"], act=ACT_NONE if last else ACT_TANH, math=self.math)
-                    hold = y  # keeps the buffer alive while its raw pointer is in use
-                    h_ptr, lda = _ptr(y), w.shape[0]
+                    h = linear(h, W[f"{p}.weight"], W[f"{p}.bias"], act=ACT_NONE if li == self.n_mask_linear - 1 else ACT_TANH, math=self.math)
                 for bb in range(b):  # the mask tensor is (b, S, T, features): one row block per batch element
-                    check(lib.b200sep_glu_rows_f32(hold.data_ptr() + bb * T * 2 * d_in * 4, mask.data_ptr() + (((bb * S + si) * T) * nfeat + off) * 4, T, d_in, 2 * d_in, nfeat,
+                    check(lib.b200sep_glu_rows_f32(h.data_ptr() + bb * T * 2 * d_in * 4, mask.data_ptr() + (((bb * S + si) * T) * nfeat + off) * 4, T, d_in, 2 * d_in, nfeat,
                                                    _stream()), "glu_rows_f32")
                 off += d_in
         if self.mel:  # masks_summed / num_bands_per_freq (mel_band_roformer.py:306-318)

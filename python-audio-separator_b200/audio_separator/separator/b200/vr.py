@@ -22,12 +22,10 @@ import numpy as np
 import torch
 
 from ._lib import LAYOUT_CFT, MATH_BF16X3, check, lib
-from .demucs import ACT_NONE, ACT_RELU, _new, block_conv_weight, conv2d, ew, linear
 from .engine import StftPlan, _ptr, _require_cuda, _stream
+from .ops import ACT_LEAKY, ACT_RELU, ACT_SIGMOID, _new, block_conv_weight, conv2d, ew, linear, lstm_bidir, lstm_bidir_weights, to_device
 from .resample import resample, resample_poly_design  # noqa: F401  (resample_poly_design: the polyphase FIR, re-exported)
 from .sharded import ShardRunner, shard_patches
-
-ACT_LEAKY, ACT_SIGMOID = 3, 4
 NON_ACCOM_STEMS = ("Vocals", "Other", "Bass", "Drums", "Guitar", "Piano", "Synthesizer", "Strings", "Woodwinds", "Brass", "Wind Inst")  # common_separator.py:55
 NN_ARCH_SIZES = (31191, 33966, 56817, 123821, 123812, 129605, 218409, 537238, 537227)  # vr_separator.py:166
 VR_51_SIZES = (56817, 218409)
@@ -117,30 +115,24 @@ def capacity(nn_architecture: int):
     raise NotImplementedError(f"nn_architecture {nn_architecture}: only CascadedASPPNet sizes are covered (VR 5.1 CascadedNet is not)")
 
 
-class VRNet:
-    """CascadedASPPNet in eval mode: BatchNorm folded into the preceding (bias-free) convolution, Dropout = identity."""
+class VRNetBase:
+    """What the VR networks share (VRNet, VRNet51): eval mode with BatchNorm folded into the preceding (bias-free) convolution, Dropout =
+    identity; the convolution + BatchNorm + activation block, the decoder step and the cropping of predict_mask."""
 
-    def __init__(self, nn_architecture: int, n_fft_bins: int, state: dict, device=None, math=MATH_BF16X3):
+    def __init__(self, n_fft_bins: int, offset: int, device=None, math=MATH_BF16X3):
         """math: MATH_BF16X3 (default, ~fp32) or MATH_FP16 (torch.autocast precision) for every tensor-core convolution / GEMM of this net."""
         _require_cuda()
         self.math = int(math)
-        self.arch = int(nn_architecture)
-        self.c1, self.cb, self.c2, self.c3 = capacity(self.arch)
-        self.n_enc = 5 if self.arch == 129605 else 4
-        self.n_extra = 1 if self.arch == 129605 else (2 if self.arch in (537238, 537227, 33966) else 0)
-        self.max_bin, self.output_bin, self.offset = n_fft_bins // 2, n_fft_bins // 2 + 1, 128
+        self.max_bin, self.output_bin, self.offset = n_fft_bins // 2, n_fft_bins // 2 + 1, offset
         self.device = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())  # one process per GPU: the rank's own device
-        st = {k: np.asarray(v) for k, v in state.items()}
         self.W = {}
+
+    def _load(self, state):
+        """Uploads the folded convolutions and the output convolution; returns the state as host arrays for what a net adds."""
+        st = {k: np.asarray(v) for k, v in state.items()}
         self._fold_all(st)
-        for nm in ("out",):
-            self._put(nm + ".w", block_conv_weight(st[nm + ".weight"].astype(np.float32)))
-        need = ["stg1_low_band_net.enc1.conv1.w", "stg3_full_band_net.dec1.conv.w", "stg2_bridge.w", "out.w", "stg1_low_band_net.aspp.conv3.dw"]
-        for n in need:
-            if n not in self.W:
-                raise ValueError(f"state dict lacks {n.rsplit('.', 1)[0]}: not a CascadedASPPNet checkpoint")
-        if self.W["stg1_low_band_net.enc1.conv1.b"].numel() != self.c1:
-            raise ValueError("checkpoint width does not match the capacity of its nn_architecture size")
+        self._put("out.w", block_conv_weight(st["out.weight"].astype(np.float32)))
+        return st
 
     def _fold_all(self, st):
         for name in st:
@@ -154,7 +146,7 @@ class VRNet:
                 self._fold(p, st[name], st, p + ".conv.1")
 
     def _put(self, name, a):
-        self.W[name] = torch.from_numpy(np.ascontiguousarray(a)).to(self.device)
+        self.W[name] = to_device(a, self.device)
 
     def _fold(self, p, w, st, bn):
         inv = st[bn + ".weight"].astype(np.float64) / np.sqrt(st[bn + ".running_var"].astype(np.float64) + 1e-5)
@@ -170,6 +162,45 @@ class VRNet:
         pad = (dil[0] * (k // 2), dil[1] * (k // 2))  # Conv2DBNActiv(..., pad=dilation, dilation=dilation) in the ASPP modules
         return conv2d(x, self.W[p + ".w"], self.W[p + ".b"], cout, (k, k), s=(stride, stride), p=pad, dw=dil[1], dh=dil[0], act=act, out=out, out_c_off=out_c_off,
                       math=self.math)
+
+    def _dec(self, x, skip, conv):
+        """Decoder: x up-sampled 2x (bilinear, align_corners), the skip cropped to its width concatenated on the channels, then the block `conv`."""
+        B, C, H, W = x.shape
+        Cs, Hs, Ws = skip.shape[1:]
+        if Hs != 2 * H or Ws < 2 * W:
+            raise ValueError(f"decoder skip {tuple(skip.shape)} does not fit the up-sampled {(B, C, 2 * H, 2 * W)} (the reference fails here too)")
+        cat = _new((B, C + Cs, 2 * H, 2 * W), x)
+        check(lib.b200sep_upsample2x_bilinear_f32(_ptr(x), _ptr(cat), B, C, H, W, C + Cs, 0, _stream()), "upsample2x_bilinear_f32")
+        d = (Ws - 2 * W) // 2  # crop_center: time axis (spec_utils.py:50-71)
+        copy_view(skip[:, :, :, d : d + 2 * W], cat[:, C:])
+        return self._cba(cat, conv)
+
+    def predict_mask(self, x: torch.Tensor) -> torch.Tensor:
+        m = self.forward(x)
+        if self.offset > 0:
+            B, _, nb, Wd = m.shape
+            out = _new((B, 2, nb, Wd - 2 * self.offset), m)
+            copy_view(m[:, :, :, self.offset : Wd - self.offset], out)
+            return out
+        return m
+
+
+class VRNet(VRNetBase):
+    """CascadedASPPNet in eval mode."""
+
+    def __init__(self, nn_architecture: int, n_fft_bins: int, state: dict, device=None, math=MATH_BF16X3):
+        super().__init__(n_fft_bins, 128, device, math)
+        self.arch = int(nn_architecture)
+        self.c1, self.cb, self.c2, self.c3 = capacity(self.arch)
+        self.n_enc = 5 if self.arch == 129605 else 4
+        self.n_extra = 1 if self.arch == 129605 else (2 if self.arch in (537238, 537227, 33966) else 0)
+        self._load(state)
+        need = ["stg1_low_band_net.enc1.conv1.w", "stg3_full_band_net.dec1.conv.w", "stg2_bridge.w", "out.w", "stg1_low_band_net.aspp.conv3.dw"]
+        for n in need:
+            if n not in self.W:
+                raise ValueError(f"state dict lacks {n.rsplit('.', 1)[0]}: not a CascadedASPPNet checkpoint")
+        if self.W["stg1_low_band_net.enc1.conv1.b"].numel() != self.c1:
+            raise ValueError("checkpoint width does not match the capacity of its nn_architecture size")
 
     def _sep(self, x, p, dil, out, out_c_off):
         B, C, H, W = x.shape
@@ -192,17 +223,6 @@ class VRNet:
             self._sep(x, f"{p}.conv{6 + i}", 16, cat, C * (5 + i))
         return self._cba(cat, p + ".bottleneck.0")
 
-    def _dec(self, x, skip, p):
-        B, C, H, W = x.shape
-        Cs, Hs, Ws = skip.shape[1:]
-        if Hs != 2 * H or Ws < 2 * W:
-            raise ValueError(f"decoder skip {tuple(skip.shape)} does not fit the up-sampled {(B, C, 2 * H, 2 * W)} (the reference fails here too)")
-        cat = _new((B, C + Cs, 2 * H, 2 * W), x)
-        check(lib.b200sep_upsample2x_bilinear_f32(_ptr(x), _ptr(cat), B, C, H, W, C + Cs, 0, _stream()), "upsample2x_bilinear_f32")
-        d = (Ws - 2 * W) // 2  # crop_center: time axis (spec_utils.py:50-71)
-        copy_view(skip[:, :, :, d : d + 2 * W], cat[:, C:])
-        return self._cba(cat, p + ".conv")
-
     def _base(self, x, p):
         skips = []
         for i in range(1, self.n_enc + 1):
@@ -211,7 +231,7 @@ class VRNet:
             skips.append(s)
         x = self._aspp(x, f"{p}.aspp")
         for i in range(self.n_enc, 0, -1):
-            x = self._dec(x, skips[i - 1], f"{p}.dec{i}")
+            x = self._dec(x, skips[i - 1], f"{p}.dec{i}.conv")
         return x
 
     def forward(self, x: torch.Tensor) -> torch.Tensor:
@@ -238,44 +258,26 @@ class VRNet:
         copy_view(m[:, :, mb - 1 : mb].expand(B, 2, self.output_bin - mb, Wd), mask[:, :, mb:])  # F.pad(mode="replicate") on the bin axis
         return mask
 
-    def predict_mask(self, x: torch.Tensor) -> torch.Tensor:
-        m = self.forward(x)
-        if self.offset > 0:
-            B, _, nb, Wd = m.shape
-            out = _new((B, 2, nb, Wd - 2 * self.offset), m)
-            copy_view(m[:, :, :, self.offset : Wd - self.offset], out)
-            return out
-        return m
 
-
-class VRNet51(VRNet):
+class VRNet51(VRNetBase):
     """CascadedNet of VR 5.1 (vr_network/nets_new.py:52-160, layers_new.py): five band nets with stride-2 encoders, an ASPP of dilated 3x3 convolutions
     (dilations (4,2), (8,4), (12,6)) and a bidirectional-LSTM branch over the time axis in front of the last decoder; eval mode (BatchNorm folded)."""
 
     def __init__(self, n_fft_bins: int, nout: int, nout_lstm: int, state: dict, nn_arch_size: int = 56817, device=None, math=MATH_BF16X3):
-        _require_cuda()
-        self.math = int(math)  # as VRNet
+        super().__init__(n_fft_bins, 64, device, math)
         self.arch = int(nn_arch_size)
         self.nout = 64 if self.arch == 218409 else int(nout)
-        self.max_bin, self.output_bin, self.offset = n_fft_bins // 2, n_fft_bins // 2 + 1, 64
-        self.device = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())  # one process per GPU: the rank's own device
-        st = {k: np.asarray(v) for k, v in state.items()}
-        self.W = {}
-        self._fold_all(st)
-        self._put("out.w", block_conv_weight(st["out.weight"].astype(np.float32)))
-        for name in st:  # LSTMModule: both directions' input projections (biases summed), recurrent weights, dense + BatchNorm1d folded
+        st = self._load(state)
+        for name in st:  # LSTMModule: the bidirectional LSTM, dense + BatchNorm1d folded
             if not name.endswith(".lstm.weight_ih_l0"):
                 continue
             p = name[: -len(".lstm.weight_ih_l0")]
-            for d, sfx in enumerate(("", "_reverse")):
-                self._put(f"{p}.wih{d}", st[f"{p}.lstm.weight_ih_l0{sfx}"].astype(np.float32))
-                self._put(f"{p}.bih{d}", (st[f"{p}.lstm.bias_ih_l0{sfx}"].astype(np.float64) + st[f"{p}.lstm.bias_hh_l0{sfx}"].astype(np.float64)).astype(np.float32))
-            self._put(f"{p}.whh", np.stack([st[f"{p}.lstm.weight_hh_l0"], st[f"{p}.lstm.weight_hh_l0_reverse"]]).astype(np.float32))
+            self.W[f"{p}.lstm"] = lstm_bidir_weights(st, f"{p}.lstm", 0, self.device)
             inv = st[f"{p}.dense.1.weight"].astype(np.float64) / np.sqrt(st[f"{p}.dense.1.running_var"].astype(np.float64) + 1e-5)
             self._put(f"{p}.dense.w", (st[f"{p}.dense.0.weight"].astype(np.float64) * inv[:, None]).astype(np.float32))
             self._put(f"{p}.dense.b", ((st[f"{p}.dense.0.bias"].astype(np.float64) - st[f"{p}.dense.1.running_mean"].astype(np.float64)) * inv
                                        + st[f"{p}.dense.1.bias"].astype(np.float64)).astype(np.float32))
-        for n in ("stg1_low_band_net.0.enc1.w", "stg1_low_band_net.1.w", "stg3_full_band_net.lstm_dec2.whh", "stg3_full_band_net.dec1.conv1.w", "out.w"):
+        for n in ("stg1_low_band_net.0.enc1.w", "stg1_low_band_net.1.w", "stg3_full_band_net.lstm_dec2.lstm", "stg3_full_band_net.dec1.conv1.w", "out.w"):
             if n not in self.W:
                 raise ValueError(f"state dict lacks {n.rsplit('.', 1)[0]}: not a VR 5.1 CascadedNet checkpoint")
         if self.W["stg3_full_band_net.enc1.b"].numel() != self.nout:
@@ -283,17 +285,6 @@ class VRNet51(VRNet):
 
     def _enc(self, x, p, stride):
         return self._cba(self._cba(x, f"{p}.conv1", stride=stride, act=ACT_LEAKY), f"{p}.conv2", act=ACT_LEAKY)
-
-    def _dec51(self, x, skip, p):
-        B, C, H, W = x.shape
-        Cs, Hs, Ws = skip.shape[1:]
-        if Hs != 2 * H or Ws < 2 * W:
-            raise ValueError(f"decoder skip {tuple(skip.shape)} does not fit the up-sampled {(B, C, 2 * H, 2 * W)} (the reference fails here too)")
-        cat = _new((B, C + Cs, 2 * H, 2 * W), x)
-        check(lib.b200sep_upsample2x_bilinear_f32(_ptr(x), _ptr(cat), B, C, H, W, C + Cs, 0, _stream()), "upsample2x_bilinear_f32")
-        d = (Ws - 2 * W) // 2
-        copy_view(skip[:, :, :, d : d + 2 * W], cat[:, C:])
-        return self._cba(cat, f"{p}.conv1")
 
     def _aspp51(self, x, p):
         B, C, H, W = x.shape
@@ -315,13 +306,7 @@ class VRNet51(VRNet):
         hc = self._cba(x, f"{p}.conv")  # (N, 1, nbins, nframes)
         seq = _new((nf, N, nb, 1), x)
         copy_view(hc.permute(3, 0, 2, 1), seq)  # "N 1 bins frames -> frames N bins"
-        hid = W[f"{p}.whh"].shape[2]
-        xp = _new((2, nf * N, 4 * hid), x)
-        for d in range(2):
-            check(lib.b200sep_gemm_f32_math(_ptr(seq), _ptr(W[f"{p}.wih{d}"]), xp.data_ptr() + d * nf * N * 4 * hid * 4, nf * N, 4 * hid, nb, nb, nb, 4 * hid, 1, 0, 0, 0,
-                                            1.0, _ptr(W[f"{p}.bih{d}"]), None, 0, None, None, None, self.math, _stream()), "gemm_f32(lstm input projection)")
-        hs = _new((nf * N, 2 * hid), x)
-        check(lib.b200sep_lstm_bidir_f32(_ptr(xp), _ptr(W[f"{p}.whh"]), _ptr(hs), nf, N, hid, _stream()), "lstm_bidir_f32")
+        hs = lstm_bidir(seq.view(nf * N, nb), N, W[f"{p}.lstm"], self.math)
         dn = linear(hs, W[f"{p}.dense.w"], W[f"{p}.dense.b"], act=ACT_RELU, math=self.math)  # Linear + BatchNorm1d (folded) + ReLU: (frames*N, bins)
         copy_view(dn.view(nf, N, nb, 1).permute(1, 3, 2, 0), out[:, out_c_off : out_c_off + 1])
 
@@ -332,14 +317,14 @@ class VRNet51(VRNet):
         e4 = self._enc(e3, f"{p}.enc4", 2)
         e5 = self._enc(e4, f"{p}.enc5", 2)
         h = self._aspp51(e5, f"{p}.aspp")
-        h = self._dec51(h, e4, f"{p}.dec4")
-        h = self._dec51(h, e3, f"{p}.dec3")
-        h = self._dec51(h, e2, f"{p}.dec2")
+        h = self._dec(h, e4, f"{p}.dec4.conv1")
+        h = self._dec(h, e3, f"{p}.dec3.conv1")
+        h = self._dec(h, e2, f"{p}.dec2.conv1")
         B, C, H, W = h.shape
         hl = _new((B, C + 1, H, W), h)  # torch.cat([bottleneck, lstm_dec2(bottleneck)], dim=1)
         copy_view(h, hl[:, :C])
         self._lstm(h, f"{p}.lstm_dec2", hl, C)
-        return self._dec51(hl, e1, f"{p}.dec1")
+        return self._dec(hl, e1, f"{p}.dec1.conv1")
 
     def forward(self, x: torch.Tensor) -> torch.Tensor:
         assert x.dim() == 4 and x.shape[1] == 2 and x.dtype == torch.float32 and x.is_cuda

@@ -17,9 +17,9 @@ RTOL = 1e-5  # fp32 accumulation of up to a few thousand products, relative to s
 @pytest.fixture(scope="module")
 def L(lib_built):
     assert torch.cuda.is_available()
-    from audio_separator.separator.b200 import _lib, demucs
+    from audio_separator.separator.b200 import _lib, ops
 
-    return _lib, demucs
+    return _lib, ops
 
 
 def p(t):
@@ -47,7 +47,7 @@ ACTS = {0: lambda t: t, 1: F.relu, 2: F.gelu, 3: lambda t: F.leaky_relu(t, 0.01)
      (2688, 512, 512, 1, 0, "bias"), (333, 270, 64, 4, 0, "none"), (77, 40, 36, 6, 4, "bias")],
 )
 def test_gemm_fp16(L, M, N, K, batch, act, epi, packed):
-    _lib, dm = L
+    _lib, ops = L
     g = torch.Generator().manual_seed(M * 7 + N + K)
     a = torch.randn((batch, M, K), generator=g)
     w = torch.randn((N, K), generator=g) / K**0.5 if batch == 1 or packed else torch.randn((batch, N, K), generator=g) / K**0.5
@@ -58,7 +58,7 @@ def test_gemm_fp16(L, M, N, K, batch, act, epi, packed):
     sB = 0 if w.dim() == 2 else N * K
     ad, wd, cd = a.cuda(), w.cuda(), torch.empty((batch, M, N), device="cuda")
     bd, resd, rsd = (t.cuda() if t is not None else None for t in (bias, res, rs))
-    pk = dm._packed_linear(wd, _lib.MATH_FP16) if packed and sB == 0 else None
+    pk = ops._packed_linear(wd, _lib.MATH_FP16) if packed and sB == 0 else None
     _lib.check(_lib.lib.b200sep_gemm_f32_math(p(ad), p(wd), p(cd), M, N, K, K, K, N, batch, M * K, sB, M * N, alpha, p(bd), None, act, p(resd), p(rsd), p(pk),
                                               _lib.MATH_FP16, 0), "gemm_f32_math")
 
@@ -78,7 +78,7 @@ def test_gemm_fp16(L, M, N, K, batch, act, epi, packed):
 def test_math0_entries_match_old_entries(L):
     """MATH_BF16X3 through the *_math entries gives the same bits as the entries without the suffix (GEMM with and without a packed image, conv,
     attention), and the packed images are equal."""
-    _lib, dm = L
+    _lib, ops = L
     lib = _lib.lib
     g = torch.Generator().manual_seed(5)
     M, N, K = 700, 300, 200
@@ -96,7 +96,7 @@ def test_math0_entries_match_old_entries(L):
         _lib.check(lib.b200sep_gemm_f32_math(p(a), p(w), p(c_new), M, N, K, K, K, N, 1, 0, 0, 0, 1.0, p(b), None, 2, None, None, p(pk), 0, 0))
         assert torch.equal(c_old, c_new)
     x = torch.randn((2, 24, 40, 60), generator=g).cuda()
-    wc = torch.from_numpy(dm.block_conv_weight((torch.randn((48, 24, 3, 3), generator=g) / 15).numpy())).cuda()
+    wc = torch.from_numpy(ops.block_conv_weight((torch.randn((48, 24, 3, 3), generator=g) / 15).numpy())).cuda()
     y_old, y_new = torch.empty((2, 48, 40, 60), device="cuda"), torch.empty((2, 48, 40, 60), device="cuda")
     args = (2, 24, 40, 60, 48, 40, 60, 3, 3, 1, 1, 1, 1, 1, 1, 1, 0, 0, 1, 0, 0, 0, 0)
     _lib.check(lib.b200sep_conv2d_f32(p(x), p(wc), None, None, p(y_old), *args, None, 0))
@@ -115,7 +115,7 @@ def test_math0_entries_match_old_entries(L):
 
 
 def test_packed_image_of_the_other_mode_is_rejected(L):
-    _lib, dm = L
+    _lib, ops = L
     lib = _lib.lib
     g = torch.Generator().manual_seed(6)
     M, N, K = 512, 256, 128
@@ -131,8 +131,8 @@ def test_packed_image_of_the_other_mode_is_rejected(L):
     _lib.check(lib.b200sep_tc_pack_linear_weights(p(w), N, K, K, p(pk3), 0))
     with pytest.raises(_lib.B200SepError, match="other math mode"):
         _lib.check(lib.b200sep_gemm_f32_math(p(a), p(w), p(c), M, N, K, K, K, N, 1, 0, 0, 0, 1.0, None, None, 0, None, None, p(pk3), 1, 0))
-    wc = torch.from_numpy(dm.block_conv_weight(torch.randn((32, 16, 3, 3), generator=g).numpy())).cuda()
-    pkc = dm._packed_conv(wc, 16, 9, 32, 0)
+    wc = torch.from_numpy(ops.block_conv_weight(torch.randn((32, 16, 3, 3), generator=g).numpy())).cuda()
+    pkc = ops._packed_conv(wc, 16, 9, 32, 0)
     x, y = torch.randn((1, 16, 30, 40), generator=g).cuda(), torch.empty((1, 32, 30, 40), device="cuda")
     with pytest.raises(_lib.B200SepError, match="other math mode"):
         _lib.check(lib.b200sep_conv2d_f32_math(p(x), p(wc), None, None, p(y), 1, 16, 30, 40, 32, 30, 40, 3, 3, 1, 1, 1, 1, 1, 1, 0, 0, 0, 1, 0, 0, 0, 0, p(pkc), 1, 0))
@@ -155,7 +155,7 @@ def test_packed_image_of_the_other_mode_is_rejected(L):
     ],
 )
 def test_conv2d_fp16(L, geom, packed):
-    _lib, dm = L
+    _lib, ops = L
     g = torch.Generator().manual_seed(geom["cin"] * 7 + geom["cout"])
     x = torch.randn((2, geom["cin"]) + geom["hw"], generator=g)
     fan = geom["cin"] * geom["k"][0] * geom["k"][1]
@@ -163,9 +163,9 @@ def test_conv2d_fp16(L, geom, packed):
     b = torch.randn(geom["cout"], generator=g)
     act = ACTS[geom["act"]]
     conv = lambda xx, ww: F.conv2d(xx, ww, stride=geom["s"], padding=geom["p"], dilation=geom["d"])  # noqa: E731
-    wb = torch.from_numpy(dm.block_conv_weight(w.numpy())).cuda()
+    wb = torch.from_numpy(ops.block_conv_weight(w.numpy())).cuda()
     if packed:
-        got = dm.conv2d(x.cuda(), wb, b.cuda(), geom["cout"], geom["k"], geom["s"], geom["p"], geom["d"][1], act=geom["act"], dh=geom["d"][0], math=_lib.MATH_FP16)
+        got = ops.conv2d(x.cuda(), wb, b.cuda(), geom["cout"], geom["k"], geom["s"], geom["p"], geom["d"][1], act=geom["act"], dh=geom["d"][0], math=_lib.MATH_FP16)
     else:  # no packed image: the producer warps round the weights themselves
         (kh, kw), (sh, sw), (ph, pw), (dh, dw) = geom["k"], geom["s"], geom["p"], geom["d"]
         H, W = geom["hw"]
@@ -179,22 +179,22 @@ def test_conv2d_fp16(L, geom, packed):
 
 
 def test_conv2d_fp16_slice_and_add(L):
-    _lib, dm = L
+    _lib, ops = L
     g = torch.Generator().manual_seed(11)
     x = torch.randn((3, 20, 30, 50), generator=g)
     w = torch.randn((33, 20, 3, 3), generator=g) / 13
     b = torch.randn(33, generator=g)
     add = torch.randn((3, 33, 30, 50), generator=g)
-    wb = torch.from_numpy(dm.block_conv_weight(w.numpy())).cuda()
+    wb = torch.from_numpy(ops.block_conv_weight(w.numpy())).cuda()
     out = torch.full((3, 50, 30, 50), 7.0).cuda()
-    dm.conv2d(x.cuda(), wb, b.cuda(), 33, (3, 3), p=(1, 1), act=dm.ACT_RELU, add=add.cuda(), add_before_act=True, out=out, out_c_off=10, math=_lib.MATH_FP16)
+    ops.conv2d(x.cuda(), wb, b.cuda(), 33, (3, 3), p=(1, 1), act=ops.ACT_RELU, add=add.cuda(), add_before_act=True, out=out, out_c_off=10, math=_lib.MATH_FP16)
     conv = lambda xx, ww: F.conv2d(xx, ww, padding=1)  # noqa: E731
     mag = conv(x.double().abs(), w.double().abs())
     o = out.cpu()
     assert_fp16_close(o[:, 10:43], F.relu(conv(r16(x), r16(w)) + b.double()[:, None, None] + add.double()), mag,
                       F.relu(conv(x.double(), w.double()) + b.double()[:, None, None] + add.double()))
     assert (o[:, :10] == 7).all() and (o[:, 43:] == 7).all()
-    got = dm.conv2d(x.cuda(), wb, b.cuda(), 33, (3, 3), p=(1, 1), act=dm.ACT_RELU, add=add.cuda(), math=_lib.MATH_FP16)
+    got = ops.conv2d(x.cuda(), wb, b.cuda(), 33, (3, 3), p=(1, 1), act=ops.ACT_RELU, add=add.cuda(), math=_lib.MATH_FP16)
     assert_fp16_close(got, F.relu(conv(r16(x), r16(w)) + b.double()[:, None, None]) + add.double(), mag,
                       F.relu(conv(x.double(), w.double()) + b.double()[:, None, None]) + add.double())
 
@@ -202,7 +202,7 @@ def test_conv2d_fp16_slice_and_add(L):
 @pytest.mark.parametrize("axis", [1, 2])
 def test_conv_transpose_fp16(L, axis):
     """nn.ConvTranspose (HTDemucs decoders) as the 2-tap up_axis convolution on the tensor cores, fp16 operands."""
-    _lib, dm = L
+    _lib, ops = L
     g = torch.Generator().manual_seed(20 + axis)
     cin, cout, stride = 64, 48, 4
     if axis == 1:
@@ -211,8 +211,8 @@ def test_conv_transpose_fp16(L, axis):
         b = torch.randn(cout, generator=g)
         out_len = 40 * stride
         ct = lambda xx, ww: F.conv_transpose2d(xx, ww, stride=(stride, 1))[..., 2 : 2 + out_len, :]  # noqa: E731
-        got = dm.conv_transpose(x.cuda(), torch.from_numpy(dm.block_convtr_weight(w.numpy().reshape(cin, cout, 8), stride)).cuda(), b.cuda(), cout, 1, stride, 2,
-                                out_len, dm.ACT_GELU, math=_lib.MATH_FP16)
+        got = ops.conv_transpose(x.cuda(), torch.from_numpy(ops.block_convtr_weight(w.numpy().reshape(cin, cout, 8), stride)).cuda(), b.cuda(), cout, 1, stride, 2,
+                                out_len, ops.ACT_GELU, math=_lib.MATH_FP16)
         act = F.gelu
         bias = b.double()[:, None, None]
     else:
@@ -221,7 +221,7 @@ def test_conv_transpose_fp16(L, axis):
         b = torch.randn(cout, generator=g)
         out_len = 1190
         ct = lambda xx, ww: F.conv_transpose1d(xx[:, :, 0], ww, stride=stride)[..., 2 : 2 + out_len][:, :, None]  # noqa: E731
-        got = dm.conv_transpose(x.cuda(), torch.from_numpy(dm.block_convtr_weight(w.numpy(), stride)).cuda(), b.cuda(), cout, 2, stride, 2, out_len,
+        got = ops.conv_transpose(x.cuda(), torch.from_numpy(ops.block_convtr_weight(w.numpy(), stride)).cuda(), b.cuda(), cout, 2, stride, 2, out_len,
                                 math=_lib.MATH_FP16)
         act = lambda t: t  # noqa: E731
         bias = b.double()[:, None, None]
@@ -268,7 +268,7 @@ def test_shape_rule_matches_the_library(L):
     fp16 mode must change the result exactly when the restated rule says tensor core (the SIMT kernels are fp32 in both modes, bit for bit)."""
     from fp16_operands import tc_conv_usable, tc_gemm_usable
 
-    _lib, dm = L
+    _lib, ops = L
     lib = _lib.lib
     g = torch.Generator().manual_seed(9)
     gemms = [(512, 32, 32), (512, 31, 32), (512, 32, 31), (512, 32, 64), (511, 32, 64), (128, 128, 40), (127, 129, 40)]
@@ -283,7 +283,7 @@ def test_shape_rule_matches_the_library(L):
     convs = [(32, 16, 1, 1, 16, 32), (31, 16, 1, 1, 16, 32), (32, 15, 1, 1, 16, 32), (32, 16, 1, 1, 511, 1), (4, 16, 3, 3, 8, 64), (3, 16, 3, 3, 8, 64)]
     for cin, cout, kh, kw, H, W in convs:
         x = torch.randn((1, cin, H, W), generator=g).cuda()
-        wb = torch.from_numpy(dm.block_conv_weight(torch.randn((cout, cin, kh, kw), generator=g).numpy())).cuda()
+        wb = torch.from_numpy(ops.block_conv_weight(torch.randn((cout, cin, kh, kw), generator=g).numpy())).cuda()
         out = {}
         for m in (0, 1):
             out[m] = torch.empty((1, cout, H, W), device="cuda")

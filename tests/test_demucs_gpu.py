@@ -31,6 +31,14 @@ def dm(lib_built):
 
 
 @pytest.fixture(scope="module")
+def ops(lib_built):
+    assert torch.cuda.is_available()
+    from audio_separator.separator.b200 import ops
+
+    return ops
+
+
+@pytest.fixture(scope="module")
 def small(dm, golden_dir):
     z = np.load(os.path.join(golden_dir, "demucs_small.npz"))
     ocfg = D.HTConfig(**SMALL)
@@ -53,19 +61,19 @@ def small(dm, golden_dir):
         dict(cin=2, cout=10, k=(1, 8), s=(1, 4), p=(0, 2), dw=1, hw=(1, 1026)),
     ],
 )
-def test_conv2d_f32(dm, geom):
+def test_conv2d_f32(ops, geom):
     g = torch.Generator().manual_seed(1)
     x = torch.randn((2, geom["cin"]) + geom["hw"], generator=g)
     w = torch.randn((geom["cout"], geom["cin"]) + geom["k"], generator=g) * 0.2
     b = torch.randn(geom["cout"], generator=g)
     ref = F.gelu(F.conv2d(x.double(), w.double(), b.double(), stride=geom["s"], padding=geom["p"], dilation=(1, geom["dw"])))
-    wb = dev(dm.block_conv_weight(w.numpy()))
-    got = dm.conv2d(x.cuda(), wb, b.cuda(), geom["cout"], geom["k"], geom["s"], geom["p"], geom["dw"], act=dm.ACT_GELU).cpu()
+    wb = dev(ops.block_conv_weight(w.numpy()))
+    got = ops.conv2d(x.cuda(), wb, b.cuda(), geom["cout"], geom["k"], geom["s"], geom["p"], geom["dw"], act=ops.ACT_GELU).cpu()
     assert got.shape == ref.shape
     assert (got.double() - ref).abs().max() <= 2e-5 * max(1.0, ref.abs().max())
 
 
-def test_conv2d_f32_ragged_time_pad_and_add(dm):
+def test_conv2d_f32_ragged_time_pad_and_add(ops):
     """The time encoder pads its input to a multiple of the stride (hdemucs.py:126-129): implicit zero columns."""
     g = torch.Generator().manual_seed(2)
     x = torch.randn((1, 3, 1, 1023), generator=g)
@@ -73,12 +81,12 @@ def test_conv2d_f32_ragged_time_pad_and_add(dm):
     b = torch.randn(6, generator=g)
     ref = F.conv2d(F.pad(x, (0, 1)), w, b, stride=(1, 4), padding=(0, 2))
     add = torch.randn(ref.shape, generator=g)
-    got = dm.conv2d(x.cuda(), dev(dm.block_conv_weight(w.numpy())), b.cuda(), 6, (1, 8), (1, 4), (0, 2), out_hw=(1, 256), add=add.cuda(), add_before_act=True, act=dm.ACT_RELU).cpu()
+    got = ops.conv2d(x.cuda(), dev(ops.block_conv_weight(w.numpy())), b.cuda(), 6, (1, 8), (1, 4), (0, 2), out_hw=(1, 256), add=add.cuda(), add_before_act=True, act=ops.ACT_RELU).cpu()
     assert (got - F.relu(ref + add)).abs().max() <= 2e-5
 
 
 @pytest.mark.parametrize("axis", [1, 2])
-def test_conv_transpose_f32(dm, axis):
+def test_conv_transpose_f32(ops, axis):
     g = torch.Generator().manual_seed(3)
     cin, cout = 12, 5
     if axis == 1:
@@ -86,20 +94,20 @@ def test_conv_transpose_f32(dm, axis):
         w = torch.randn((cin, cout, 8, 1), generator=g) * 0.2
         b = torch.randn(cout, generator=g)
         ref = F.gelu(F.conv_transpose2d(x.double(), w.double(), b.double(), stride=(4, 1))[..., 2:-2, :])
-        got = dm.conv_transpose(x.cuda(), dev(dm.block_convtr_weight(w.numpy().reshape(cin, cout, 8), 4)), b.cuda(), cout, 1, 4, 2, 36, dm.ACT_GELU).cpu()
+        got = ops.conv_transpose(x.cuda(), dev(ops.block_convtr_weight(w.numpy().reshape(cin, cout, 8), 4)), b.cuda(), cout, 1, 4, 2, 36, ops.ACT_GELU).cpu()
     else:
         x = torch.randn((2, cin, 1, 301), generator=g)
         w = torch.randn((cin, cout, 8), generator=g) * 0.2
         b = torch.randn(cout, generator=g)
         length = 1201  # the skip length of the time decoder: odd, shorter than 4 * 301
         ref = F.conv_transpose1d(x[:, :, 0].double(), w.double(), b.double(), stride=4)[..., 2 : 2 + length][:, :, None]
-        got = dm.conv_transpose(x.cuda(), dev(dm.block_convtr_weight(w.numpy(), 4)), b.cuda(), cout, 2, 4, 2, length).cpu()
+        got = ops.conv_transpose(x.cuda(), dev(ops.block_convtr_weight(w.numpy(), 4)), b.cuda(), cout, 2, 4, 2, length).cpu()
     assert got.shape == ref.shape
     assert (got.double() - ref).abs().max() <= 2e-5 * max(1.0, ref.abs().max())
 
 
 @pytest.mark.parametrize("axis", [1, 2])
-def test_conv_transpose_f32_tensor_core_route(dm, axis):
+def test_conv_transpose_f32_tensor_core_route(ops, axis):
     """Same operator at shapes the wgmma kernel takes (real output channels a multiple of 16, >= 512 coarse pixels): the scatter epilogue of tc_f32.cu."""
     g = torch.Generator().manual_seed(5)
     cin, cout = 96, 48
@@ -108,37 +116,37 @@ def test_conv_transpose_f32_tensor_core_route(dm, axis):
         w = torch.randn((cin, cout, 8, 1), generator=g) / cin**0.5
         b = torch.randn(cout, generator=g)
         ref = F.gelu(F.conv_transpose2d(x.double(), w.double(), b.double(), stride=(4, 1))[..., 2:-2, :])
-        got = dm.conv_transpose(x.cuda(), dev(dm.block_convtr_weight(w.numpy().reshape(cin, cout, 8), 4)), b.cuda(), cout, 1, 4, 2, 32, dm.ACT_GELU).cpu()
+        got = ops.conv_transpose(x.cuda(), dev(ops.block_convtr_weight(w.numpy().reshape(cin, cout, 8), 4)), b.cuda(), cout, 1, 4, 2, 32, ops.ACT_GELU).cpu()
     else:
         x = torch.randn((2, cin, 1, 700), generator=g)
         w = torch.randn((cin, cout, 8), generator=g) / cin**0.5
         b = torch.randn(cout, generator=g)
         length = 2797
         ref = F.conv_transpose1d(x[:, :, 0].double(), w.double(), b.double(), stride=4)[..., 2 : 2 + length][:, :, None]
-        got = dm.conv_transpose(x.cuda(), dev(dm.block_convtr_weight(w.numpy(), 4)), b.cuda(), cout, 2, 4, 2, length).cpu()
+        got = ops.conv_transpose(x.cuda(), dev(ops.block_convtr_weight(w.numpy(), 4)), b.cuda(), cout, 2, 4, 2, length).cpu()
     assert got.shape == ref.shape and torch.isfinite(got).all()
     assert (got.double() - ref).abs().max() <= 5e-5 * max(1.0, ref.abs().max())
 
 
-def test_groupnorm_glu_layernorm_softmax_permute(dm):
+def test_groupnorm_glu_layernorm_softmax_permute(ops):
     g = torch.Generator().manual_seed(4)
     x = torch.randn((2, 6, 5, 77), generator=g) * 3 + 1
     ga, be = torch.rand(6, generator=g) + 0.5, torch.randn(6, generator=g)
     # DConv applied per frequency row: samples are (b, fr), statistics over (C, T)
     ref = F.gelu(F.group_norm(x.permute(0, 2, 1, 3).reshape(10, 6, 77), 1, ga, be)).view(2, 5, 6, 77).permute(0, 2, 1, 3)
-    got = dm.groupnorm1(x.cuda().clone(), ga.cuda(), be.cuda(), dm.ACT_GELU).cpu()
+    got = ops.groupnorm1(x.cuda().clone(), ga.cuda(), be.cuda(), ops.ACT_GELU).cpu()
     assert (got - ref).abs().max() <= 1e-5
     tok = torch.randn((3, 50, 6), generator=g) * 2 - 1
     ref = F.group_norm(tok.transpose(1, 2), 1, ga, be).transpose(1, 2)
-    got = dm.groupnorm1(tok.cuda().clone(), ga.cuda(), be.cuda(), channel_last=True).cpu()
+    got = ops.groupnorm1(tok.cuda().clone(), ga.cuda(), be.cuda(), channel_last=True).cpu()
     assert (got - ref).abs().max() <= 1e-5
     a = torch.randn((2, 12, 5, 33), generator=g)
     res, sc = torch.randn((2, 6, 5, 33), generator=g), torch.rand(6, generator=g)
-    assert (dm.glu(a.cuda()).cpu() - F.glu(a, 1)).abs().max() <= 1e-6
-    assert (dm.glu(a.cuda(), res.cuda(), sc.cuda()).cpu() - (res + sc[None, :, None, None] * F.glu(a, 1))).abs().max() <= 1e-6
+    assert (ops.glu(a.cuda()).cpu() - F.glu(a, 1)).abs().max() <= 1e-6
+    assert (ops.glu(a.cuda(), res.cuda(), sc.cuda()).cpu() - (res + sc[None, :, None, None] * F.glu(a, 1))).abs().max() <= 1e-6
     t = torch.randn((7, 9, 40), generator=g) * 4
     g2, b2 = torch.rand(40, generator=g), torch.randn(40, generator=g)
-    assert (dm.layernorm(t.cuda(), g2.cuda(), b2.cuda()).cpu() - F.layer_norm(t, (40,), g2, b2)).abs().max() <= 1e-5
+    assert (ops.layernorm(t.cuda(), g2.cuda(), b2.cuda()).cpu() - F.layer_norm(t, (40,), g2, b2)).abs().max() <= 1e-5
     from audio_separator.separator.b200._lib import check, lib
 
     s = (torch.randn((33, 300), generator=g) * 5).cuda()
@@ -153,18 +161,18 @@ def test_groupnorm_glu_layernorm_softmax_permute(dm):
     assert torch.equal(out.cpu(), p.cpu().permute(0, 3, 2, 1).contiguous())
 
 
-def test_gemm_f32_and_attention_pattern(dm):
+def test_gemm_f32_and_attention_pattern(ops):
     g = torch.Generator().manual_seed(5)
     x = torch.randn((130, 72), generator=g)
     w = torch.randn((200, 72), generator=g) * 0.1
     b = torch.randn(200, generator=g)
     res, rs = torch.randn((130, 200), generator=g), torch.rand(200, generator=g)
     ref = res + rs * F.gelu(F.linear(x.double(), w.double(), b.double()))
-    got = dm.linear(x.cuda(), w.cuda(), b.cuda(), act=dm.ACT_GELU, res=res.cuda(), res_scale=rs.cuda()).cpu()
+    got = ops.linear(x.cuda(), w.cuda(), b.cuda(), act=ops.ACT_GELU, res=res.cuda(), res_scale=rs.cuda()).cpu()
     assert (got.double() - ref).abs().max() <= 2e-5
     # odd K / unaligned leading dimensions take the scalar load path
     x2, w2 = torch.randn((17, 45), generator=g), torch.randn((9, 45), generator=g)
-    assert (dm.linear(x2.cuda(), w2.cuda(), None).cpu() - x2 @ w2.t()).abs().max() <= 2e-5
+    assert (ops.linear(x2.cuda(), w2.cuda(), None).cpu() - x2 @ w2.t()).abs().max() <= 2e-5
 
 
 @pytest.mark.timeout(180)
@@ -201,7 +209,7 @@ def test_fused_dconv_layer_vs_torch(dm, B, C, Fr, L, hid, dil, u_in):
     assert torch.equal(d[0], y)
 
 
-def test_meanstd_and_stats_ops(dm):
+def test_meanstd_and_stats_ops(ops):
     from audio_separator.separator.b200._lib import check, lib
 
     g = torch.Generator().manual_seed(6)
@@ -210,9 +218,9 @@ def test_meanstd_and_stats_ops(dm):
     check(lib.b200sep_meanstd_f32(x.data_ptr(), x.numel(), st.data_ptr(), 0))
     m, s = st.cpu().tolist()
     assert abs(m - x.double().mean().item()) <= 1e-6 and abs(s - x.double().std().item()) <= 1e-5
-    y = dm.ew(x, st, torch.empty_like(x), op=2)
+    y = ops.ew(x, st, torch.empty_like(x), op=2)
     assert (y.cpu() - (x.cpu() - m) / (1e-5 + s)).abs().max() <= 1e-6
-    z = dm.ew(y, st, torch.empty_like(x), op=3)
+    z = ops.ew(y, st, torch.empty_like(x), op=3)
     assert (z.cpu() - x.cpu()).abs().max() <= 1e-4
 
 

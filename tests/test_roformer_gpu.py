@@ -113,7 +113,7 @@ def test_roformer_operator_kernels(rf):
         got = sdv2.cpu()
         assert (got[:, :n] - torch.softmax(sc[:, :n], -1)).abs().max() <= 1e-6 and torch.equal(got[:, n:], sc[:, n:])
     # tiny-N GEMM (the attention gates): warp-per-row kernel
-    from audio_separator.separator.b200.demucs import linear
+    from audio_separator.separator.b200.ops import linear
 
     xg, wg, bg = torch.randn((2500, 96), generator=g), torch.randn((8, 96), generator=g) * 0.1, torch.randn(8, generator=g)
     assert (linear(xg.cuda(), wg.cuda(), bg.cuda()).cpu() - F.linear(xg, wg, bg)).abs().max() <= 2e-5

@@ -11,11 +11,11 @@ pytestmark = pytest.mark.gpu
 
 
 @pytest.fixture(scope="module")
-def dm(lib_built):
+def ops(lib_built):
     assert torch.cuda.is_available()
-    from audio_separator.separator.b200 import demucs
+    from audio_separator.separator.b200 import ops
 
-    return demucs
+    return ops
 
 
 def rel_err(got, ref):
@@ -23,37 +23,35 @@ def rel_err(got, ref):
 
 
 @pytest.mark.parametrize("M,N,K", [(300, 200, 100), (128, 128, 64), (1000, 513, 72), (129, 260, 2048), (2688, 512, 512), (77, 40, 36)])
-def test_tc_linear(dm, M, N, K):
+def test_tc_linear(ops, M, N, K):
     g = torch.Generator().manual_seed(M + N + K)
     x, w, b = torch.randn((M, K), generator=g), torch.randn((N, K), generator=g) / K**0.5, torch.randn(N, generator=g)
     res, rs = torch.randn((M, N), generator=g), torch.rand(N, generator=g)
     ref = res.double() + rs.double() * F.gelu(F.linear(x.double(), w.double(), b.double()))
-    got = dm.linear(x.cuda(), w.cuda(), b.cuda(), act=dm.ACT_GELU, res=res.cuda(), res_scale=rs.cuda()).cpu()
+    got = ops.linear(x.cuda(), w.cuda(), b.cuda(), act=ops.ACT_GELU, res=res.cuda(), res_scale=rs.cuda()).cpu()
     assert rel_err(got, ref) <= 3e-5
-    got2 = dm.linear(x.cuda(), w.cuda(), None).cpu()
+    got2 = ops.linear(x.cuda(), w.cuda(), None).cpu()
     assert rel_err(got2, x.double() @ w.double().t()) <= 3e-5
 
 
-def test_tc_attention_pattern(dm):
+def test_tc_attention_pattern(ops):
     """scores = Q K^T / sqrt(hd) per head via strides into (L, D) tensors; V^T = Wv X^T with a per-row bias; O = P V into head columns."""
-    from audio_separator.separator.b200.demucs import _gemm_raw
-
     g = torch.Generator().manual_seed(3)
     Lq, Lk, H, hd = 333, 270, 4, 64
     D = H * hd
     q, k = torch.randn((Lq, D), generator=g).cuda(), torch.randn((Lk, D), generator=g).cuda()
     sc = torch.empty((H, Lq, Lk), device="cuda")
-    _gemm_raw(q.data_ptr(), k.data_ptr(), sc.data_ptr(), Lq, Lk, hd, D, D, Lk, H, hd, hd, Lq * Lk, alpha=0.125)
+    ops.gemm(q.data_ptr(), k.data_ptr(), sc.data_ptr(), Lq, Lk, hd, D, D, Lk, H, hd, hd, Lq * Lk, alpha=0.125)
     ref = torch.einsum("qhd,khd->hqk", q.cpu().double().view(Lq, H, hd), k.cpu().double().view(Lk, H, hd)) * 0.125
     assert rel_err(sc.cpu(), ref) <= 3e-5
     wv, bv, x = torch.randn((D, D), generator=g).cuda() / 16, torch.randn(D, generator=g).cuda(), torch.randn((2, Lk, D), generator=g).cuda()
     vt = torch.empty((2, D, Lk), device="cuda")
-    _gemm_raw(wv.data_ptr(), x.data_ptr(), vt.data_ptr(), D, Lk, D, D, D, Lk, 2, 0, Lk * D, D * Lk, bias_m=bv.data_ptr())
+    ops.gemm(wv.data_ptr(), x.data_ptr(), vt.data_ptr(), D, Lk, D, D, D, Lk, 2, 0, Lk * D, D * Lk, bias_m=bv.data_ptr())
     refv = (x.cpu().double() @ wv.cpu().double().t() + bv.cpu().double()).transpose(1, 2)
     assert rel_err(vt.cpu(), refv) <= 3e-5
     p = torch.softmax(sc, -1).contiguous()
     o = torch.zeros((Lq, D), device="cuda")
-    _gemm_raw(p.data_ptr(), vt.data_ptr(), o.data_ptr(), Lq, hd, Lk, Lk, Lk, D, H, Lq * Lk, hd * Lk, hd)
+    ops.gemm(p.data_ptr(), vt.data_ptr(), o.data_ptr(), Lq, hd, Lk, Lk, Lk, D, H, Lq * Lk, hd * Lk, hd)
     refo = torch.einsum("hqk,hdk->qhd", p.cpu().double(), vt[0].cpu().double().view(H, hd, Lk)).reshape(Lq, D)
     assert rel_err(o.cpu(), refo) <= 3e-5
 
@@ -70,7 +68,7 @@ def test_tc_attention_pattern(dm):
         dict(cin=130, cout=64, k=(1, 1), s=(1, 1), p=(0, 0), dw=1, hw=(64, 64), act=4),
     ],
 )
-def test_tc_conv2d(dm, geom):
+def test_tc_conv2d(ops, geom):
     g = torch.Generator().manual_seed(geom["cin"] * 7 + geom["cout"])
     x = torch.randn((2, geom["cin"]) + geom["hw"], generator=g)
     fan = geom["cin"] * geom["k"][0] * geom["k"][1]
@@ -78,13 +76,13 @@ def test_tc_conv2d(dm, geom):
     b = torch.randn(geom["cout"], generator=g)
     act = {0: lambda t: t, 1: F.relu, 2: F.gelu, 3: lambda t: F.leaky_relu(t, 0.01), 4: torch.sigmoid}[geom["act"]]
     ref = act(F.conv2d(x.double(), w.double(), b.double(), stride=geom["s"], padding=geom["p"], dilation=(1, geom["dw"])))
-    wb = torch.from_numpy(dm.block_conv_weight(w.numpy())).cuda()
-    got = dm.conv2d(x.cuda(), wb, b.cuda(), geom["cout"], geom["k"], geom["s"], geom["p"], geom["dw"], act=geom["act"]).cpu()
+    wb = torch.from_numpy(ops.block_conv_weight(w.numpy())).cuda()
+    got = ops.conv2d(x.cuda(), wb, b.cuda(), geom["cout"], geom["k"], geom["s"], geom["p"], geom["dw"], act=geom["act"]).cpu()
     assert got.shape == ref.shape
     assert rel_err(got, ref) <= 3e-5, rel_err(got, ref)
 
 
-def test_tc_conv2d_slice_and_add(dm):
+def test_tc_conv2d_slice_and_add(ops):
     g = torch.Generator().manual_seed(11)
     x = torch.randn((3, 20, 30, 50), generator=g)
     w = torch.randn((33, 20, 3, 3), generator=g) / 13
@@ -92,12 +90,12 @@ def test_tc_conv2d_slice_and_add(dm):
     ref = F.conv2d(x.double(), w.double(), b.double(), padding=1)
     add = torch.randn(ref.shape, generator=g)
     out = torch.full((3, 50, 30, 50), 7.0).cuda()
-    wb = torch.from_numpy(dm.block_conv_weight(w.numpy())).cuda()
-    dm.conv2d(x.cuda(), wb, b.cuda(), 33, (3, 3), p=(1, 1), act=dm.ACT_RELU, add=add.cuda(), add_before_act=True, out=out, out_c_off=10)
+    wb = torch.from_numpy(ops.block_conv_weight(w.numpy())).cuda()
+    ops.conv2d(x.cuda(), wb, b.cuda(), 33, (3, 3), p=(1, 1), act=ops.ACT_RELU, add=add.cuda(), add_before_act=True, out=out, out_c_off=10)
     o = out.cpu()
     assert rel_err(o[:, 10:43], F.relu(ref + add.double())) <= 3e-5
     assert (o[:, :10] == 7).all() and (o[:, 43:] == 7).all()
-    got = dm.conv2d(x.cuda(), wb, b.cuda(), 33, (3, 3), p=(1, 1), act=dm.ACT_RELU, add=add.cuda(), add_before_act=False).cpu()
+    got = ops.conv2d(x.cuda(), wb, b.cuda(), 33, (3, 3), p=(1, 1), act=ops.ACT_RELU, add=add.cuda(), add_before_act=False).cpu()
     assert rel_err(got, F.relu(ref) + add.double()) <= 3e-5
 
 

@@ -43,7 +43,7 @@ def gold(golden_dir):
 
 def test_vr_operator_kernels(vr):
     from audio_separator.separator.b200._lib import check, lib
-    from audio_separator.separator.b200.demucs import block_conv_weight, conv2d
+    from audio_separator.separator.b200.ops import block_conv_weight, conv2d
 
     g = torch.Generator().manual_seed(1)
     x = torch.randn((2, 6, 21, 40), generator=g)
@@ -233,7 +233,7 @@ def test_vr_separator_plugin_end_to_end(vr, tmp_path):
 # ------------------------------------------------------------------------------------------------ VR 5.1 (CascadedNet + LSTM)
 def test_lstm_and_dilated_conv_kernels(vr):
     from audio_separator.separator.b200._lib import check, lib
-    from audio_separator.separator.b200.demucs import block_conv_weight, conv2d
+    from audio_separator.separator.b200.ops import block_conv_weight, conv2d
 
     g = torch.Generator().manual_seed(21)
     T, N, nin, hid = 37, 3, 20, 12
