@@ -15,7 +15,6 @@ import random
 from fractions import Fraction
 
 import numpy as np
-import torch
 
 from ..b200.demucs import DemucsEngine, HTDemucsNet
 from ..b200.demucs_loader import load_demucs
@@ -35,17 +34,7 @@ class DemucsSeparator(CommonSeparator):
         self.overlap = arch_config.get("overlap", 0.25)
         self.segments_enabled = arch_config.get("segments_enabled", True)
         self.batch_size = int(arch_config.get("batch_size", 4))  # segments per forward (H100 addition; results do not depend on it)
-        self.sharded = bool(arch_config.get("b200_sharded", False))  # one process per GPU (torch.distributed, nccl): time-shard every track over the ranks
-        if not torch.cuda.is_available():
-            raise RuntimeError("DemucsSeparator (H100 build) needs a CUDA device: there is no CPU path in this package")
-        self.dist = None
-        if self.sharded:
-            import torch.distributed as dist
-
-            if not dist.is_initialized():
-                raise RuntimeError("demucs_params['b200_sharded'] needs torch.distributed to be initialised (backend nccl, one process per GPU)")
-            self.dist = dist
-        self.torch_device = torch.device("cuda", torch.cuda.current_device())
+        self.setup_device(arch_config, "DemucsSeparator", "demucs_params")
         self.demucs_source_map = DEMUCS_4_SOURCE_MAPPER
         self.load_model()
 
@@ -87,11 +76,4 @@ class DemucsSeparator(CommonSeparator):
         if source is None:  # sharded, rank != 0: rank 0 holds the stems and writes the files
             return []
         self.demucs_source_map = {2: DEMUCS_2_SOURCE_MAPPER, 6: DEMUCS_6_SOURCE_MAPPER}.get(len(source), DEMUCS_4_SOURCE_MAPPER)  # :134-146
-        output_files = []
-        for stem_name, stem_value in self.demucs_source_map.items():
-            if self.output_single_stem is not None and stem_name.lower() != self.output_single_stem.lower():
-                continue
-            stem_path = self.get_stem_output_path(stem_name, custom_output_names)
-            self.final_process(stem_path, source[stem_value].T, stem_name)
-            output_files.append(stem_path)
-        return output_files
+        return self.write_stems([(name, source[i].T) for name, i in self.demucs_source_map.items()], custom_output_names)

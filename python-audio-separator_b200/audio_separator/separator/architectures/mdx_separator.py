@@ -14,7 +14,7 @@ import torch
 
 from ..b200 import mdx_weights, onnx_reader
 from ..b200.engine import MdxEngine, MdxNet
-from ..common_separator import CommonSeparator, DeviceStem
+from ..common_separator import CommonSeparator, DeviceStem, load_checkpoint
 from ..uvr_lib_v5.stft import STFT
 
 
@@ -27,7 +27,6 @@ class MDXSeparator(CommonSeparator):
         self.hop_length = arch_config.get("hop_length")
         self.enable_denoise = arch_config.get("enable_denoise")
         self.precision = int(arch_config.get("b200_precision", 1))  # 0 = fp32 SIMT, 1 = bf16x3 split tensor-core path
-        self.sharded = bool(arch_config.get("b200_sharded", False))  # one process per GPU (torch.distributed, nccl): time-shard every track over the ranks
 
         self.compensate = self.model_data["compensate"]
         self.dim_f = self.model_data["mdx_dim_f_set"]
@@ -35,16 +34,7 @@ class MDXSeparator(CommonSeparator):
         self.n_fft = self.model_data["mdx_n_fft_scale_set"]
         self.config_yaml = self.model_data.get("config_yaml", None)
 
-        if not torch.cuda.is_available():
-            raise RuntimeError("MDXSeparator (H100 build) needs a CUDA device: there is no onnxruntime / CPU path in this package")
-        self.dist = None
-        if self.sharded:
-            import torch.distributed as dist
-
-            if not dist.is_initialized():
-                raise RuntimeError("mdx_params['b200_sharded'] needs torch.distributed to be initialised (backend nccl, one process per GPU)")
-            self.dist = dist
-        self.torch_device = torch.device("cuda", torch.cuda.current_device())
+        self.setup_device(arch_config, "MDXSeparator", "mdx_params", missing="onnxruntime / CPU path")
         self.n_bins = self.trim = self.chunk_size = self.gen_size = 0
         self._host_bufs = {}
         self.stft = None
@@ -61,8 +51,7 @@ class MDXSeparator(CommonSeparator):
         if path.lower().endswith(".onnx"):
             state = onnx_reader.load_convtdfnet_state(path)
         elif path.lower().endswith(".npz"):
-            with np.load(path) as z:
-                state = {k: z[k] for k in z.files}
+            state = load_checkpoint(path)
         else:
             raise ValueError(f"unsupported MDX model file {path!r} (expected .onnx or .npz)")
         hp = mdx_weights.infer_hparams_from_state(state)
@@ -146,19 +135,7 @@ class MDXSeparator(CommonSeparator):
             self.primary_source = DeviceStem(primary_dev)
         if not isinstance(self.secondary_source, np.ndarray):
             self.secondary_source = DeviceStem(secondary_dev)
-
-        output_files = []
-        for is_secondary in (True, False):  # secondary stem file first, then primary (:185-197)
-            name = self.secondary_stem_name if is_secondary else self.primary_stem_name
-            if self.output_single_stem and self.output_single_stem.lower() != name.lower():
-                continue
-            path = self.get_stem_output_path(name, custom_output_names)
-            self.logger.info(f"Saving {name} stem to {path}...")
-            src = self.secondary_source if is_secondary else self.primary_source
-            self.final_process(path, src.tensor if isinstance(src, DeviceStem) else src, name)
-            if is_secondary:
-                self.secondary_stem_output_path = path
-            else:
-                self.primary_stem_output_path = path
-            output_files.append(path)
-        return output_files
+        unwrap = lambda src: src.tensor if isinstance(src, DeviceStem) else src  # noqa: E731
+        # secondary stem file first, then primary (:185-197)
+        return self.write_stems([(self.secondary_stem_name, unwrap(self.secondary_source)), (self.primary_stem_name, unwrap(self.primary_source))],
+                                custom_output_names)

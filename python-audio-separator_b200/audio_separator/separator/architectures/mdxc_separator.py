@@ -23,7 +23,7 @@ import torch
 from ..b200.engine import MdxcEngine, TfcNet
 from ..b200.resample import match_length, resample
 from ..b200.roformer import BSRoformerConfig, BSRoformerNet, MelBandRoformerConfig, RoformerEngine
-from ..common_separator import CommonSeparator, normalize, tensor_core_math
+from ..common_separator import CommonSeparator, load_checkpoint, normalize, tensor_core_math
 
 PITCH_RES_TYPE = "sinc_fastest"  # spec_utils.wav_resolution_float_resampling on Linux
 
@@ -39,23 +39,13 @@ class MDXCSeparator(CommonSeparator):
         self.pitch_shift = arch_config.get("pitch_shift", 0)
         self.process_all_stems = arch_config.get("process_all_stems", True)
         self.is_roformer = bool(self.is_roformer_model)
-        self.sharded = bool(arch_config.get("b200_sharded", False))  # one process per GPU (torch.distributed, nccl): time-shard every track over the ranks
-        if not torch.cuda.is_available():
-            raise RuntimeError("MDXCSeparator (H100 build) needs a CUDA device: there is no CPU path in this package")
-        self.dist = None
-        if self.sharded:
-            import torch.distributed as dist
-
-            if not dist.is_initialized():
-                raise RuntimeError("mdxc_params['b200_sharded'] needs torch.distributed to be initialised (backend nccl, one process per GPU)")
-            self.dist = dist
-        self.torch_device = torch.device("cuda", torch.cuda.current_device())
+        self.setup_device(arch_config, "MDXCSeparator", "mdxc_params")
         self.is_primary_stem_main_target = bool(self.model_data_cfgdict["training"].get("target_instrument"))  # :69, both model families
         self._engines = {}  # dim_t -> engine: the chunk length is fixed per engine, and separate() switches it for clips shorter than 10 s (:137-143)
         self.load_model()
 
     def load_model(self):
-        """Replaces TFC_TDF_net(config).load_state_dict(torch.load(ckpt)) (mdxc_separator.py:76-116)."""
+        """Replaces TFC_TDF_net(config).load_state_dict(checkpoint) (mdxc_separator.py:76-116)."""
         cfg = self.model_data_cfgdict
         audio, model, training = cfg["audio"], cfg["model"], cfg["training"]
         if self.is_roformer:
@@ -64,14 +54,7 @@ class MDXCSeparator(CommonSeparator):
             self.logger.debug("use_autocast: MDX23C (TFC_TDF_net) keeps full precision; its pair-format kernels have no fp16 mode")
         if model.get("norm") != "InstanceNorm" or model.get("act", "gelu") != "gelu" or list(model.get("scale", [2, 2])) != [2, 2]:
             raise ValueError("the H100 TFC_TDF_net supports norm=InstanceNorm, act=gelu, scale=[2,2] (the MDX23C configuration)")
-        path = self.model_path
-        if path.lower().endswith(".npz"):
-            with np.load(path) as z:
-                state = {k: z[k] for k in z.files}
-        else:
-            sd = torch.load(path, map_location="cpu", weights_only=True)
-            state = {k: v.float().numpy() for k, v in (sd.get("state_dict", sd)).items()}
-        self._state = state
+        self._state = load_checkpoint(self.model_path)
         self._select_engine()
 
     def _select_engine(self):
@@ -101,14 +84,7 @@ class MDXCSeparator(CommonSeparator):
             rcfg = BSRoformerConfig.from_model_section(model)
         else:
             raise ValueError("Unknown Roformer model type in configuration (neither num_bands nor freqs_per_bands)")
-        path = self.model_path
-        if path.lower().endswith(".npz"):
-            with np.load(path) as z:
-                state = {k: z[k] for k in z.files}
-        else:
-            sd = torch.load(path, map_location="cpu", weights_only=True)
-            state = {k: v.float().numpy() for k, v in (sd.get("state_dict", sd)).items()}
-        self.net = BSRoformerNet(rcfg, state, device=self.torch_device, math=tensor_core_math("Roformer", self.use_autocast))
+        self.net = BSRoformerNet(rcfg, load_checkpoint(self.model_path), device=self.torch_device, math=tensor_core_math("Roformer", self.use_autocast))
         self._select_engine()
 
     def _demix_stems(self, orig):
@@ -128,32 +104,15 @@ class MDXCSeparator(CommonSeparator):
             full = torch.stack([match_length(resample(stem, sr_pitched, sr_back, PITCH_RES_TYPE), orig.shape[1]) for stem in full])
         return full.cpu().numpy()
 
-    def _demix_roformer(self, mix):
-        """Roformer branch of demix + the stem dictionary (mdxc_separator.py:272-343, :406-468)."""
-        training = self.model_data_cfgdict["training"]
-        orig = np.ascontiguousarray(mix, dtype=np.float32)
-        out = self._demix_stems(orig)
-        if out is None:
-            return None
-        if self.net.cfg.num_stems > 1:
-            return {k: v for k, v in zip(training["instruments"], out)}
-        primary = out[0]
-        if self.is_primary_stem_main_target:  # single-target models also return the residual as the secondary stem
-            return {self.primary_stem_name: primary, self.secondary_stem_name: orig - primary}
-        return primary
-
     def demix(self, mix):
-        """(2, N) ndarray -> {instrument: (2, N) ndarray} (mdxc_separator.py:406-434) or the single target's array; None on the ranks other
-        than 0 of a sharded run."""
-        if self.is_roformer:
-            return self._demix_roformer(mix)
+        """(2, N) ndarray -> {instrument: (2, N) ndarray} (mdxc_separator.py:272-343, :406-434) or the single target's array; None on the ranks
+        other than 0 of a sharded run."""
         orig = np.ascontiguousarray(mix, dtype=np.float32)
         out = self._demix_stems(orig)
         if out is None:
             return None
-        training = self.model_data_cfgdict["training"]
-        if self.net.num_targets > 1:
-            return {k: v for k, v in zip(training["instruments"], out)}
+        if out.shape[0] > 1:  # one row per stem of a multi-stem model
+            return dict(zip(self.model_data_cfgdict["training"]["instruments"], out))
         primary = out[0]
         if self.is_primary_stem_main_target:  # single-target models also return the residual as the secondary stem (:452-461)
             return {self.primary_stem_name: primary, self.secondary_stem_name: orig - primary}
@@ -170,33 +129,15 @@ class MDXCSeparator(CommonSeparator):
             self._select_engine()
         mix = normalize(wave=np.array(mix, dtype=np.float32), max_peak=self.normalization_threshold, min_peak=self.amplification_threshold)  # :149
         source = self.demix(mix)
-        output_files = []
         if source is None:  # sharded, rank != 0: rank 0 holds the stems and writes the files
-            return output_files
-        if isinstance(source, dict):  # (:156-214)
-            training = self.model_data_cfgdict["training"]
-            stem_list = [training["target_instrument"]] if training.get("target_instrument") else list(training["instruments"])
-            norm = lambda w: normalize(wave=w, max_peak=self.normalization_threshold, min_peak=self.amplification_threshold).T  # noqa: E731
-            if self.process_all_stems and len(stem_list) > 2:  # every stem of a multi-stem model, in the model's order
-                for stem_name in stem_list:
-                    if self.output_single_stem and self.output_single_stem.lower() != stem_name.lower():
-                        continue
-                    path = self.get_stem_output_path(stem_name, custom_output_names)
-                    self.final_process(path, norm(source[stem_name]), stem_name)
-                    output_files.append(path)
-                return output_files
-            self.primary_source, self.secondary_source = norm(source[self.primary_stem_name]), norm(source[self.secondary_stem_name])
-            for name, src in ((self.secondary_stem_name, self.secondary_source), (self.primary_stem_name, self.primary_source)):  # secondary file first
-                if self.output_single_stem and self.output_single_stem.lower() != name.lower():
-                    continue
-                path = self.get_stem_output_path(name, custom_output_names)
-                self.final_process(path, src, name)
-                output_files.append(path)
-            return output_files
-        # a bare array = a single-source model without a target instrument: only the primary stem is written, as it is (:216-226)
-        if not self.output_single_stem or self.output_single_stem.lower() == self.primary_stem_name.lower():
+            return []
+        if not isinstance(source, dict):  # a single-source model without a target instrument: only the primary stem is written, as it is (:216-226)
             self.primary_source = source.T
-            path = self.get_stem_output_path(self.primary_stem_name, custom_output_names)
-            self.final_process(path, self.primary_source, self.primary_stem_name)
-            output_files.append(path)
-        return output_files
+            return self.write_stems([(self.primary_stem_name, self.primary_source)], custom_output_names)
+        training = self.model_data_cfgdict["training"]  # (:156-214)
+        stem_list = [training["target_instrument"]] if training.get("target_instrument") else list(training["instruments"])
+        norm = lambda w: normalize(wave=w, max_peak=self.normalization_threshold, min_peak=self.amplification_threshold).T  # noqa: E731
+        if self.process_all_stems and len(stem_list) > 2:  # every stem of a multi-stem model, in the model's order
+            return self.write_stems([(name, norm(source[name])) for name in stem_list], custom_output_names)
+        self.primary_source, self.secondary_source = norm(source[self.primary_stem_name]), norm(source[self.secondary_stem_name])
+        return self.write_stems([(self.secondary_stem_name, self.secondary_source), (self.primary_stem_name, self.primary_source)], custom_output_names)

@@ -13,11 +13,10 @@ import math
 import os
 
 import numpy as np
-import torch
 
 from ..b200 import vr_params
 from ..b200.vr import NN_ARCH_SIZES, VR_51_SIZES, VREngine, VRNet, VRNet51
-from ..common_separator import CommonSeparator, tensor_core_math
+from ..common_separator import CommonSeparator, load_checkpoint, tensor_core_math
 
 
 class VRSeparator(CommonSeparator):
@@ -37,32 +36,17 @@ class VRSeparator(CommonSeparator):
         self.high_end_process = arch_config.get("high_end_process", False)
         self.aggression_setting = int(arch_config.get("aggression", 5))
         self.aggression = float(self.aggression_setting / 100)
-        self.sharded = bool(arch_config.get("b200_sharded", False))  # one process per GPU (torch.distributed, nccl): split every track's patches over the ranks
-        if not torch.cuda.is_available():
-            raise RuntimeError("VRSeparator (H100 build) needs a CUDA device: there is no CPU path in this package")
-        self.dist = None
-        if self.sharded:
-            import torch.distributed as dist
-
-            if not dist.is_initialized():
-                raise RuntimeError("vr_params['b200_sharded'] needs torch.distributed to be initialised (backend nccl, one process per GPU)")
-            self.dist = dist
-        self.torch_device = torch.device("cuda", torch.cuda.current_device())
+        self.setup_device(arch_config, "VRSeparator", "vr_params")
         self.model_samplerate = self.model_params["sr"]
         self.load_model()
 
     def load_model(self):
-        """nets.determine_model_capacity(bins * 2, nn_arch_size).load_state_dict(torch.load(path)) (vr_separator.py:166-181)."""
+        """nets.determine_model_capacity(bins * 2, nn_arch_size).load_state_dict(checkpoint) (vr_separator.py:166-181)."""
         model_size = math.ceil(os.stat(self.model_path).st_size / 1024)
         nn_arch_size = min(NN_ARCH_SIZES, key=lambda x: abs(x - model_size))
         arch = int(self.model_data.get("b200_nn_architecture", nn_arch_size))  # tests use reduced widths whose file size is off the table
         self.is_vr_51_model = self.is_vr_51_model or arch in VR_51_SIZES  # :175-179
-        if self.model_path.lower().endswith(".npz"):
-            with np.load(self.model_path) as z:
-                state = {k: z[k] for k in z.files}
-        else:
-            sd = torch.load(self.model_path, map_location="cpu", weights_only=True)
-            state = {k: v.numpy() for k, v in sd.items()}
+        state = load_checkpoint(self.model_path)
         tc_math = tensor_core_math("VR", self.use_autocast)
         if self.is_vr_51_model:
             self.net = VRNet51(self.model_params["bins"] * 2, self.model_capacity[0], self.model_capacity[1], state, nn_arch_size=arch, device=self.torch_device,
@@ -80,19 +64,10 @@ class VRSeparator(CommonSeparator):
         stems = self.engine.separate(np.asarray(wave, dtype=np.float32), enable_tta=bool(self.enable_tta),
                                      post_process_threshold=self.post_process_threshold if self.enable_post_process else None,
                                      high_end_process=bool(self.high_end_process), sr=44100)
-        output_files = []
         if stems is None:  # sharded, rank != 0: rank 0 holds the stems and writes the files
-            return output_files
+            return []
         primary, secondary = stems
         self.primary_source, self.secondary_source = primary.T, secondary.T
         if self.output_single_stem and self.output_single_stem.lower() not in (self.primary_stem_name.lower(), self.secondary_stem_name.lower()):
             self.output_single_stem = None  # vr_separator.py:197-199
-        if not self.output_single_stem or self.output_single_stem.lower() == self.primary_stem_name.lower():
-            self.primary_stem_output_path = self.get_stem_output_path(self.primary_stem_name, custom_output_names)
-            self.final_process(self.primary_stem_output_path, self.primary_source, self.primary_stem_name)
-            output_files.append(self.primary_stem_output_path)
-        if not self.output_single_stem or self.output_single_stem.lower() == self.secondary_stem_name.lower():
-            self.secondary_stem_output_path = self.get_stem_output_path(self.secondary_stem_name, custom_output_names)
-            self.final_process(self.secondary_stem_output_path, self.secondary_source, self.secondary_stem_name)
-            output_files.append(self.secondary_stem_output_path)
-        return output_files
+        return self.write_stems([(self.primary_stem_name, self.primary_source), (self.secondary_stem_name, self.secondary_source)], custom_output_names)

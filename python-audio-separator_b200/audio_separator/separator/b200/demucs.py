@@ -565,7 +565,7 @@ class DemucsEngine:
 
     def gather(self, part: torch.Tensor, N: int):
         """Rank 0: the full (S, 2, N) sources from every rank's demix_device slice (None elsewhere); identity on a single GPU."""
-        return self.runner.gather_cols(part, [self.runner.out_range(N, r) for r in range(self.runner.world)], N)
+        return self.runner.gather(part, N)
 
     def demix_host(self, mix_host: torch.Tensor, out_host: torch.Tensor, shift_offsets):
         """End-to-end entry point on page-locked host tensors: mix_host (2, N) -> out_host (S, 2, N).  Sharded runs map the SAME two buffers in every rank:

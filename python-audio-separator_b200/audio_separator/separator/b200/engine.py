@@ -40,6 +40,28 @@ def _stream() -> int:
     return torch.cuda.current_stream().cuda_stream
 
 
+def normalize_scale(peak: float, max_peak: float, min_peak) -> float:
+    """The factor spec_utils.normalize (and b200sep_normalize) applies to a signal whose absolute peak is `peak`: max_peak / peak above max_peak,
+    min_peak / peak for a nonzero peak below min_peak (None: never amplify), 1 otherwise."""
+    if peak > max_peak:
+        return max_peak / peak
+    if min_peak is not None and 0 < peak < min_peak:
+        return min_peak / peak
+    return 1.0
+
+
+def peak_normalize(x: torch.Tensor, max_peak, min_peak, peak: torch.Tensor | None = None):
+    """spec_utils.normalize of the contiguous CUDA tensor x on the device -> (normalised copy, (1,) float32 device peak).  The peak is x's own
+    (b200sep_absmax) unless the caller passes one, e.g. a peak all-reduced over the ranks."""
+    if peak is None:
+        peak = torch.empty(1, dtype=torch.float32, device=x.device)
+        check(lib.b200sep_absmax(_ptr(x), x.numel(), _ptr(peak), _stream()), "absmax")
+    out = torch.empty_like(x)
+    min_peak = -1.0 if min_peak is None else float(min_peak)
+    check(lib.b200sep_normalize(_ptr(x), x.numel(), _ptr(peak), float(max_peak), min_peak, _ptr(out), _stream()), "normalize")
+    return out, peak
+
+
 class StftPlan:
     """b200sep_stft_plan handle (replaces STFT.__init__, uvr_lib_v5/stft.py:11-18)."""
 
@@ -266,9 +288,7 @@ class MdxEngine:
         if self.runner.world > 1:
             dist = self.runner.dist
             dist.all_reduce(peak, op=dist.ReduceOp.MAX, group=self.runner.group)
-        min_peak = -1.0 if amplification_threshold is None else float(amplification_threshold)
-        partn = torch.empty_like(part)
-        check(lib.b200sep_normalize(_ptr(part), part.numel(), _ptr(peak), float(normalization_threshold), min_peak, _ptr(partn), _stream()), "normalize")
+        partn, _ = peak_normalize(part, normalization_threshold, amplification_threshold, peak)
         peak_h = float(peak.item())  # `source = demix(mix) * peak` (:159): out_scale is a host float in the C ABI
         sl = _window(partn[:, :n_part], p0 - self.trim - lo, p0 - self.trim - lo + max(p1 - p0, 1))
         prim = torch.empty((max(n_q, 1), 2), dtype=torch.float32, device=self.device)
@@ -283,35 +303,19 @@ class MdxEngine:
     # ---- array-level body of MDXSeparator.separate (mdx_separator.py:152-182)
     def separate_device(self, mix_dev: torch.Tensor, normalization_threshold=0.9, amplification_threshold=0.0):
         """mix_dev (2,N) float32 CUDA as loaded -> (primary (N,2), secondary (N,2)) CUDA float32; (None, None) on the ranks other than 0."""
-        n = mix_dev.numel()
-        peak = torch.empty(1, dtype=torch.float32, device=self.device)
-        check(lib.b200sep_absmax(_ptr(mix_dev), n, _ptr(peak), _stream()), "absmax")  # :155
-        mixn = torch.empty_like(mix_dev)
-        min_peak = -1.0 if amplification_threshold is None else float(amplification_threshold)
-        check(lib.b200sep_normalize(_ptr(mix_dev), n, _ptr(peak), float(normalization_threshold), min_peak, _ptr(mixn), _stream()), "normalize")  # :156
+        mixn, peak = peak_normalize(mix_dev, normalization_threshold, amplification_threshold)  # :155-156
         # `source = demix(mix) * peak` (:159): out_scale is a host float in the C ABI; read the peak back (4 bytes)
         peak_h = float(peak.item())
         return self.demix_device(mixn, out_scale=peak_h, with_secondary=True, interleave=True)
 
     def to_pcm16(self, stem: torch.Tensor, normalization_threshold=0.9, amplification_threshold=0.0):
-        """write_audio_pydub's sample path on the device (common_separator.py:310-339): returns int16 (N*2,) or None."""
-        stem = stem.contiguous()
-        n = stem.numel()
-        peak = torch.empty(1, dtype=torch.float32, device=self.device)
-        check(lib.b200sep_absmax(_ptr(stem), n, _ptr(peak), _stream()), "absmax")
-        norm = torch.empty_like(stem)
-        min_peak = -1.0 if amplification_threshold is None else float(amplification_threshold)
-        check(lib.b200sep_normalize(_ptr(stem), n, _ptr(peak), float(normalization_threshold), min_peak, _ptr(norm), _stream()), "normalize")
+        """write_audio_pydub's sample path on the device (common_separator.py:310-339): returns int16 (N*2,), or None for a near-silent stem."""
+        norm, peak = peak_normalize(stem.contiguous(), normalization_threshold, amplification_threshold)
         pk = float(peak.item())
-        s = 1.0
-        if pk > normalization_threshold:
-            s = normalization_threshold / pk
-        elif min_peak >= 0 and pk < min_peak:
-            s = min_peak / pk
-        if pk * s < 1e-6:
+        if pk * normalize_scale(pk, normalization_threshold, amplification_threshold) < 1e-6:
             return None
-        out = torch.empty(n, dtype=torch.int16, device=self.device)
-        check(lib.b200sep_to_pcm16(_ptr(norm), n, _ptr(out), _stream()), "to_pcm16")
+        out = torch.empty(norm.numel(), dtype=torch.int16, device=self.device)
+        check(lib.b200sep_to_pcm16(_ptr(norm), norm.numel(), _ptr(out), _stream()), "to_pcm16")
         return out
 
 
@@ -479,4 +483,4 @@ class MdxcEngine:
 
     def gather(self, part: torch.Tensor, N: int):
         """Rank 0: the full (S, 2, N) stems from every rank's demix_device slice (None elsewhere); identity on a single GPU."""
-        return self.runner.gather_cols(part, [self.runner.out_range(N, r) for r in range(self.runner.world)], N)
+        return self.runner.gather(part, N)

@@ -351,4 +351,4 @@ class RoformerEngine:
 
     def gather(self, part: torch.Tensor, N: int):
         """Rank 0: the full (n_out, 2, N) stems from every rank's demix_device slice (None elsewhere); identity on a single GPU."""
-        return self.runner.gather_cols(part, [self.runner.out_range(N, r) for r in range(self.runner.world)], N)
+        return self.runner.gather(part, N)

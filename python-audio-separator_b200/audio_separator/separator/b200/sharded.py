@@ -237,3 +237,7 @@ class ShardRunner:
         for q0, q1, t in stage:
             full[..., q0:q1] = t
         return full
+
+    def gather(self, part: torch.Tensor, n: int):
+        """gather_cols over the even partition of n (out_range): every rank's (..., q1 - q0) slice -> the full (..., n) tensor on rank 0."""
+        return self.gather_cols(part, [self.out_range(n, r) for r in range(self.world)], n)

@@ -42,6 +42,16 @@ def tensor_core_math(arch: str, use_autocast) -> int:
     return MATH_FP16 if use_autocast and arch in AUTOCAST_FP16_ARCHS else MATH_BF16X3
 
 
+def load_checkpoint(path) -> dict:
+    """Model weights -> {name: ndarray}: a `.npz` as stored, anything else through torch.load(weights_only=True) as float32 arrays (the
+    `state_dict` entry of a training checkpoint, the mapping itself otherwise)."""
+    if path.lower().endswith(".npz"):
+        with np.load(path) as z:
+            return {k: z[k] for k in z.files}
+    sd = torch.load(path, map_location="cpu", weights_only=True)
+    return {k: v.float().numpy() for k, v in sd.get("state_dict", sd).items()}
+
+
 class DeviceStem:
     """A float stem that lives in HBM.  `primary_source` / `secondary_source` of a plugin hold these after separate(); np.asarray(stem) downloads it
     (once) for code that expects the reference's host arrays, while write_audio consumes the tensor directly."""
@@ -102,6 +112,22 @@ class CommonSeparator:
 
     def separate(self, audio_file_path, custom_output_names=None):
         raise NotImplementedError
+
+    def setup_device(self, arch_config, name, params_key, missing="CPU path"):
+        """Sets `torch_device` (the current CUDA device), `sharded` (arch key `b200_sharded`: one process per GPU under an initialised
+        torch.distributed group, nccl, every track split by time over the ranks) and `dist` (the torch.distributed module when sharded, else
+        None).  `name` (the plugin's class), `params_key` (its *_params argument) and `missing` (what this package lacks) word the errors."""
+        self.sharded = bool(arch_config.get("b200_sharded", False))
+        if not torch.cuda.is_available():
+            raise RuntimeError(f"{name} (H100 build) needs a CUDA device: there is no {missing} in this package")
+        self.dist = None
+        if self.sharded:
+            import torch.distributed as dist
+
+            if not dist.is_initialized():
+                raise RuntimeError(f"{params_key}['b200_sharded'] needs torch.distributed to be initialised (backend nccl, one process per GPU)")
+            self.dist = dist
+        self.torch_device = torch.device("cuda", torch.cuda.current_device())
 
     def get_roformer_loading_stats(self):
         return {}
@@ -218,33 +244,34 @@ class CommonSeparator:
         self.write_audio(stem_path, source)
         return {stem_name: source}
 
+    def write_stems(self, stems, custom_output_names):
+        """Writes the (stem_name, source) pairs in their order -- only the one named `output_single_stem` (any case) when that is set -- and returns
+        the paths written.  The path of the primary / secondary stem is also kept in primary_stem_output_path / secondary_stem_output_path."""
+        paths = []
+        for name, source in stems:
+            if self.output_single_stem and self.output_single_stem.lower() != name.lower():
+                continue
+            path = self.get_stem_output_path(name, custom_output_names)
+            self.logger.info(f"Saving {name} stem to {path}...")
+            self.final_process(path, source, name)
+            if name == self.primary_stem_name:
+                self.primary_stem_output_path = path
+            elif name == self.secondary_stem_name:
+                self.secondary_stem_output_path = path
+            paths.append(path)
+        return paths
+
     def _output_bits(self):
         """Output sample width follows the input file (common_separator.py:322-324); 16 bits when unknown."""
         return self.input_bit_depth if self.input_bit_depth in (16, 24, 32) else 16
 
-    def pcm16_interleaved(self, stem_source):
-        """normalise -> near-silence check -> (x*32767).astype(int16) (truncation) -> interleave (common_separator.py:310-339)."""
-        s = normalize(np.array(stem_source, dtype=np.float32, copy=True), self.normalization_threshold, self.amplification_threshold)
-        if np.max(np.abs(s)) < 1e-6:
-            self.logger.warning("Warning: stem_source array is near-silent or empty.")
-            return None
-        return np.ascontiguousarray((s * 32767).astype(np.int16)).reshape(-1)
-
     def _normalized_on_device(self, stem):
         """spec_utils.normalize of a CUDA stem with the b200sep_absmax / _normalize kernels; None (with the reference's warning) for a near-silent stem."""
-        from .b200._lib import check, lib
+        from .b200.engine import normalize_scale, peak_normalize
 
-        x = stem.contiguous()
-        n = x.numel()
-        st = torch.cuda.current_stream().cuda_stream
-        peak = torch.empty(1, dtype=torch.float32, device=x.device)
-        check(lib.b200sep_absmax(x.data_ptr(), n, peak.data_ptr(), st), "absmax")
-        norm = torch.empty_like(x)
-        min_peak = -1.0 if self.amplification_threshold is None else float(self.amplification_threshold)
-        check(lib.b200sep_normalize(x.data_ptr(), n, peak.data_ptr(), float(self.normalization_threshold), min_peak, norm.data_ptr(), st), "normalize")
+        norm, peak = peak_normalize(stem.contiguous(), self.normalization_threshold, self.amplification_threshold)
         pk = float(peak.item())
-        scale = self.normalization_threshold / pk if pk > self.normalization_threshold else (min_peak / pk if (min_peak >= 0 and 0 < pk < min_peak) else 1.0)
-        if pk * scale < 1e-6:
+        if pk * normalize_scale(pk, self.normalization_threshold, self.amplification_threshold) < 1e-6:
             self.logger.warning("Warning: stem_source array is near-silent or empty.")
             return None
         return norm

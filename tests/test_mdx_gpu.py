@@ -186,6 +186,8 @@ def test_demix_and_separate_vs_golden(eng, golden_dir, precision):
         assert pcm.shape == ref_pcm.shape and pcm.dtype == np.int16
         assert np.abs(pcm.astype(np.int32) - ref_pcm.astype(np.int32)).max() <= int(np.ceil(tol * 32767 * 4)) + 1
         assert np.array_equal(pcm, O.to_pcm16(stem, 0.9, 0.0))  # the device conversion itself is bit-exact
+    for amplification_threshold in (0.0, 0.5):  # an all-zero stem is near-silent, also where amplifying would divide by its zero peak
+        assert e.to_pcm16(dev(np.zeros_like(prim)), 0.9, amplification_threshold) is None
     # denoise branch (mdx_separator.py:435-440)
     ed = eng.MdxEngine(net, cfg.n_fft, cfg.hop_length, cfg.dim_f, cfg.segment_size, cfg.overlap, cfg.compensate, enable_denoise=True)
     den = ed.run_model(dev(mix[None, :, : cfg.chunk_size])).cpu().numpy()
