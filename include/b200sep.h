@@ -445,6 +445,16 @@ int b200sep_resample_poly_f32(const float* x, const float* taps, int n_taps, int
  * ratio must lie in [1/16, 16] (B200SEP_ERR_ARG otherwise). */
 int b200sep_resample_sinc_f32(const float* x, int channels, int64_t n_in, const float* table, int n_zeros, int per_zero, double ratio,
                               int64_t n_out, float* y, void* stream);
+/* The input end of the time-domain Demucs v3 forward (uvr_lib_v5/demucs/demucs.py:409-422) on a batch of stereo chunks x (B, 2, length):
+ * stats[b] = {mean, unbiased std} of the channel mean over time, z = (x - mean) / (1e-5 + std) zero-padded to `valid` samples
+ * ((valid - length) / 2 on the left), then julius.resample_frac(z, 1, 2): replicate edges of `width` samples, the two phase filters
+ * taps (2, 2 * width + 1) -> y (B, 2, 2 * valid).  work: b200sep_meanstd_work_floats(B) floats, 16-byte aligned. */
+int b200sep_demucs_upsample2_f32(const float* x, int B, int64_t length, int64_t valid, const float* taps, int width, float* stats, float* y,
+                                 float* work, void* stream);
+/* The output end (demucs.py:437-441): julius.resample_frac(x, 2, 1) on x (B, channels, 2 * valid) with replicate edges of `width` samples and
+ * the filter taps (2 * width + 2), then * stats[b].std + stats[b].mean and center_trim to `length` -> y (B, channels, length). */
+int b200sep_demucs_downsample2_f32(const float* x, int B, int channels, int64_t valid, int64_t length, const float* taps, int width,
+                                   const float* stats, float* y, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------
  * Operators of the BS-Roformer path (uvr_lib_v5/roformer/bs_roformer.py, attend.py; mdxc_separator.py:272-343).

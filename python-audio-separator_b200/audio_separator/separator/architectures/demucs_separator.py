@@ -1,10 +1,11 @@
-"""H100 Demucs architecture plugin (HTDemucs v4 models and bags: htdemucs, htdemucs_ft, ...; Hybrid Demucs v3: hdemucs_mmi, mdx_extra, ...).
+"""H100 Demucs architecture plugin (HTDemucs v4 models and bags: htdemucs, htdemucs_ft, ...; Demucs v3: hdemucs_mmi and the bags mdx / mdx_extra,
+whose members are time-domain Demucs and Hybrid Demucs models).
 
 Plugin contract of the reference's DemucsSeparator (audio_separator/separator/architectures/demucs_separator.py:26-195):
 ctor `(common_config, arch_config)` with arch keys segment_size / shifts / overlap / segments_enabled,
 `separate(path, custom_output_names)`, `demix_demucs(mix) -> (S, 2, N)` with sources 0 and 1 swapped.
 Every forward, the shift trick, the segment overlap-add and the bag average run on the GPU (b200.demucs.DemucsEngine).
-Time-domain Demucs v1 / v2 packages are not part of this path.
+Demucs v1 / v2 packages and the DiffQ-quantised bags (mdx_q, mdx_extra_q) are not part of this path.
 
 arch key `b200_sharded`: one process per GPU under an initialised torch.distributed group (nccl); every rank calls `separate(path)` on the same
 file, the segments of every (model, shift) pass are split by time over the ranks (b200/sharded.py), with rank 0's shift offsets used on every
@@ -18,6 +19,7 @@ import numpy as np
 
 from ..b200.demucs import DemucsEngine, HTDemucsNet
 from ..b200.demucs_loader import load_demucs
+from ..b200.demucs_v3 import DemucsConfig, DemucsNet
 from ..b200.hdemucs import HDemucsConfig, HDemucsNet
 from ..common_separator import CommonSeparator, tensor_core_math
 
@@ -51,7 +53,8 @@ class DemucsSeparator(CommonSeparator):
                     cfg.segment = Fraction(int(self.segment_size))  # demucs_segments: sub.segment = int(segment)
                 except (TypeError, ValueError):
                     pass
-            nets.append((HDemucsNet if isinstance(cfg, HDemucsConfig) else HTDemucsNet)(cfg, state, device=self.torch_device, math=math))
+            klass = HDemucsNet if isinstance(cfg, HDemucsConfig) else DemucsNet if isinstance(cfg, DemucsConfig) else HTDemucsNet
+            nets.append(klass(cfg, state, device=self.torch_device, math=math))
         # segments_enabled=False: apply_model(split=False), one forward over the whole track (HTDemucs raises beyond its training segment, like the reference)
         self.engine = DemucsEngine(nets, bag_weights=weights, overlap=self.overlap, batch_size=self.batch_size, split=bool(self.segments_enabled),
                                    dist=self.dist)

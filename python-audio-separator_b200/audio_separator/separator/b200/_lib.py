@@ -123,6 +123,8 @@ _SIGS = {
     "b200sep_vr_mirror_high_end": (i32, [vp, i32, vp, i32, i32, vp, i32, i32, i32, i32, i32, vp]),
     "b200sep_resample_poly_f32": (i32, [vp, vp, i32, i32, i32, i64, i32, i64, i64, vp, vp]),
     "b200sep_resample_sinc_f32": (i32, [vp, i32, i64, vp, i32, i32, C.c_double, i64, vp, vp]),
+    "b200sep_demucs_upsample2_f32": (i32, [vp, i32, i64, i64, vp, i32, vp, vp, vp, vp]),
+    "b200sep_demucs_downsample2_f32": (i32, [vp, i32, i32, i64, i64, vp, i32, vp, vp, vp]),
     "b200sep_rmsnorm_f32": (i32, [vp, vp, vp, i64, i32, i64, i64, vp]),
     "b200sep_rope_split_heads_f32": (i32, [vp, vp, vp, vp, vp, i32, i32, i32, i32, vp]),
     "b200sep_gemm_kn_f32": (i32, [vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, i64, i64, i64, f32, vp]),

@@ -63,6 +63,9 @@ class HTDemucsConfig:
     def seg_len(self):  # int(self.segment * self.samplerate), htdemucs.py:486
         return int(Fraction(self.segment) * self.samplerate)
 
+    def valid_length(self, length):  # HTDemucs.valid_length (htdemucs.py:469-481): every input runs at the training segment
+        return self.seg_len
+
     def validate(self):
         if self.audio_channels != 2:
             raise ValueError("the H100 HTDemucs path handles stereo models only")
@@ -99,9 +102,8 @@ def sin_embedding_2d_tokens(dim: int, height: int, width: int, max_period: float
 
 
 # --------------------------------------------------------------------------------------------------------- the networks
-class HybridDemucsNet:
-    """What the hybrid (spectrogram + waveform) Demucs nets share: device, math mode, STFT plan and weights, the plain DConv branch, and the
-    spectral front and back ends of the forward.  HTDemucsNet and HDemucsNet add their layers and launch order."""
+class DemucsNetBase:
+    """What every Demucs net shares: device, math mode, device weights and the plain DConv branch."""
 
     def __init__(self, cfg, device=None, math=MATH_BF16X3):
         """math: MATH_BF16X3 (default, ~fp32) or MATH_FP16 (torch.autocast precision) for every tensor-core GEMM, convolution and attention of
@@ -112,7 +114,6 @@ class HybridDemucsNet:
         self.math = int(math)
         self.device = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())  # one process per GPU: the rank's own device
         self.S = len(cfg.sources)
-        self.stft = StftPlan(cfg.nfft, cfg.hop)
         self.W = {}
 
     def _put(self, name, a):
@@ -145,6 +146,15 @@ class HybridDemucsNet:
             groupnorm1(h, W[f"{p}.4.weight"], W[f"{p}.4.bias"])
             x = glu(h, res=x, scale=W[f"{p}.6.scale"])
         return x
+
+
+class HybridDemucsNet(DemucsNetBase):
+    """The spectral front and back ends of the hybrid (spectrogram + waveform) Demucs forwards and their STFT plan.  HTDemucsNet and HDemucsNet add
+    their layers and launch order."""
+
+    def __init__(self, cfg, device=None, math=MATH_BF16X3):
+        super().__init__(cfg, device, math)
+        self.stft = StftPlan(cfg.nfft, cfg.hop)
 
     def spec_in(self, mix, pad_mode):
         """_spec + _magnitude and the input normalisation (htdemucs.py:383-403, :415-424, :501-510; hdemucs.py:529-548, :570-579) on mix
@@ -424,8 +434,9 @@ class HTDemucsNet(HybridDemucsNet):
 # --------------------------------------------------------------------------------------------------------- apply_model / demix
 def group_units(clens, seg, pads):
     """Consecutive units (segments of one apply_model pass) that can share a forward: -> [(j0, j1, input width)].  A model that pads every chunk to its training
-    segment (HTDemucs.valid_length, htdemucs.py:469-481) takes all of them at width `seg`; a model without valid_length (HDemucs) runs every chunk at its own
-    length (apply.py:252-257), so only runs of equal length batch -- in practice all full segments, then the shorter last one."""
+    segment (HTDemucs.valid_length, htdemucs.py:469-481) takes all of them at width `seg`; otherwise `clens` are the input widths (the chunk lengths for HDemucs,
+    which has no valid_length, apply.py:252-257; their valid lengths for Demucs), and only runs of equal width batch -- in practice all full segments, then the
+    shorter last one."""
     if pads:
         return [(0, len(clens), seg)] if clens else []
     groups, j0 = [], 0
@@ -447,6 +458,8 @@ class DemucsEngine:
     Per output sample the passes accumulate in the single-GPU order, so the sharded result is the single-GPU result."""
 
     def __init__(self, nets, bag_weights=None, overlap=0.25, batch_size=4, dist=None, group=None, split=True):
+        """nets: the bag's members, each run at its own segment and padding rule (cfg.seg_len, cfg.valid_length); self.cfg (the first member's)
+        supplies only what a bag shares: sources and sample rate (apply.py:46-50)."""
         _require_cuda()
         self.nets = list(nets)
         cfg = self.nets[0].cfg
@@ -471,7 +484,7 @@ class DemucsEngine:
     def _apply_split(self, net, tensor, offset, length, out, q0, n_out, scale, chan_scale, accumulate):
         """apply_model's split branch on TensorChunk(tensor, offset, length) (apply.py:215-250); the weighted result's samples
         [q0, q0 + n_out) -- this rank's part [r0, r1) of them -- are scaled and written / accumulated into out (S*2, r1 - r0)."""
-        cfg = self.cfg
+        cfg = net.cfg
         seg = cfg.seg_len
         S = len(cfg.sources)
         stride = int((1 - self.overlap) * seg)
@@ -484,18 +497,20 @@ class DemucsEngine:
         ext = _window(tensor, lo, hi)
         local = torch.empty((sh.halo + sh.n_own, S * 2, seg), dtype=torch.float32, device=tensor.device)
 
-        pads = getattr(cfg, "pads_to_segment", True)  # HTDemucs: chunk.padded(valid_length = training segment); HDemucs: every chunk at its own length (apply.py:252-257)
-
         def compute(buf, slot0, unit0, n):
             clens = [min(length - offs[unit0 + j], seg) for j in range(n)]
-            for j0, j1, width in group_units(clens, seg, pads):  # units of one input length form one forward (only the last segment of a pass is shorter)
+            # chunk.padded(model.valid_length(chunk length)) (apply.py:252-257): HTDemucs the training segment, HDemucs the chunk itself, Demucs the nearest
+            # length its convolutions consume whole -- centred, real neighbouring samples where the tensor has them
+            widths = [cfg.valid_length(c) for c in clens]
+            for j0, j1, width in group_units(widths, seg, False):  # units of one input width form one forward (only the last segment of a pass is shorter)
                 batch = _new((j1 - j0, 2, width), tensor)
                 for j in range(j0, j1):
-                    start = offset + offs[unit0 + j] - ((seg - clens[j]) // 2 if pads else 0)
-                    batch[j - j0].copy_(ext[:, start - lo : start - lo + width])
+                    start = offset + offs[unit0 + j] - (width - clens[j]) // 2 - lo
+                    assert 0 <= start and start + width <= ext.shape[-1], (start, width, ext.shape)
+                    batch[j - j0].copy_(ext[:, start : start + width])
                 y = net.graphed(batch)  # (n, S, 2, width): the launch list of the forward (HTDemucs: replayed as one CUDA graph per batch size)
-                for j in range(j0, j1):  # center_trim to the chunk's valid length (apply.py:258), stored from sample 0
-                    d = (seg - clens[j]) // 2 if pads else 0
+                for j in range(j0, j1):  # center_trim to the chunk length (apply.py:258), stored from sample 0
+                    d = (width - clens[j]) // 2
                     buf[slot0 + j, :, : clens[j]].copy_(y[j - j0].reshape(S * 2, width)[:, d : d + clens[j]])
 
         self.runner.wait_all(self.runner.run_units(sh, local, compute, self.batch_size))
@@ -507,10 +522,9 @@ class DemucsEngine:
     def _apply_whole(self, net, tensor, offset, length, out, q0, n_out, scale, chan_scale, accumulate):
         """apply_model's leaf (apply.py:251-260) on TensorChunk(tensor, offset, length): the chunk zero-padded (centred) to model.valid_length(length) -- the training
         segment for HTDemucs, which REFUSES anything longer (htdemucs.py:469-481); the length itself for models without valid_length -- one forward, center_trim."""
-        cfg = self.cfg
+        cfg = net.cfg
         S = len(cfg.sources)
-        seg = cfg.seg_len
-        valid = seg if getattr(cfg, "pads_to_segment", True) else length
+        valid = cfg.valid_length(length)
         if valid < length:
             raise ValueError(f"Given length {length} is longer than training length {valid}")
         delta = valid - length
@@ -536,7 +550,7 @@ class DemucsEngine:
         if not shift_offsets:
             one(net, mix, 0, N, out, 0, N, 1.0, chan_scale, accumulate)
             return out
-        ms = int(0.5 * self.cfg.samplerate)
+        ms = int(0.5 * net.cfg.samplerate)
         pm = torch.zeros((2, N + 2 * ms), dtype=torch.float32, device=mix.device)
         pm[:, ms : ms + N].copy_(mix)
         for i, o in enumerate(shift_offsets):

@@ -1,4 +1,4 @@
-"""Reading Demucs v4 model packages without the reference's Python classes.
+"""Reading Demucs v3 / v4 model packages without the reference's Python classes.
 
 A `.th` file is `torch.save({"klass": HTDemucs, "args": ..., "kwargs": {...}, "state": {...}, ...})`
 (uvr_lib_v5/demucs/states.py:34-64); a bag is a YAML file listing signatures, per-source weights and a segment
@@ -16,6 +16,7 @@ import torch
 import yaml
 
 from .demucs import HTDemucsConfig
+from .demucs_v3 import DemucsConfig
 from .hdemucs import HDemucsConfig
 
 # constructor arguments that must keep the value the H100 graph was built for (htdemucs.py:36-98)
@@ -30,6 +31,12 @@ _MAPPED = ("sources", "audio_channels", "channels", "growth", "nfft", "depth", "
 _HD_REQUIRED = dict(cac=True, wiener_iters=0, end_iters=0, wiener_residual=False, rewrite=True, hybrid=True, channels_time=None)
 _HD_MAPPED = ("sources", "audio_channels", "channels", "growth", "nfft", "depth", "hybrid_old", "freq_emb", "emb_scale", "kernel_size", "time_stride", "stride", "context",
               "context_enc", "norm_starts", "norm_groups", "dconv_mode", "dconv_depth", "dconv_comp", "dconv_attn", "dconv_lstm", "samplerate", "segment")
+
+
+# Demucs (v3 time-domain) constructor arguments (demucs.py:236-272): values the H100 graph is built for, and the ones that map onto DemucsConfig
+_V3_REQUIRED = dict(glu=True, gelu=True, rewrite=True, normalize=True, resample=True)
+_V3_MAPPED = ("sources", "audio_channels", "channels", "growth", "depth", "kernel_size", "stride", "context", "norm_starts", "norm_groups", "dconv_mode",
+              "dconv_depth", "dconv_comp", "dconv_attn", "dconv_lstm", "samplerate", "segment")
 
 
 class _Placeholder:
@@ -79,16 +86,36 @@ def _hdemucs_config(kwargs: dict) -> HDemucsConfig:
     return HDemucsConfig(**fields)
 
 
+def _demucs_v3_config(kwargs: dict) -> DemucsConfig:
+    for k, v in _V3_REQUIRED.items():
+        if k in kwargs and kwargs[k] != v:
+            raise NotImplementedError(f"Demucs option {k}={kwargs[k]!r} is outside the supported structure (needs {v!r})")
+    if kwargs.get("lstm_layers", 0):
+        raise NotImplementedError("Demucs lstm_layers > 0 (the bottleneck BLSTM) is not supported")
+    fields = {k: kwargs[k] for k in _V3_MAPPED if k in kwargs}
+    if "sources" in fields:
+        fields["sources"] = tuple(fields["sources"])
+    cfg = DemucsConfig(**fields)
+    if cfg.kernel_size != 2 * cfg.stride:
+        raise NotImplementedError(f"Demucs kernel_size={cfg.kernel_size} with stride={cfg.stride}: only kernel_size == 2 * stride is supported")
+    return cfg
+
+
 def config_from_package(package: dict):
     klass = package["klass"]
     name = getattr(klass, "__name__", str(klass))
-    if name not in ("HTDemucs", "HDemucs"):
-        raise NotImplementedError(f"model class {name}: the H100 Demucs path covers HTDemucs (v4) and HDemucs (v3 hybrid) packages; Demucs v1 / v2 time-domain models are not built")
+    # v1 / v2 packages pickle classes of the same name from demucs.model / model_v2 / tasnet: only demucs.demucs.Demucs is the v3 network
+    v3 = name == "Demucs" and getattr(klass, "__module__", "").rsplit(".", 1)[-1] == "demucs"
+    if name not in ("HTDemucs", "HDemucs") and not v3:
+        raise NotImplementedError(f"model class {getattr(klass, '__module__', '?')}.{name}: the H100 Demucs path covers HTDemucs (v4), HDemucs (v3 hybrid) and "
+                                  "Demucs (v3 time-domain, module demucs.demucs) packages; Demucs v1 / v2 models are not built")
     kwargs = dict(package.get("kwargs", {}))
     if package.get("args"):
         raise ValueError("positional constructor arguments in a Demucs package are not supported")
     if name == "HDemucs":
         return _hdemucs_config(kwargs)
+    if v3:
+        return _demucs_v3_config(kwargs)
     for k, v in _REQUIRED.items():
         if k in kwargs and kwargs[k] != v:
             raise NotImplementedError(f"HTDemucs option {k}={kwargs[k]!r} is outside the supported structure (needs {v!r})")
@@ -114,7 +141,7 @@ def state_from_package(package: dict) -> dict:
 
 def load_demucs(model_path: str):
     """get_model(name, repo) of demucs/pretrained.py:58-79 for a local repo: `model_path` is a bag `.yaml` or a single `.th`.
-    -> (list of (HTDemucsConfig, state dict), bag weights or None, bag segment or None)"""
+    -> (list of (HTDemucsConfig / HDemucsConfig / DemucsConfig, state dict), bag weights or None, bag segment or None)"""
     repo = os.path.dirname(os.path.abspath(model_path))
     if model_path.endswith((".yaml", ".yml")):
         with open(model_path) as f:

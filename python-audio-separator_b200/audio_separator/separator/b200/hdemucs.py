@@ -16,7 +16,7 @@ import numpy as np
 import torch
 
 from ._lib import MATH_BF16X3, check, lib
-from .demucs import HybridDemucsNet
+from .demucs import DemucsNetBase, HybridDemucsNet
 from .engine import _ptr, _stream
 from .ops import (ACT_GELU, ACT_NONE, _new, block_conv_weight, block_convtr_weight, conv2d, conv_transpose, ew, glu, groupnorm, groupnorm1, linear, lstm_bidir,
                   lstm_bidir_weights)
@@ -64,6 +64,9 @@ class HDemucsConfig:
 
     pads_to_segment = False  # apply_model runs every chunk at its own length (no valid_length)
 
+    def valid_length(self, length):  # HDemucs has no valid_length: apply_model runs a chunk at its own length (apply.py:252-257)
+        return length
+
     def validate(self):
         if self.audio_channels != 2:
             raise ValueError("the H100 HDemucs path handles stereo models only")
@@ -108,20 +111,14 @@ def layer_plan(cfg: HDemucsConfig):
     return plan
 
 
-class HDemucsNet(HybridDemucsNet):
-    """Device-resident HDemucs weights + the launch sequence of one forward."""
+class DemucsLayers(DemucsNetBase):
+    """The encoder and decoder layers of the v3 models (HEncLayer / HDecLayer, hdemucs.py:67-330, with the DConv branch and its BLSTM / LocalState)
+    and the device layout of their weights, under the HEncLayer / HDecLayer parameter names.  HDemucsNet runs them in both branches of the hybrid
+    model; DemucsNet (demucs_v3.py) runs them as the whole time-domain Demucs, whose layers are the time branch's."""
 
-    def __init__(self, cfg: HDemucsConfig, state: dict, device=None, math=MATH_BF16X3):
-        super().__init__(cfg, device, math)
-        self.plan = layer_plan(cfg)
-        self.encs = [(f"encoder.{i}", P["enc"]) for i, P in enumerate(self.plan)]
-        self.decs = [(f"decoder.{j}", P["dec"]) for j, P in enumerate(self.plan[::-1])]
-        tencs = [P["tenc"] for P in self.plan if P["tenc"] is not None]
-        tdecs = [P["tdec"] for P in self.plan if P["tdec"] is not None][::-1]
-        self.tencs = [(f"tencoder.{i}", L) for i, L in enumerate(tencs)]
-        self.tdecs = [(f"tdecoder.{j}", L) for j, L in enumerate(tdecs)]
-        st = {k: np.asarray(v, dtype=np.float32) for k, v in state.items()}
-        self._check_structure(st)
+    def _load_weights(self, st):
+        """Host arrays (float32) of the layer parameters -> device tensors in the layouts the operators take."""
+        cfg = self.cfg
         for name, a in st.items():
             if ".lstm." in name:
                 continue  # repacked below
@@ -140,32 +137,6 @@ class HDemucsNet(HybridDemucsNet):
                 p = name[: -len(".weight_ih_l0")]
                 for layer in range(cfg.lstm_layers):
                     self.W[f"{p}.{layer}"] = lstm_bidir_weights(st, p, layer, self.device)
-        if cfg.freq_emb:
-            # ScaledEmbedding.forward * freq_emb_scale (hdemucs.py:62-64, :708-713) as one value per (channel, frequency) row
-            emb = st["freq_emb.embedding.weight"] * np.float32(cfg.emb_scale)  # (Fr, C)
-            self._put("freq_emb:rows", (np.float32(cfg.freq_emb) * emb).T.reshape(-1))
-        self.graphed = self.forward  # variable lengths: launched directly
-
-    def _check_structure(self, st):
-        cfg = self.cfg
-        for prefix, L in self.encs + self.tencs:
-            w = st.get(f"{prefix}.conv.weight")
-            if w is None or w.shape[0] != L["chout"] or w.shape[1] != L["chin"] or w.shape[2] != L["k"]:
-                raise ValueError(f"{prefix}.conv.weight {None if w is None else w.shape} does not match the configured HDemucs structure {L}")
-            if (f"{prefix}.norm1.weight" in st) != (L["norm"] and not L["empty"]):
-                raise ValueError(f"{prefix}: GroupNorm presence does not match norm_starts={cfg.norm_starts}")
-        if f"encoder.{cfg.depth}.conv.weight" in st:
-            raise ValueError(f"state dict is deeper than depth {cfg.depth}")
-        if any(".query_freqs." in n for n in st):
-            raise ValueError("LocalState with nfreqs > 0 is not supported")
-        for prefix, L in self.encs + self.tencs + self.decs + self.tdecs:
-            if L["empty"] or not L["dconv"]:
-                continue
-            if L["freq"] and L["k"] != cfg.kernel_size and (L["lstm"] or L["attn"]):
-                pass  # the merge layer: one frequency row after its convolution
-            has_lstm = f"{prefix}.dconv.layers.0.3.lstm.weight_ih_l0" in st
-            if has_lstm != L["lstm"]:
-                raise ValueError(f"{prefix}: BLSTM presence does not match dconv_lstm={cfg.dconv_lstm}")
 
     # ---- DConv with BLSTM / LocalState ----------------------------------------------------------------------------------------
     def _blstm(self, h, p):
@@ -203,7 +174,7 @@ class HDemucsNet(HybridDemucsNet):
         return conv2d(res, W[f"{p}.proj.weight"], W[f"{p}.proj.bias"], C, (1, 1), add=h, math=self.math)
 
     def _dconv_layer(self, x, prefix, L):
-        """DConv.forward (demucs.py:166-168) for the layer kinds of this model: the plain branch (HybridDemucsNet._dconv), or conv -> GroupNorm+GELU ->
+        """DConv.forward (demucs.py:166-168) for the layer kinds of this model: the plain branch (DemucsNetBase._dconv), or conv -> GroupNorm+GELU ->
         BLSTM -> LocalState -> 1x1 -> GroupNorm -> GLU with the LayerScale residual."""
         if not (L["lstm"] or L["attn"]):
             return self._dconv(x, prefix)
@@ -240,9 +211,9 @@ class HDemucsNet(HybridDemucsNet):
         else:
             if x.shape[2] != 1:
                 raise ValueError(f"{prefix}: a time layer needs one frequency row, got {tuple(x.shape)}")
-            le = x.shape[-1]  # F.pad to a multiple of the stride == implicit zero columns on the right
+            le = -(-x.shape[-1] // s) * s  # F.pad to a multiple of the stride == implicit zero columns on the right
             y = conv2d(x, W[f"{prefix}.conv.weight"], W[f"{prefix}.conv.bias"], co, (1, k), s=(1, s), p=(0, pad), act=fused_act, add=inject, add_before_act=inject is not None,
-                       out_hw=(1, -(-le // s)), math=self.math)
+                       out_hw=(1, (le + 2 * pad - k) // s + 1), math=self.math)
         if L["empty"]:
             return y
         if L["norm"]:
@@ -284,7 +255,7 @@ class HDemucsNet(HybridDemucsNet):
         full = (n_in + 1) * s  # (n_in - 1) * s + kernel, kernel = 2 * s
         target = full - 2 * pad if L["freq"] else length
         wt, bt = W[f"{prefix}.conv_tr.weight"], W[f"{prefix}.conv_tr.bias"]
-        if not L["norm"]:
+        if not L.get("norm_tr", L["norm"]):  # norm_tr: the time-domain Demucs, whose outermost decoder has no GroupNorm after its transposed convolution
             return conv_transpose(y, wt, bt, co, axis, s, pad, target, act, math=self.math), y
         # GroupNorm sees the UNtrimmed transposed convolution (hdemucs.py:322-328: norm2, then the crop, then GELU)
         z = conv_transpose(y, wt, bt, co, axis, s, 0, full, ACT_NONE, math=self.math)
@@ -292,6 +263,49 @@ class HDemucsNet(HybridDemucsNet):
         if target != full:
             z = (z[:, :, pad : pad + target, :] if L["freq"] else z[:, :, :, pad : pad + target]).contiguous()  # a strided device copy
         return z, y
+
+
+class HDemucsNet(HybridDemucsNet, DemucsLayers):
+    """Device-resident HDemucs weights + the launch sequence of one forward."""
+
+    def __init__(self, cfg: HDemucsConfig, state: dict, device=None, math=MATH_BF16X3):
+        super().__init__(cfg, device, math)
+        self.plan = layer_plan(cfg)
+        self.encs = [(f"encoder.{i}", P["enc"]) for i, P in enumerate(self.plan)]
+        self.decs = [(f"decoder.{j}", P["dec"]) for j, P in enumerate(self.plan[::-1])]
+        tencs = [P["tenc"] for P in self.plan if P["tenc"] is not None]
+        tdecs = [P["tdec"] for P in self.plan if P["tdec"] is not None][::-1]
+        self.tencs = [(f"tencoder.{i}", L) for i, L in enumerate(tencs)]
+        self.tdecs = [(f"tdecoder.{j}", L) for j, L in enumerate(tdecs)]
+        st = {k: np.asarray(v, dtype=np.float32) for k, v in state.items()}
+        self._check_structure(st)
+        self._load_weights(st)
+        if cfg.freq_emb:
+            # ScaledEmbedding.forward * freq_emb_scale (hdemucs.py:62-64, :708-713) as one value per (channel, frequency) row
+            emb = st["freq_emb.embedding.weight"] * np.float32(cfg.emb_scale)  # (Fr, C)
+            self._put("freq_emb:rows", (np.float32(cfg.freq_emb) * emb).T.reshape(-1))
+        self.graphed = self.forward  # variable lengths: launched directly
+
+    def _check_structure(self, st):
+        cfg = self.cfg
+        for prefix, L in self.encs + self.tencs:
+            w = st.get(f"{prefix}.conv.weight")
+            if w is None or w.shape[0] != L["chout"] or w.shape[1] != L["chin"] or w.shape[2] != L["k"]:
+                raise ValueError(f"{prefix}.conv.weight {None if w is None else w.shape} does not match the configured HDemucs structure {L}")
+            if (f"{prefix}.norm1.weight" in st) != (L["norm"] and not L["empty"]):
+                raise ValueError(f"{prefix}: GroupNorm presence does not match norm_starts={cfg.norm_starts}")
+        if f"encoder.{cfg.depth}.conv.weight" in st:
+            raise ValueError(f"state dict is deeper than depth {cfg.depth}")
+        if any(".query_freqs." in n for n in st):
+            raise ValueError("LocalState with nfreqs > 0 is not supported")
+        for prefix, L in self.encs + self.tencs + self.decs + self.tdecs:
+            if L["empty"] or not L["dconv"]:
+                continue
+            if L["freq"] and L["k"] != cfg.kernel_size and (L["lstm"] or L["attn"]):
+                pass  # the merge layer: one frequency row after its convolution
+            has_lstm = f"{prefix}.dconv.layers.0.3.lstm.weight_ih_l0" in st
+            if has_lstm != L["lstm"]:
+                raise ValueError(f"{prefix}: BLSTM presence does not match dconv_lstm={cfg.dconv_lstm}")
 
     # ---- forward -------------------------------------------------------------------------------------------------------------
     def forward(self, mix: torch.Tensor) -> torch.Tensor:
