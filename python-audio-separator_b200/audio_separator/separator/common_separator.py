@@ -74,6 +74,8 @@ class CommonSeparator:
     VOCAL_STEM, INST_STEM, OTHER_STEM, BASS_STEM, DRUM_STEM = "Vocals", "Instrumental", "Other", "Bass", "Drums"
     GUITAR_STEM, PIANO_STEM, PRIMARY_STEM, SECONDARY_STEM, NO_STEM = "Guitar", "Piano", "Primary Stem", "Secondary Stem", "No "
     STEM_PAIR_MAPPER = _PAIR
+    _mix_slice = None  # separate_mix: the samples prepare_mix hands to separate() in place of the file's
+    _collected = None  # separate_mix(collect=True): the (stem_name, stem) pairs write_stems collects instead of writing
 
     _CONFIG_KEYS = (
         "logger", "log_level", "torch_device", "torch_device_cpu", "torch_device_mps", "onnx_execution_provider", "model_name", "model_path",
@@ -133,8 +135,27 @@ class CommonSeparator:
         return {}
 
     # ---- input ----------------------------------------------------------------------------------------
+    def separate_mix(self, audio_file_path, mix, custom_output_names=None, collect=False):
+        """separate(audio_file_path, custom_output_names) run on `mix` -- a (C, n) CUDA tensor or DeviceStem holding that file's samples, or one
+        chunk of them, decoded by the caller -- instead of a decode of the file; input_bit_depth stays as the caller's decode set it.  Returns
+        what separate() returns; with `collect`, the stems are not written and the plugin's (stem_name, stem) pairs come back instead, in its
+        order and after its output_single_stem filter, each peak-normalised on the device ((n, 2) float32 CUDA) or None when near-silent."""
+        self._mix_slice, self._collected = mix, ([] if collect else None)
+        try:
+            out = self.separate(audio_file_path, custom_output_names)
+            return self._collected if collect else out
+        finally:
+            self._mix_slice = self._collected = None
+
     def prepare_mix(self, mix):
-        """path or (N, C) ndarray -> float32 (2, N) (common_separator.py:217-282)."""
+        """path, (N, C) ndarray or mix slice ((C, N) CUDA tensor / DeviceStem) -> float32 (2, N) (common_separator.py:217-282).  Inside
+        separate_mix the path separate() passes stands for the caller's samples.  A mix slice leaves input_bit_depth as it is."""
+        if self._mix_slice is not None and isinstance(mix, str):
+            mix = self._mix_slice
+        if isinstance(mix, DeviceStem):
+            mix = mix.tensor
+        if isinstance(mix, torch.Tensor):
+            return self._device_mix(f"{self.audio_file_path} (mix slice)", mix.to(self.torch_device).float().contiguous())
         if isinstance(mix, np.ndarray):
             if self.input_bit_depth is None:
                 self.input_bit_depth, self.input_subtype = 16, "PCM_16"
@@ -251,6 +272,9 @@ class CommonSeparator:
         for name, source in stems:
             if self.output_single_stem and self.output_single_stem.lower() != name.lower():
                 continue
+            if self._collected is not None:
+                self._collected.append((name, self._normalized_on_device(self._cuda_stem(source))))
+                continue
             path = self.get_stem_output_path(name, custom_output_names)
             self.logger.info(f"Saving {name} stem to {path}...")
             self.final_process(path, source, name)
@@ -264,6 +288,13 @@ class CommonSeparator:
     def _output_bits(self):
         """Output sample width follows the input file (common_separator.py:322-324); 16 bits when unknown."""
         return self.input_bit_depth if self.input_bit_depth in (16, 24, 32) else 16
+
+    @staticmethod
+    def _cuda_stem(source):
+        """A float stem as a float32 CUDA tensor (a host array is uploaded)."""
+        if not (isinstance(source, torch.Tensor) and source.is_cuda):
+            source = torch.as_tensor(np.ascontiguousarray(source, dtype=np.float32), device="cuda")
+        return source.float()
 
     def _normalized_on_device(self, stem):
         """spec_utils.normalize of a CUDA stem with the b200sep_absmax / _normalize kernels; None (with the reference's warning) for a near-silent stem."""
@@ -283,15 +314,10 @@ class CommonSeparator:
         bits = self._output_bits()
         via16 = not self.use_soundfile  # write_audio_pydub quantises to int16 first; write_audio_soundfile converts the floats (:322-336 / :391-451)
         if isinstance(stem_source, torch.Tensor) and stem_source.is_cuda:
-            from .b200._lib import check, lib
-
             norm = self._normalized_on_device(stem_source)
             if norm is None:
                 return None
-            n = norm.numel()
-            out = torch.empty(n * bits // 8, dtype=torch.uint8, device=norm.device)
-            check(lib.b200sep_to_pcm_bytes(norm.data_ptr(), n, bits, int(via16), out.data_ptr(), torch.cuda.current_stream().cuda_stream), "to_pcm_bytes")
-            return bits, out.cpu().numpy().tobytes()
+            return bits, self.pack_pcm(norm, bits).tobytes()
         if isinstance(stem_source, np.ndarray) and stem_source.dtype == np.int16:
             q = stem_source.reshape(-1).astype(np.int64)
             via16 = True
@@ -316,6 +342,16 @@ class CommonSeparator:
         b4 = q.astype("<i4").view(np.uint8).reshape(-1, 4)
         return bits, np.ascontiguousarray(b4[:, :3]).tobytes()
 
+    def pack_pcm(self, norm, bits):
+        """A peak-normalised CUDA stem -> its interleaved little-endian PCM at `bits` bits as a host uint8 array, quantised on the device by the
+        writer's rule (b200sep_to_pcm_bytes; int16 first unless use_soundfile)."""
+        from .b200._lib import check, lib
+
+        out = torch.empty(norm.numel() * bits // 8, dtype=torch.uint8, device=norm.device)
+        check(lib.b200sep_to_pcm_bytes(norm.data_ptr(), norm.numel(), bits, int(not self.use_soundfile), out.data_ptr(),
+                                       torch.cuda.current_stream().cuda_stream), "to_pcm_bytes")
+        return out.cpu().numpy()
+
     def write_flac(self, stem_path, stem_source):
         """`.flac` output encoded on the GPU (b200/flac.py).  A CUDA stem never leaves the device as PCM; a host array is uploaded first.  The stored
         samples are the WAV writer's at the input bit depth, at the stream sample size of the reference's writer (flac.stream_bps)."""
@@ -323,9 +359,7 @@ class CommonSeparator:
 
         if isinstance(stem_source, np.ndarray) and stem_source.dtype == np.int16:
             raise TypeError("FLAC output takes float stems")
-        if not (isinstance(stem_source, torch.Tensor) and stem_source.is_cuda):
-            stem_source = torch.as_tensor(np.ascontiguousarray(stem_source, dtype=np.float32), device="cuda")
-        norm = self._normalized_on_device(stem_source.float())
+        norm = self._normalized_on_device(self._cuda_stem(stem_source))
         if norm is None:
             return
         bits = self._output_bits()

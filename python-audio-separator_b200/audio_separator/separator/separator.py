@@ -1,7 +1,9 @@
 """`Separator` facade: same constructor / load_model() / separate() surface as the reference orchestrator
 (audio_separator/separator/separator.py:108-257, :830-933, :935-1045), restricted to what the accelerated path
-needs.  Model download, ensembles, presets and file-level chunking are out of scope (SURVEY.md section 2, rows 1, 14, 15):
-models are looked up in `model_file_dir` only.
+needs.  Model download and ensemble presets are out of scope (SURVEY.md section 2, rows 1, 14): models are looked up in `model_file_dir` only.
+
+`chunk_duration` (seconds) separates a file longer than that in fixed-length chunks and joins the stems (separator.py:1003-1012, :1047-1156):
+the file is decoded once into device memory, every chunk is a slice of it, and every joined stem is written once (DESIGN §28).
 """
 import importlib
 import json
@@ -11,6 +13,7 @@ import re
 import shutil
 import tempfile
 import time
+import wave
 
 import numpy as np
 import torch
@@ -59,8 +62,11 @@ class Separator:
         if self.sample_rate <= 0 or self.sample_rate > 12800000:
             raise ValueError(f"The sample rate setting is {self.sample_rate} but it must be a non-zero whole number.")
         self.use_soundfile, self.use_autocast = use_soundfile, use_autocast
-        if ensemble_preset or chunk_duration:
-            raise NotImplementedError("ensemble presets (ensemble_presets.json) / file-level chunking are outside the H100 hot-path scope; pass the model list and algorithm explicitly")
+        if ensemble_preset:
+            raise NotImplementedError("ensemble presets (ensemble_presets.json) are outside the H100 hot-path scope; pass the model list and algorithm explicitly")
+        if chunk_duration is not None and chunk_duration <= 0:  # separator.py:217-219
+            raise ValueError("chunk_duration must be greater than 0")
+        self.chunk_duration = chunk_duration
         self.ensemble_algorithm = ensemble_algorithm or "avg_wave"  # separator.py:237-238
         self.ensemble_weights = ensemble_weights
         self.ensemble_preset = None
@@ -170,11 +176,14 @@ class Separator:
             original_output_dir = self.output_dir
             try:
                 stems_by_type = {}
-                for model_filename in models:
+                for k, model_filename in enumerate(models):
                     self.logger.info(f"Processing with model: {model_filename}")
                     self.load_model(model_filename)
-                    self.output_dir = temp_dir
-                    self.model_instance.output_dir = temp_dir
+                    # one directory per model: joined chunked stems are named without the model, so models sharing a directory would overwrite
+                    # each other's (the reference's temp directory has that collision)
+                    model_dir = os.path.join(temp_dir, str(k))
+                    self.output_dir = model_dir
+                    self.model_instance.output_dir = model_dir
                     if self.output_format.lower() == "flac":
                         # lossless either way: WAV intermediates hold the samples the reference's FLAC round trip holds, and need no FLAC reader
                         self.model_instance.output_format = "WAV"
@@ -195,7 +204,7 @@ class Separator:
                             stem = "Instrumental"  # the non-vocal stem of a two-stem model
                         else:
                             stem = STEM_NAME_MAP.get(low, raw.title())
-                        stems_by_type.setdefault(stem, []).append(stem_path if os.path.isabs(stem_path) else os.path.join(temp_dir, stem_path))
+                        stems_by_type.setdefault(stem, []).append(stem_path if os.path.isabs(stem_path) else os.path.join(model_dir, stem_path))
                 ensembler = Ensembler(self.logger, self.ensemble_algorithm, self.ensemble_weights)
                 base_name = os.path.splitext(os.path.basename(path))[0]
                 writer = self.model_instance
@@ -228,8 +237,83 @@ class Separator:
 
     def _separate_file(self, audio_file_path, custom_output_names=None):
         t0 = time.perf_counter()
-        out = self.model_instance.separate(audio_file_path, custom_output_names)
+        if self.chunk_duration is not None:
+            out = self._separate_chunked(audio_file_path, custom_output_names)
+        else:
+            out = self.model_instance.separate(audio_file_path, custom_output_names)
         self.model_instance.clear_gpu_cache()
         self.model_instance.clear_file_specific_paths()
         self.logger.info(f"Separation duration: {time.perf_counter() - t0:.2f}s")
         return out
+
+    def _separate_chunked(self, audio_file_path, custom_output_names=None):
+        """Separator._process_with_chunking (separator.py:1047-1156) without chunk files -> the paths of the stems.  The file is decoded once
+        into device memory.  A file not longer than `chunk_duration` is then separated and written as without chunking, from that decode.
+        Otherwise every chunk is a slice of it that the plugin separates as it would a file holding those samples (CommonSeparator.separate_mix),
+        with its stems normalised on the device.  WAV: each chunk's stems are packed on the device (24-bit input at 32 bits, the width of the
+        reference's joined WAV) and their bytes joined on the host.  FLAC: the normalised floats of each stem are joined in one device buffer and encoded once.  A near-silent chunk stem is
+        left out of its joined stem, as the reference's merge leaves out the file it does not write."""
+        from .b200 import chunking, flac
+        from .common_separator import DeviceStem
+
+        plugin = self.model_instance
+        mix = plugin.prepare_mix(audio_file_path)  # the one decode; sets input_bit_depth / input_subtype
+        mix = mix.tensor if isinstance(mix, DeviceStem) else torch.from_numpy(np.ascontiguousarray(mix, dtype=np.float32)).to(plugin.torch_device)
+        n_frames = mix.shape[1]
+        if not chunking.should_chunk(n_frames, self.sample_rate, self.chunk_duration):
+            return plugin.separate_mix(audio_file_path, mix, custom_output_names)
+        ext = plugin.output_format.lower()
+        if ext not in ("wav", "flac"):
+            raise NotImplementedError(f"chunk_duration writes WAV or FLAC; output_format {plugin.output_format!r} is not supported with it")
+        bounds = chunking.chunk_bounds(n_frames, self.sample_rate, self.chunk_duration)
+        self.logger.info(f"File duration {n_frames / self.sample_rate:.1f}s exceeds chunk size {self.chunk_duration}s: {len(bounds)} chunks")
+        bits = plugin._output_bits()
+        wav_bits = 32 if bits == 24 else bits  # pydub reads a 24-bit WAV as 32-bit samples and writes them back at that width
+        via16 = not plugin.use_soundfile
+        total = sum(b - a for a, b in bounds)
+        parts = {}  # stem key -> WAV: [host uint8 arrays]; FLAC: [device buffer, frames filled]
+        for i, (a, b) in enumerate(bounds):
+            self.logger.info(f"Processing chunk {i + 1}/{len(bounds)}: frames [{a}, {b})")
+            piece = mix[:, a:min(b, n_frames)]
+            if b > n_frames:  # pydub pads a slice that ends past the data with silence
+                piece = torch.cat([piece, piece.new_zeros(mix.shape[0], b - n_frames)], dim=1)
+            stems = plugin.separate_mix(audio_file_path, piece.contiguous(), collect=True)
+            for name, norm in stems:
+                key = chunking.stem_key(plugin.get_stem_output_path(name, None)) or name
+                if norm is None:
+                    self.logger.warning(f"Chunk {i + 1}/{len(bounds)}: the {name} stem is near-silent and is left out of the joined {key} stem")
+                    continue
+                if ext == "flac":
+                    acc = parts.setdefault(key, [torch.empty(total, 2, dtype=torch.float32, device=norm.device), 0])
+                    acc[0][acc[1]:acc[1] + norm.shape[0]].copy_(norm)
+                    acc[1] += norm.shape[0]
+                else:
+                    parts.setdefault(key, []).append(plugin.pack_pcm(norm, wav_bits))
+            plugin.clear_file_specific_paths()
+            plugin.clear_gpu_cache()
+        del mix
+        if plugin.dist is not None and plugin.dist.get_rank() != 0:  # sharded: rank 0 holds the stems and writes the files
+            return []
+        base = os.path.splitext(os.path.basename(audio_file_path))[0]
+        os.makedirs(self.output_dir, exist_ok=True)
+        outputs = []
+        for key in sorted(parts):
+            path = os.path.join(self.output_dir, chunking.joined_name(base, key, ext, custom_output_names))
+            self.logger.info(f"Joining {key} stem into {path}")
+            if ext == "flac":
+                buf, filled = parts[key]
+                bps = flac.stream_bps(bits, bool(plugin.use_soundfile))
+                if bps is None:
+                    self.logger.error(f"Error exporting audio file: libsndfile has no {bits}-bit FLAC subtype, {path} not written")
+                    continue
+                data = flac.encode(buf[:filled], bits, via16, bps, int(self.sample_rate))
+                with open(path, "wb") as f:
+                    f.write(data)
+            else:
+                with wave.open(path, "wb") as wf:
+                    wf.setnchannels(2)
+                    wf.setsampwidth(wav_bits // 8)
+                    wf.setframerate(int(self.sample_rate))
+                    wf.writeframes(np.concatenate(parts[key]))
+            outputs.append(path)
+        return outputs
