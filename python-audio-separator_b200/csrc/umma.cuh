@@ -42,6 +42,23 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   while (!mbar_try_wait(bar, parity))
     if (++spins > (1u << 22)) __trap();
 }
+// Unbounded wait.  For waits inside a wgmma pipeline whose accumulators need most of the register file: the trap path of mbar_wait makes
+// ptxas serialise the wgmma pipeline and spill there (two n144 accumulator sets of the ping-pong 3x3 convolution).
+__device__ __forceinline__ void mbar_wait_spin(uint64_t* bar, uint32_t parity) {
+  while (!mbar_try_wait(bar, parity)) {
+  }
+}
+
+// ---- named barriers (id 0 is __syncthreads; n threads, a multiple of 32) --------------------------------------
+__device__ __forceinline__ void bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+// counts toward barrier id without waiting for it
+__device__ __forceinline__ void bar_arrive(int id, int n) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+
+// ---- per-warpgroup register budget (every warp of the warpgroup executes it; N a multiple of 8 in [24, 256]) ------
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
 
 // ---- TMA ----------------------------------------------------------------------------------------------
 __device__ __forceinline__ void prefetch_tensormap(const CUtensorMap* m) {

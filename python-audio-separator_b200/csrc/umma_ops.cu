@@ -16,7 +16,8 @@
 //          to the OUTPUT side: B holds the three dx filter columns side by side (N = 3*n_c accumulator columns,
 //          P_dx[m] = W[dy][dx] . x[f0+m]) and the epilogue forms out[f0+j] = P_0[j-1] + P_1[j] + P_2[j+1] with warp
 //          shuffles (+ a small smem exchange at warp edges).
-// Warp roles per CTA (288 threads): warps 0-7 = two consumer warpgroups (wgmma issue + epilogue), warp 8 = TMA producer.
+// Warp roles per CTA (288 threads): warps 0-7 = two consumer warpgroups (wgmma issue + epilogue), warp 8 = TMA producer.  The ping-pong 3x3
+// instances have 384 threads: warps 9-11 only hand their registers to the consumers (see conv3_pingpong).
 #include <cuda_bf16.h>
 #include <string.h>
 
@@ -38,7 +39,7 @@ constexpr int kMaxChannels = 1024;  // per-channel scale/shift staged in shared 
 constexpr int kTileM = 128;
 constexpr int kMaxNTile = 128;      // accumulator columns of umma_pair_kernel: n_tile / 2 fp32 registers per consumer thread
 constexpr int kConvStride = 112;    // output pixels per 3x3 tile: rows 8..119 of the 128 loaded pixels [f0 - 8, f0 + 120), so that loads AND stores start 16-byte aligned
-constexpr int kEpiBar = 1;          // named barrier of the 256 consumer threads
+constexpr int kEpiBar = 1;          // named barrier of the 256 consumer threads (ping-pong 3x3: kEpiBar + wg, one per warpgroup)
 
 struct UmmaParams {
   int mode;  // 0 GEMM, 1 CONV3x3, 2 UP (ConvTranspose2d k2 s2), 3 DOWN (Conv2d k2 s2), 4 PW (Conv2d 1x1)
@@ -164,11 +165,18 @@ __device__ __forceinline__ void umma_producer_loop(const CUtensorMap& tmA_hi, co
 // ===== one tile's main loop of a consumer warpgroup =====
 // Per ring stage and 16-deep k-step, mma() issues the three products Ah*Bh + Ah*Bl + Al*Bh into the register accumulator.  A stage is released
 // (one arrive per consumer thread) when the wgmma group that read it has completed, one stage late, so the tensor core always has the next group queued.
-template <class Mma>
-__device__ __forceinline__ void consumer_mainloop(const UmmaParams& p, uint8_t* smem, uint64_t* full_bar, uint64_t* empty_bar, int& s, uint32_t& phase, Mma mma) {
+// issued() runs once the tile's last wgmma group is issued, before the wait for it.  kBoundedWait = false waits for full stages without the
+// trap of mbar_wait (see mbar_wait_spin).
+struct NoHook {
+  __device__ void operator()() const {}
+};
+template <bool kBoundedWait = true, class Mma, class Issued = NoHook>
+__device__ __forceinline__ void consumer_mainloop(const UmmaParams& p, uint8_t* smem, uint64_t* full_bar, uint64_t* empty_bar, int& s, uint32_t& phase, Mma mma,
+                                                  Issued issued = Issued()) {
   int prev = -1;
   for (int i = 0; i < p.num_iters; ++i) {
-    ptx::mbar_wait(&full_bar[s], phase);
+    if constexpr (kBoundedWait) ptx::mbar_wait(&full_bar[s], phase);
+    else ptx::mbar_wait_spin(&full_bar[s], phase);
     const uint32_t st = ptx::smem_u32(smem + (size_t)s * p.stage_bytes);
     const uint32_t a_hi = st, a_lo = st + p.a_bytes;
     const uint32_t b_hi = p.b_resident ? ptx::smem_u32(smem + p.b_res_off + (size_t)i * 2 * p.b_bytes) : st + 2 * p.a_bytes, b_lo = b_hi + p.b_bytes;
@@ -183,8 +191,17 @@ __device__ __forceinline__ void consumer_mainloop(const UmmaParams& p, uint8_t* 
       phase ^= 1;
     }
   }
+  issued();
   ptx::wgmma_wait<0>();
   if (prev >= 0) ptx::mbar_arrive(&empty_bar[prev]);
+}
+// moves a consumer's ring position past n stages that the other consumer warpgroup reads
+__device__ __forceinline__ void ring_skip(const UmmaParams& p, int& s, uint32_t& phase, int n) {
+  s += n;
+  while (s >= p.stages) {
+    s -= p.stages;
+    phase ^= 1;
+  }
 }
 
 // A operand descriptors of consumer warpgroup wg (rows 64*wg..): GEMM = K-major 128-byte-swizzled rows of 64 k; conv modes = the two TMA boxes of
@@ -400,14 +417,108 @@ __device__ __forceinline__ void conv3_mma(float (&acc)[3 * NC / 2], uint64_t da,
   else ptx::wgmma_ss_n240<1>(acc, da, db, accum);
 }
 
+// Which schedule an instance runs, chosen at compile time from the instance:
+//   * ping-pong: each consumer warpgroup owns whole tiles (tiles 2k + wg of the CTA's walk) and issues two m64 products per k-step and bf16
+//     product, one per A box (rows 0-63 into acc[0], rows 64-127 into acc[1]).  A warpgroup issues a tile's MMAs only once the other has issued
+//     all MMAs of the previous tile (named barriers kOrderBar + wg), so one warpgroup's epilogue runs while the other's MMAs keep the tensor
+//     core busy.  The two warpgroups take turns on one output staging buffer: a warpgroup's issuer arrives on sfree_bar once its store has
+//     read the planes out, and the next tile's epilogue waits for that before it writes them.
+//     The two accumulator sets (3 * NC fp32 registers per thread) need more than the 168 registers a 288-thread CTA can give every thread (three
+//     warps share each SM sub-partition's 16K registers), so ping-pong CTAs have 384 threads: the producer warpgroup (warp 8 loads, 9-11 idle)
+//     gives registers back with setmaxnreg and the consumer warpgroups take kPingPongRegs each.
+//   * cooperative (288 threads): the two warpgroups split every tile (rows 0-63 / 64-127) and run its epilogue together.  Kept for the instances
+//     whose two accumulator sets do not fit kPingPongRegs without spilling.
+template <int NC, bool RES, bool MUL>
+__host__ __device__ constexpr bool conv3_pingpong() { return NC <= 32 || (NC == 48 && !MUL); }
+constexpr int kPingPongThreads = kConsumerThreads + 128;
+constexpr int kPingPongRegs = 232, kProducerRegs = 40;  // per thread: 2 * 232 + 40 <= 512 per sub-partition (one warp of each warpgroup)
+template <int NC, bool RES, bool MUL>
+__host__ __device__ constexpr int conv3_threads() { return conv3_pingpong<NC, RES, MUL>() ? kPingPongThreads : kUmmaThreads; }
+// edge-row exchange floats: edge0 + edge2, [8 row blocks][NC] each, one set per warpgroup (ping-pong) or one shared set
+template <int NC, bool RES, bool MUL>
+__host__ __device__ constexpr int conv3_edge_floats() { return (conv3_pingpong<NC, RES, MUL>() ? 2 : 1) * 2 * 8 * NC; }
+constexpr int kOrderBar = 3;  // ping-pong: named barriers 3 + wg, "warpgroup wg may issue its next tile" (kEpiBar + wg are its epilogue barriers)
+
+// Row block rb (0..7) of a tile holds rows 16 rb + g and 16 rb + g + 8 of a 64-row accumulator fragment: warp rb of the cooperative schedule,
+// warp rb % 4 of the owning warpgroup (acc[rb / 4]) in the ping-pong one.  conv3_edges publishes the block's rows that its neighbours need:
+// P_0 of its last row (edge0[rb]) and P_2 of its first row (edge2[rb]).
+template <int NC>
+__device__ __forceinline__ void conv3_edges(const float (&acc)[3 * NC / 2], int rb, int lane, float* edge0, float* edge2) {
+  constexpr int G = NC / 8;  // 8-column groups per dx
+  const int g = lane >> 2, cq = lane & 3;
+#pragma unroll
+  for (int i = 0; i < G; ++i) {
+    const int col = 8 * i + 2 * cq;
+    if (g == 7) *reinterpret_cast<float2*>(&edge0[rb * NC + col]) = make_float2(acc[4 * i + 2], acc[4 * i + 3]);
+    if (g == 0) *reinterpret_cast<float2*>(&edge2[rb * NC + col]) = make_float2(acc[4 * (2 * G + i)], acc[4 * (2 * G + i) + 1]);
+  }
+}
+
+// Row block rb: 3-tap combine, folded BatchNorm + activation (+ residual, * multiplier), bf16 hi/lo split into the staging planes [NC][112].
+template <int NC, int ACT, bool RES, bool MUL>
+__device__ __forceinline__ void conv3_epilogue(const float (&acc)[3 * NC / 2], int rb, int lane, const UmmaParams& p, const TileCoord& tc, const float* sc_s,
+                                               const float* sh_s, const float* edge0, const float* edge2, bf16* s_hi, bf16* s_lo) {
+  constexpr int G = NC / 8;
+  const int g = lane >> 2, cq = lane & 3;
+  const int mrow0 = 16 * rb + g;  // tile rows mrow0 and mrow0 + 8
+  const int n0 = tc.n_idx * NC;
+  // Tile row m = 16 * rb + g + 8h is output pixel f0 + m - 8 for m in [8, 120): block 0 stores only its h = 1 rows, block 7 only its h = 0 rows.
+  const bool row_out[2] = {rb != 0, rb != 7};
+  // residual / multiplier (B, Cout, T, F): element (n0 + col, row h) is at ro[h] + col * plane; pixels f >= F are staged unread (the store clips them)
+  const size_t plane = (size_t)p.T * p.F;
+  size_t ro[2];
+  bool f_in[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int f = tc.f0 + mrow0 + 8 * h - 8;
+    f_in[h] = f < p.F;
+    ro[h] = ((size_t)tc.b * p.Cout + n0) * plane + (size_t)tc.t * p.F + f;
+  }
+#pragma unroll
+  for (int i = 0; i < G; ++i) {
+    const int col0 = 8 * i + 2 * cq;
+    // the neighbouring blocks' edge rows of both columns: row 16 rb - 1 (P_0, read by g = 0) and row 16 rb + 16 (P_2, read by g = 7)
+    float2 prev = make_float2(0.f, 0.f), next = make_float2(0.f, 0.f);
+    if (g == 0 && rb > 0) prev = *reinterpret_cast<const float2*>(&edge0[(rb - 1) * NC + col0]);
+    if (g == 7 && rb < 7) next = *reinterpret_cast<const float2*>(&edge2[(rb + 1) * NC + col0]);
+    const float2 sc2 = *reinterpret_cast<const float2*>(&sc_s[n0 + col0]), sh2 = *reinterpret_cast<const float2*>(&sh_s[n0 + col0]);
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      const int col = col0 + e;
+      const float p0a = acc[4 * i + e], p0b = acc[4 * i + 2 + e];
+      const float p1a = acc[4 * (G + i) + e], p1b = acc[4 * (G + i) + 2 + e];
+      const float p2a = acc[4 * (2 * G + i) + e], p2b = acc[4 * (2 * G + i) + 2 + e];
+      const float up_a = __shfl_sync(0xffffffffu, p0a, (lane + 28) & 31), up_b = __shfl_sync(0xffffffffu, p0b, (lane + 28) & 31);
+      const float dn_a = __shfl_sync(0xffffffffu, p2a, (lane + 4) & 31), dn_b = __shfl_sync(0xffffffffu, p2b, (lane + 4) & 31);
+      float x[2];
+      x[0] = p1a + ((g > 0) ? up_a : (e ? prev.y : prev.x)) + ((g < 7) ? dn_a : dn_b);
+      x[1] = p1b + ((g > 0) ? up_b : up_a) + ((g < 7) ? dn_b : (e ? next.y : next.x));
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        if (!row_out[h]) continue;
+        const int m = mrow0 + 8 * h;
+        float y = act_c<ACT>(fmaf(x[h], e ? sc2.y : sc2.x, e ? sh2.y : sh2.x));
+        if constexpr (RES || MUL) {
+          if (f_in[h]) {
+            const size_t o = ro[h] + (size_t)col * plane;
+            if constexpr (RES) y += pair_at(p.res_hi, p.res_lo, o);
+            if constexpr (MUL) y *= pair_at(p.mul_hi, p.mul_lo, o);
+          }
+        }
+        split_store2(y, s_hi[col * kConvStride + (m - 8)], s_lo[col * kConvStride + (m - 8)]);
+      }
+    }
+  }
+}
+
 // The epilogue is fixed at compile time: ACT (0 none, 1 ReLU, 2 GELU), RES (+ residual), MUL (* multiplier).  umma_conv_run instantiates the
 // combinations the networks use (conv3_instance below).
 template <int NC, int ACT, bool RES, bool MUL>
-__global__ void __launch_bounds__(kUmmaThreads, 1) umma_conv3_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
+__global__ void __launch_bounds__(conv3_threads<NC, RES, MUL>(), 1) umma_conv3_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
                                                                      const __grid_constant__ CUtensorMap tmO_hi, const __grid_constant__ CUtensorMap tmO_lo,
                                                                      const UmmaParams p) {
+  constexpr bool kPingPong = conv3_pingpong<NC, RES, MUL>();
   constexpr int kPlane = NC * kConvStride;  // bf16 elements of one staged plane [NC][112]
-  constexpr int G = NC / 8;                 // 8-column groups per dx
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (ptx::smem_u32(smem_raw) & 1023u)) & 1023u);
   // [ring: stages x stage_bytes][resident weights, when b_resident][output staging hi | lo][barriers][BN coefficients][edge rows]
@@ -416,18 +527,20 @@ __global__ void __launch_bounds__(kUmmaThreads, 1) umma_conv3_kernel(const __gri
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(s_lo + kPlane);
   uint64_t* empty_bar = full_bar + p.stages;
   uint64_t* wres_bar = empty_bar + p.stages;
+  uint64_t* sfree_bar = wres_bar + 1;  // ping-pong: the staging planes have been read out by the latest store (one arrive per tile)
   float* sc_s = reinterpret_cast<float*>(wres_bar + 2);
   float* sh_s = sc_s + kMaxChannels;
-  float* edge0 = sh_s + kMaxChannels;  // [8 warps][NC]: P_0 of the warp's last row (row 16w + 15)
-  float* edge2 = edge0 + 8 * NC;       // [8 warps][NC]: P_2 of the warp's first row (row 16w)
+  float* edge0 = sh_s + kMaxChannels;  // [edge sets][8 row blocks][NC]: P_0 of the block's last row
+  float* edge2 = edge0 + conv3_edge_floats<NC, RES, MUL>() / 2;  // same layout: P_2 of the block's first row
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
     for (int s = 0; s < p.stages; ++s) {
       ptx::mbar_init(&full_bar[s], 1);
-      ptx::mbar_init(&empty_bar[s], kConsumerThreads);
+      ptx::mbar_init(&empty_bar[s], kPingPong ? kConsumerThreads / 2 : kConsumerThreads);  // a stage is read by one warpgroup, or by both
     }
     ptx::mbar_init(wres_bar, 1);
+    ptx::mbar_init(sfree_bar, 1);
     ptx::fence_barrier_init();
     ptx::prefetch_tensormap(&tmA_hi);
     ptx::prefetch_tensormap(&tmA_lo);
@@ -440,94 +553,94 @@ __global__ void __launch_bounds__(kUmmaThreads, 1) umma_conv3_kernel(const __gri
   }
   __syncthreads();
 
-  if (warp == kConsumerThreads / 32) {
-    if (lane == 0) umma_producer_loop(tmA_hi, tmA_lo, tmA_hi, tmA_lo, p, smem, full_bar, empty_bar, wres_bar);
+  if (warp >= kConsumerThreads / 32) {
+    if constexpr (kPingPong) ptx::setmaxnreg_dec<kProducerRegs>();
+    if (warp == kConsumerThreads / 32 && lane == 0) umma_producer_loop(tmA_hi, tmA_lo, tmA_hi, tmA_lo, p, smem, full_bar, empty_bar, wres_bar);
     return;
   }
-  const int wg = warp >> 2, g = lane >> 2, cq = lane & 3;
-  const int mrow0 = wg * 64 + (warp & 3) * 16 + g;  // tile rows mrow0 and mrow0 + 8
-  const bool issuer = threadIdx.x == 0;             // owns the bulk store groups
-  if (p.b_resident) ptx::mbar_wait(wres_bar, 0);  // the resident weight image has landed
+  if constexpr (kPingPong) ptx::setmaxnreg_inc<kPingPongRegs>();
+  const int wg = warp >> 2;
+  auto store_tile = [&](const TileCoord& tc) {  // the staged planes -> the output's channels [n0, n0 + NC), one bulk group
+    const int cc = tc.b * p.out_c_total + p.out_c_off + tc.n_idx * NC;
+    ptx::tma_store_3d(&tmO_hi, s_hi, tc.f0, tc.t, cc);
+    ptx::tma_store_3d(&tmO_lo, s_lo, tc.f0, tc.t, cc);
+    ptx::bulk_commit();
+  };
+  if (p.b_resident) {  // the resident weight image has landed
+    if constexpr (kPingPong) ptx::mbar_wait_spin(wres_bar, 0);
+    else ptx::mbar_wait(wres_bar, 0);
+  }
   int s = 0;
   uint32_t phase = 0;
-  float acc[3 * NC / 2];
-  for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-    const TileCoord tc = decode_tile(p, tile);
-    consumer_mainloop(p, smem, full_bar, empty_bar, s, phase, [&](uint32_t ah, uint32_t al, uint32_t bh, uint32_t bl, int j, int accum) {
-      const uint64_t dah = a_desc(p, ah, wg, j), dal = a_desc(p, al, wg, j), dbh = b_desc(p, bh, j), dbl = b_desc(p, bl, j);
-      conv3_mma<NC>(acc, dah, dbh, accum);
-      conv3_mma<NC>(acc, dah, dbl, 1);
-      conv3_mma<NC>(acc, dal, dbh, 1);
-    });
-    ptx::fence_regs(acc);
-    // boundary rows for the neighbouring warps
-#pragma unroll
-    for (int i = 0; i < G; ++i) {
-      const int col = 8 * i + 2 * cq;
-      if (g == 7) *reinterpret_cast<float2*>(&edge0[warp * NC + col]) = make_float2(acc[4 * i + 2], acc[4 * i + 3]);
-      if (g == 0) *reinterpret_cast<float2*>(&edge2[warp * NC + col]) = make_float2(acc[4 * (2 * G + i)], acc[4 * (2 * G + i) + 1]);
-    }
-    // the staging planes must have been read out by the previous tile's store
-    if (issuer) ptx::bulk_wait_read<0>();
-    asm volatile("bar.sync %0, %1;" ::"n"(kEpiBar), "n"(kConsumerThreads) : "memory");
-    const int n0 = tc.n_idx * NC;
-    // Tile row m = 16 * warp + g + 8h is output pixel f0 + m - 8 for m in [8, 120): warp 0 stores only its h = 1 rows, warp 7 only its h = 0 rows.
-    const bool row_out[2] = {warp != 0, warp != 7};
-    // residual / multiplier (B, Cout, T, F): element (n0 + col, row h) is at ro[h] + col * plane; pixels f >= F are staged unread (the store clips them)
-    const size_t plane = (size_t)p.T * p.F;
-    size_t ro[2];
-    bool f_in[2];
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int f = tc.f0 + mrow0 + 8 * h - 8;
-      f_in[h] = f < p.F;
-      ro[h] = ((size_t)tc.b * p.Cout + n0) * plane + (size_t)tc.t * p.F + f;
-    }
-#pragma unroll
-    for (int i = 0; i < G; ++i) {
-      const int col0 = 8 * i + 2 * cq;
-      // the neighbouring warps' edge rows of both columns: row 16w - 1 (P_0, read by g = 0) and row 16w + 16 (P_2, read by g = 7)
-      float2 prev = make_float2(0.f, 0.f), next = make_float2(0.f, 0.f);
-      if (g == 0 && warp > 0) prev = *reinterpret_cast<const float2*>(&edge0[(warp - 1) * NC + col0]);
-      if (g == 7 && warp < 7) next = *reinterpret_cast<const float2*>(&edge2[(warp + 1) * NC + col0]);
-      const float2 sc2 = *reinterpret_cast<const float2*>(&sc_s[n0 + col0]), sh2 = *reinterpret_cast<const float2*>(&sh_s[n0 + col0]);
-#pragma unroll
-      for (int e = 0; e < 2; ++e) {
-        const int col = col0 + e;
-        const float p0a = acc[4 * i + e], p0b = acc[4 * i + 2 + e];
-        const float p1a = acc[4 * (G + i) + e], p1b = acc[4 * (G + i) + 2 + e];
-        const float p2a = acc[4 * (2 * G + i) + e], p2b = acc[4 * (2 * G + i) + 2 + e];
-        const float up_a = __shfl_sync(0xffffffffu, p0a, (lane + 28) & 31), up_b = __shfl_sync(0xffffffffu, p0b, (lane + 28) & 31);
-        const float dn_a = __shfl_sync(0xffffffffu, p2a, (lane + 4) & 31), dn_b = __shfl_sync(0xffffffffu, p2b, (lane + 4) & 31);
-        float x[2];
-        x[0] = p1a + ((g > 0) ? up_a : (e ? prev.y : prev.x)) + ((g < 7) ? dn_a : dn_b);
-        x[1] = p1b + ((g > 0) ? up_b : up_a) + ((g < 7) ? dn_b : (e ? next.y : next.x));
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          if (!row_out[h]) continue;
-          const int m = mrow0 + 8 * h;
-          float y = act_c<ACT>(fmaf(x[h], e ? sc2.y : sc2.x, e ? sh2.y : sh2.x));
-          if constexpr (RES || MUL) {
-            if (f_in[h]) {
-              const size_t o = ro[h] + (size_t)col * plane;
-              if constexpr (RES) y += pair_at(p.res_hi, p.res_lo, o);
-              if constexpr (MUL) y *= pair_at(p.mul_hi, p.mul_lo, o);
-            }
-          }
-          split_store2(y, s_hi[col * kConvStride + (m - 8)], s_lo[col * kConvStride + (m - 8)]);
-        }
+  if constexpr (kPingPong) {
+    const int rb = warp & 3;                           // row blocks rb (acc[0]) and 4 + rb (acc[1])
+    const bool issuer = (threadIdx.x & 127) == 0;      // owns this warpgroup's bulk store groups
+    float* e0 = edge0 + wg * 8 * NC;
+    float* e2 = edge2 + wg * 8 * NC;
+    float acc[2][3 * NC / 2];
+    if (wg == 1) ring_skip(p, s, phase, p.num_iters);  // the ring stages of warpgroup 0's first tile
+    int k = wg;                                        // index of the tile in the CTA's walk
+    for (int tile = blockIdx.x + wg * gridDim.x; tile < p.num_tiles; tile += 2 * gridDim.x, k += 2) {
+      const TileCoord tc = decode_tile(p, tile);
+      const bool other_next = tile + (int)gridDim.x < p.num_tiles;  // the other warpgroup has the following tile
+      if (k > 0) ptx::bar_sync(kOrderBar + wg, kConsumerThreads);   // the other warpgroup has issued every MMA of the previous tile
+      consumer_mainloop<false>(
+          p, smem, full_bar, empty_bar, s, phase,
+          [&](uint32_t ah, uint32_t al, uint32_t bh, uint32_t bl, int j, int accum) {
+            const uint64_t dbh = b_desc(p, bh, j), dbl = b_desc(p, bl, j);
+            const uint64_t dah0 = a_desc(p, ah, 0, j), dal0 = a_desc(p, al, 0, j), dah1 = a_desc(p, ah, 1, j), dal1 = a_desc(p, al, 1, j);
+            conv3_mma<NC>(acc[0], dah0, dbh, accum);
+            conv3_mma<NC>(acc[0], dah0, dbl, 1);
+            conv3_mma<NC>(acc[0], dal0, dbh, 1);
+            conv3_mma<NC>(acc[1], dah1, dbh, accum);
+            conv3_mma<NC>(acc[1], dah1, dbl, 1);
+            conv3_mma<NC>(acc[1], dal1, dbh, 1);
+          },
+          [&] {
+            if (other_next) ptx::bar_arrive(kOrderBar + (wg ^ 1), kConsumerThreads);
+          });
+      ring_skip(p, s, phase, p.num_iters);  // the other warpgroup's tile
+      ptx::fence_regs(acc[0]);
+      ptx::fence_regs(acc[1]);
+      conv3_edges<NC>(acc[0], rb, lane, e0, e2);
+      conv3_edges<NC>(acc[1], 4 + rb, lane, e0, e2);
+      // the staging planes must have been read out by the previous tile's store (the other warpgroup's)
+      if (issuer && k > 0) ptx::mbar_wait_spin(sfree_bar, (uint32_t)(k - 1) & 1u);
+      ptx::bar_sync(kEpiBar + wg, kConsumerThreads / 2);
+      conv3_epilogue<NC, ACT, RES, MUL>(acc[0], rb, lane, p, tc, sc_s, sh_s, e0, e2, s_hi, s_lo);
+      conv3_epilogue<NC, ACT, RES, MUL>(acc[1], 4 + rb, lane, p, tc, sc_s, sh_s, e0, e2, s_hi, s_lo);
+      ptx::fence_proxy_async();
+      ptx::bar_sync(kEpiBar + wg, kConsumerThreads / 2);
+      if (issuer) {
+        store_tile(tc);
+        ptx::bulk_wait_read<0>();
+        ptx::mbar_arrive(sfree_bar);
       }
     }
-    ptx::fence_proxy_async();
-    asm volatile("bar.sync %0, %1;" ::"n"(kEpiBar), "n"(kConsumerThreads) : "memory");
-    if (issuer) {
-      const int cc = tc.b * p.out_c_total + p.out_c_off + n0;
-      ptx::tma_store_3d(&tmO_hi, s_hi, tc.f0, tc.t, cc);
-      ptx::tma_store_3d(&tmO_lo, s_lo, tc.f0, tc.t, cc);
-      ptx::bulk_commit();
+    if (issuer) ptx::bulk_wait_all();
+  } else {
+    const bool issuer = threadIdx.x == 0;  // owns the bulk store groups
+    float acc[3 * NC / 2];
+    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+      const TileCoord tc = decode_tile(p, tile);
+      consumer_mainloop(p, smem, full_bar, empty_bar, s, phase, [&](uint32_t ah, uint32_t al, uint32_t bh, uint32_t bl, int j, int accum) {
+        const uint64_t dah = a_desc(p, ah, wg, j), dal = a_desc(p, al, wg, j), dbh = b_desc(p, bh, j), dbl = b_desc(p, bl, j);
+        conv3_mma<NC>(acc, dah, dbh, accum);
+        conv3_mma<NC>(acc, dah, dbl, 1);
+        conv3_mma<NC>(acc, dal, dbh, 1);
+      });
+      ptx::fence_regs(acc);
+      conv3_edges<NC>(acc, warp, lane, edge0, edge2);
+      // the staging planes must have been read out by the previous tile's store
+      if (issuer) ptx::bulk_wait_read<0>();
+      ptx::bar_sync(kEpiBar, kConsumerThreads);
+      conv3_epilogue<NC, ACT, RES, MUL>(acc, warp, lane, p, tc, sc_s, sh_s, edge0, edge2, s_hi, s_lo);
+      ptx::fence_proxy_async();
+      ptx::bar_sync(kEpiBar, kConsumerThreads);
+      if (issuer) store_tile(tc);
     }
+    if (issuer) ptx::bulk_wait_all();
   }
-  if (issuer) ptx::bulk_wait_all();
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -583,10 +696,10 @@ static int num_sms() {
 }
 
 // Persistent launch: one CTA per SM.
-template <class Kernel, class... Args>
+template <int Threads = kUmmaThreads, class Kernel, class... Args>
 static int launch_persistent(Kernel kernel, int num_tiles, size_t smem, cudaStream_t st, Args... args) {
   const int grid = std::min(num_tiles, num_sms());
-  kernel<<<grid, kUmmaThreads, smem, st>>>(args...);
+  kernel<<<grid, Threads, smem, st>>>(args...);
   B2_LAUNCHED();
   return B200SEP_OK;
 }
@@ -836,26 +949,44 @@ static int store_map(const void* base, int F, int T, int C, int box_c, CUtensorM
   return B200SEP_OK;
 }
 
+// Shared memory of a 3x3 launch: [ring][resident weights][output staging][barriers, BN coefficients, edge rows of edge_floats]; as many ring
+// stages as fit next to the rest, up to 8.
+static int conv3_layout(UmmaParams& p, size_t edge_floats, size_t* smem) {
+  const size_t b_all = p.b_resident ? (size_t)2 * p.b_bytes * p.num_iters : 0;
+  const size_t sbuf_bytes = (size_t)2 * p.n_c * kConvStride * 2;  // staged output: hi + lo planes [n_c][112] bf16
+  const size_t fixed = 1024 /*alignment slack*/ + 64 * sizeof(uint64_t) + 64 + 2 * kMaxChannels * sizeof(float) + edge_floats * sizeof(float) + b_all;
+  const size_t budget = 227 * 1024 - fixed;
+  int stages = (int)((budget - sbuf_bytes) / p.stage_bytes);
+  if (stages > 8) stages = 8;
+  B2_CHECK_ARG(stages >= 2, "umma_conv: a pipeline stage of %u bytes does not fit twice in shared memory", p.stage_bytes);
+  p.stages = stages;
+  p.b_res_off = (uint32_t)((size_t)stages * p.stage_bytes);
+  *smem = (size_t)stages * p.stage_bytes + sbuf_bytes + fixed;
+  return B200SEP_OK;
+}
+
 template <int NC, int ACT, bool RES, bool MUL>
-static int launch_conv3(const CUtensorMap& a_hi, const CUtensorMap& a_lo, const CUtensorMap& o_hi, const CUtensorMap& o_lo, UmmaParams& p, size_t smem, cudaStream_t st) {
+static int launch_conv3(const CUtensorMap& a_hi, const CUtensorMap& a_lo, const CUtensorMap& o_hi, const CUtensorMap& o_lo, UmmaParams& p, cudaStream_t st) {
+  size_t smem = 0;
+  int rc = conv3_layout(p, conv3_edge_floats<NC, RES, MUL>(), &smem);
+  if (rc) return rc;
   static bool attr_set[kMaxDevices] = {};
   B2_DEVICE_SLOT(dev);
   if (!attr_set[dev]) {
     B2_CUDA(cudaFuncSetAttribute(umma_conv3_kernel<NC, ACT, RES, MUL>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     attr_set[dev] = true;
   }
-  return launch_persistent(umma_conv3_kernel<NC, ACT, RES, MUL>, p.num_tiles, smem, st, a_hi, a_lo, o_hi, o_lo, p);
+  return launch_persistent<conv3_threads<NC, RES, MUL>()>(umma_conv3_kernel<NC, ACT, RES, MUL>, p.num_tiles, smem, st, a_hi, a_lo, o_hi, o_lo, p);
 }
 
 // The epilogue variants with a kernel instance: MDX-Net's BN + ReLU; MDX23C's TFC convolutions (plain, + residual, + residual * multiplier).
 template <int NC>
-static int conv3_instance(const CUtensorMap& a_hi, const CUtensorMap& a_lo, const CUtensorMap& o_hi, const CUtensorMap& o_lo, UmmaParams& p, size_t smem,
-                          cudaStream_t st) {
+static int conv3_instance(const CUtensorMap& a_hi, const CUtensorMap& a_lo, const CUtensorMap& o_hi, const CUtensorMap& o_lo, UmmaParams& p, cudaStream_t st) {
   const bool res = p.res_hi != nullptr, mul = p.mul_hi != nullptr;
-  if (p.act == 1 && !res && !mul) return launch_conv3<NC, 1, false, false>(a_hi, a_lo, o_hi, o_lo, p, smem, st);
-  if (p.act == 0 && !res && !mul) return launch_conv3<NC, 0, false, false>(a_hi, a_lo, o_hi, o_lo, p, smem, st);
-  if (p.act == 0 && res && !mul) return launch_conv3<NC, 0, true, false>(a_hi, a_lo, o_hi, o_lo, p, smem, st);
-  if (p.act == 0 && res && mul) return launch_conv3<NC, 0, true, true>(a_hi, a_lo, o_hi, o_lo, p, smem, st);
+  if (p.act == 1 && !res && !mul) return launch_conv3<NC, 1, false, false>(a_hi, a_lo, o_hi, o_lo, p, st);
+  if (p.act == 0 && !res && !mul) return launch_conv3<NC, 0, false, false>(a_hi, a_lo, o_hi, o_lo, p, st);
+  if (p.act == 0 && res && !mul) return launch_conv3<NC, 0, true, false>(a_hi, a_lo, o_hi, o_lo, p, st);
+  if (p.act == 0 && res && mul) return launch_conv3<NC, 0, true, true>(a_hi, a_lo, o_hi, o_lo, p, st);
   set_error("umma_conv: no 3x3 kernel instance for the epilogue act=%d residual=%d multiplier=%d", p.act, (int)res, (int)mul);
   return B200SEP_ERR_ARG;
 }
@@ -874,26 +1005,16 @@ int umma_conv_run(const UmmaConvPlan& pl, const void* wb_hi, const void* wb_lo, 
   p.t_tiles = pl.T;
   p.num_tiles = p.n_ftiles * pl.T * B * p.n_tiles;
   B2_CHECK_ARG(n_c % 16 == 0 && n_c <= 80, "umma_conv: n_c=%d is not a multiple of 16 up to 80", n_c);
-  const size_t sbuf_bytes = (size_t)2 * n_c * kConvStride * 2;  // staged output: hi + lo planes [n_c][112] bf16
-  const size_t fixed = 1024 /*alignment slack*/ + 64 * sizeof(uint64_t) + 64 + 2 * kMaxChannels * sizeof(float) + (size_t)16 * n_c * sizeof(float) +
-                       (p.b_resident ? b_all : 0);
-  const size_t budget = 227 * 1024 - fixed;
-  int stages = (int)((budget - sbuf_bytes) / p.stage_bytes);
-  if (stages > 8) stages = 8;
-  B2_CHECK_ARG(stages >= 2, "umma_conv: a pipeline stage of %u bytes does not fit twice in shared memory", p.stage_bytes);
-  p.stages = stages;
-  p.b_res_off = (uint32_t)((size_t)stages * p.stage_bytes);
-  const size_t smem = (size_t)stages * p.stage_bytes + sbuf_bytes + fixed;
   CUtensorMap o_hi, o_lo;
   int rc = store_map(p.out_hi, pl.F, pl.T, B * p.out_c_total, n_c, &o_hi);
   if (!rc) rc = store_map(p.out_lo, pl.F, pl.T, B * p.out_c_total, n_c, &o_lo);
   if (rc) return rc;
   switch (n_c) {
-    case 16: return conv3_instance<16>(pl.a_hi, pl.a_lo, o_hi, o_lo, p, smem, st);
-    case 32: return conv3_instance<32>(pl.a_hi, pl.a_lo, o_hi, o_lo, p, smem, st);
-    case 48: return conv3_instance<48>(pl.a_hi, pl.a_lo, o_hi, o_lo, p, smem, st);
-    case 64: return conv3_instance<64>(pl.a_hi, pl.a_lo, o_hi, o_lo, p, smem, st);
-    case 80: return conv3_instance<80>(pl.a_hi, pl.a_lo, o_hi, o_lo, p, smem, st);
+    case 16: return conv3_instance<16>(pl.a_hi, pl.a_lo, o_hi, o_lo, p, st);
+    case 32: return conv3_instance<32>(pl.a_hi, pl.a_lo, o_hi, o_lo, p, st);
+    case 48: return conv3_instance<48>(pl.a_hi, pl.a_lo, o_hi, o_lo, p, st);
+    case 64: return conv3_instance<64>(pl.a_hi, pl.a_lo, o_hi, o_lo, p, st);
+    case 80: return conv3_instance<80>(pl.a_hi, pl.a_lo, o_hi, o_lo, p, st);
   }
   set_error("umma_conv: n_c=%d has no kernel instance", n_c);
   return B200SEP_ERR_ARG;
